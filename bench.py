@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """Benchmark of the dense-BA update hot path (BASELINE.json metric: "BA-update iters/sec (512 edges, 344x64x48) at
-1/2/4/8 B200; corr HBM GB/s vs peak").
+1/2/4/8 GPUs; corr HBM GB/s vs peak").
 
 One STEP = the droid_backends work of one FactorGraph.update (SURVEY.md section 8d): a 4-level radius-3
 corr_index_forward over all edges + ba(iterations=2, lm=1e-4, ep=0.1) on a synthetic 512-edge / 72-keyframe graph at
 48x64 (fp16 correlation volumes as in the live system).
 
-    python bench.py [--gpus N --steps K --warmup W] [--impl reference]
+    python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--dump-outputs DIR]
 
 * our arm: `value` times the step with all inputs resident in HBM, launched through the C ABI (ctypes); `e2e` goes
   through the pybind `droid_backends` API from pinned HOST buffers (per-step inputs H2D, BA results D2H inside the timed
@@ -15,10 +15,13 @@ corr_index_forward over all edges + ba(iterations=2, lm=1e-4, ep=0.1) on a synth
 * N > 1 (torchrun, one rank per GPU): weak scaling in edges -- the graph has 512*N edges over the same 72-keyframe
   window, sharded by source frame (droid_slam_b200/sharded.py); one NCCL all-reduce of the reduced pose system per
   Gauss-Newton iteration; `value` = 512-edge-equivalents per second = N / step time (max over ranks).
-* --impl reference: the UNMODIFIED reference CUDA kernels (oracle/_ref/droid_backends_ref: /root/reference/src built for
-  sm_100a against the dense-LLT Eigen stand-in) on the same tensors, same protocol; corr_index is issued in chunks of
+* --impl reference: the UNMODIFIED reference CUDA kernels (oracle/_ref/droid_backends_ref: the reference's src/ built for
+  sm_90a against the dense-LLT Eigen stand-in) on the same tensors, same protocol; corr_index is issued in chunks of
   128 edges because the reference's 32-bit accessors cannot address a 512-edge level-0 volume.  Falls back to the CPU
   oracle port when that build is absent.  Rank 0 only.
+* --dump-outputs DIR (our arm): after the timed steps, rank 0 writes what the last timed step computed as DIR/<name>.npy
+  (float32): the updated poses and inverse depths, and the 196-channel lookup of a fixed seeded subset of edges.  The inputs
+  are generated from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes
@@ -50,9 +53,10 @@ CONFIGS = {
     "c2": dict(edges=128, frames=25, ht=48, wd=64, dtype="f32", itrs=2, lm=1e-4, ep=0.1, scaling="weak", corr=True, stereo=False),
     "c3": dict(edges=2048, frames=400, ht=48, wd=64, dtype="f16", itrs=10, lm=1e-5, ep=1e-2, scaling="strong", corr=False, stereo=False),
     "c4": dict(edges=256, frames=64, ht=48, wd=64, dtype="f16", itrs=2, lm=1e-4, ep=0.1, scaling="weak", corr=True, stereo=True),
-    "c5": dict(edges=8192, frames=1000, ht=72, wd=96, dtype="bf16", itrs=2, lm=1e-4, ep=0.1, scaling="strong", corr=True, stereo=False),
-    # one rank's share of c5 on ONE GPU (1024 edges = 130 GB of bf16 volumes, 125 keyframes): the single-GPU proxy of the stress config
-    "c5_rank": dict(edges=1024, frames=125, ht=72, wd=96, dtype="bf16", itrs=2, lm=1e-4, ep=0.1, scaling="strong", corr=True, stereo=False),
+    # stress: 512 edges per GPU at 8 GPUs (512 x 127 MB = 65 GB of bf16 volumes per 80 GB GPU)
+    "c5": dict(edges=4096, frames=500, ht=72, wd=96, dtype="bf16", itrs=2, lm=1e-4, ep=0.1, scaling="strong", corr=True, stereo=False),
+    # one rank's share of c5 on ONE GPU (512 edges = 65 GB of bf16 volumes, 63 keyframes): the single-GPU proxy of the stress config
+    "c5_rank": dict(edges=512, frames=63, ht=72, wd=96, dtype="bf16", itrs=2, lm=1e-4, ep=0.1, scaling="strong", corr=True, stereo=False),
 }
 
 
@@ -80,6 +84,7 @@ def parse():
     ap.add_argument("--no-graph", action="store_true", help="launch the step eagerly instead of replaying a captured CUDA graph (N=1)")
     ap.add_argument("--dropin-lookup", action="store_true", help="time the step with the four drop-in corr_index_forward launches on reference-layout volumes (round-1 definition) instead of the fused one-launch lookup on tiled volumes")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary kernels (update operator, volume build, altcorr, geometry, solve) timed for `rooflines`")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     select_config(args)
     if args.steps is None:
@@ -89,7 +94,7 @@ def parse():
 
 # ---------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region"""
 
     def __init__(self, index):
         self.index = index; self.proc = None; self.lines = []
@@ -137,18 +142,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def roofline_traffic():
-    """dram bytes per step of the corr_index kernels from the committed ncu capture (profiles/), or None"""
-    p = os.path.join(ROOT, "profiles", "corr_index_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -189,6 +183,21 @@ def build_problem(args, rank, world, dev):
 def alg_bytes_corr(E, dtype):
     s = 4 if dtype == torch.float32 else 2
     return E * HT * WD * (LEVELS * ((2 * RADIUS + 2) ** 2 + (2 * RADIUS + 1) ** 2) * s + LEVELS * 8)     # SURVEY 8d: HW*(452 s + 32)
+
+
+def dump_outputs(out_dir, poses, disps, corr):
+    """the arrays the timed step hands its caller: poses [N,7] and inverse depths [N,ht,wd] after the BA update and, for configs
+    with correlation volumes, the lookup [E,196,ht,wd] of a fixed seeded subset of at most 16 edges (at most ~48 MB), all float32"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "poses.npy"), poses.float().cpu().numpy())
+    np.save(os.path.join(out_dir, "disps.npy"), disps.float().cpu().numpy())
+    if corr is not None:
+        E = corr.shape[0]
+        k = max(1, min(16, E, int(48e6 // (corr[0].numel() * 4))))
+        sel = torch.randperm(E, generator=torch.Generator().manual_seed(0))[:k].sort().values
+        np.save(os.path.join(out_dir, "corr_lookup_edges.npy"), corr[sel.to(corr.device)].float().cpu().numpy())
+        np.save(os.path.join(out_dir, "corr_lookup_edge_ids.npy"), sel.double().numpy())
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -312,6 +321,9 @@ def run_ours(args, rank, world, dev):
     barrier()
     clocks = sampler.stop()
     ms_total = t_beg.elapsed_time(t_end)
+    if args.dump_outputs and rank == 0:
+        corr = corr196 if FUSED else (torch.cat([c.view(E, 49, HT, WD) for c in corr_out], 1) if NL else None)
+        dump_outputs(args.dump_outputs, d["poses"], d["disps"], corr)
     # the dominant kernel on its own stream position: the four corr_index launches of a step, CUDA events around them
     evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
     for k in range(args.steps):
@@ -431,7 +443,6 @@ def run_ours(args, rank, world, dev):
     peak, peak_src = measured_peak()
     alg = alg_bytes_corr(E, dtype)
     achieved = alg / (corr_ms * 1e-3) / 1e9 if (WITH_CORR and corr_ms > 0) else 0.0
-    traffic = roofline_traffic()
     launches_per_step = (1 if FUSED else NL) + 2 + BA_ITERS * 6        # corr x4, prepare+csr, per GN iter: build, schur x2, chol, backsub, pose_retr
     Ptot = pb["t1"] - pb["t0"]
     sys_bytes = 8 * (36 * Ptot * Ptot + 6 * Ptot)
@@ -468,9 +479,7 @@ def run_ours(args, rank, world, dev):
         kname = "corr_lookup_pyramid_f16_kernel<tiled levels 0-1> (1 launch/step: all 4 levels)" if FUSED else "corr_index_fwd_%s_r3_kernel (4 launches/step)" % args.dtype
         line["roofline"] = {"kernel": kname, "bound": "hbm", "achieved": achieved, "peak": peak,
                             "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src, "algorithmic_bytes_per_step": alg,
-                            "kernel_ms_per_step": corr_ms, "share_of_step": corr_ms / ms_step,
-                            "traffic": (traffic or {}).get("dram_bytes_per_step_" + ("fused_tiled_f16" if FUSED else args.dtype)),
-                            "traffic_source": "ncu dram__bytes_read.sum + dram__bytes_write.sum of the four launches, profiles/ (captured once per kernel change, not re-measured by this run)"}
+                            "kernel_ms_per_step": corr_ms, "share_of_step": corr_ms / ms_step}
     else:
         alg_ba = BA_ITERS * (16 * E * HT * WD + 16 * pb["M"] * HT * WD + 28 * FRAMES)
         line["roofline"] = {"kernel": "ba (build + Schur + solve + back-substitution per GN iteration)", "bound": "hbm", "achieved": alg_ba / ((ms_step - corr_ms) * 1e-3) / 1e9,
@@ -481,7 +490,7 @@ def run_ours(args, rank, world, dev):
         line["dropin_lookup"] = {"kernel": "corr_index_fwd_f16_r3_kernel (4 launches on reference-layout volumes, the round-1 step)", "kernel_ms_per_step": dropin_ms,
                                  "achieved": alg / (dropin_ms * 1e-3) / 1e9, "frac": alg / (dropin_ms * 1e-3) / 1e9 / peak, "unit": "GB/s",
                                  "step_ms_with_dropin_lookup": ms_step - corr_ms + dropin_ms, "value_with_dropin_lookup": mult * 1e3 / (ms_step - corr_ms + dropin_ms),
-                                 "traffic": (traffic or {}).get("dram_bytes_per_step_" + args.dtype), "outputs": "bit-identical to the fused lookup (checked in this run)"}
+                                 "outputs": "bit-identical to the fused lookup (checked in this run)"}
     if world == 1 and not args.no_extras:
         extras = secondary_kernels(E, dev, ms_step, L, be, cpu_legs=not args.no_cpu_baseline)
         line["update_operator"] = extras.pop("update_operator")
@@ -505,7 +514,7 @@ def _time_ms(fn, iters=5, warm=2):
 
 def secondary_kernels(E, dev, ms_step, L, be, cpu_legs=True):
     """The other kernels of the path, each timed on its own with CUDA events (not part of `value`): the update operator (row A6,
-    tcgen05 convolutions), the correlation-volume build (A7), altcorr (A2), the streaming geometry ops (A8-A11) and the fp64 solve.
+    wgmma convolutions), the correlation-volume build (A7), altcorr (A2), the streaming geometry ops (A8-A11) and the fp64 solve.
     Each entry carries its algorithmic work (SURVEY 8d) and the roofline it is held against.  Failures are reported, never raised."""
     out = {"update_operator": None, "rooflines": []}
     peaks = {}
@@ -513,9 +522,9 @@ def secondary_kernels(E, dev, ms_step, L, be, cpu_legs=True):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
-    tf_burst, tf_sust = float(peaks.get("bf16_tflops", 1590.0)), float(peaks.get("bf16_tflops_sustained", 1400.0))
-    src = "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md)"
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
+    tf_burst, tf_sust = float(peaks.get("bf16_tflops", 989.0)), float(peaks.get("bf16_tflops_sustained", 989.0))
+    src = "MEASURED_PEAKS.json" if peaks else "fallback (H100 SXM data sheet)"
     from droid_slam_b200 import synth
     g = torch.Generator(device=dev).manual_seed(7)
     # ---- update operator: same E edges as the step, 72 source frames
@@ -532,7 +541,7 @@ def secondary_kernels(E, dev, ms_step, L, be, cpu_legs=True):
             ms = _time_ms(lambda: mod(net, inp, corr, motn, ii))
         flops = (14.03e9 * E + 1.37e9 * min(E, FRAMES)) * (HT * WD / 3072.0)              # SURVEY 8d
         out["update_operator"] = {"ms": ms, "full_update_ms": ms + ms_step, "edges": E, "tflops": flops / ms / 1e9,
-                                  "impl": "droid_slam_b200.UpdateModule: tcgen05 implicit-GEMM convolutions (csrc/update_op.cu), reference-layout (NCHW) inputs, f16 operands / fp32 accumulation; "
+                                  "impl": "droid_slam_b200.UpdateModule: wgmma implicit-GEMM convolutions (csrc/update_op.cu), reference-layout (NCHW) inputs, f16 operands / fp32 accumulation; "
                                           "not part of `value`; the reference formula through torch/cuDNN is timed by --impl reference"}
         out["rooflines"].append({"kernel": "update operator (conv_tc_kernel x12 + layout / aggregation kernels)", "bound": "tensor", "achieved": flops / ms / 1e9, "peak": tf_sust, "unit": "TFLOP/s",
                                  "frac": flops / ms / 1e9 / tf_sust, "peak_source": src + " bf16_tflops_sustained (a 10+ ms tensor-bound kernel sequence runs under the power cap)", "ms": ms,
@@ -605,7 +614,7 @@ def secondary_kernels(E, dev, ms_step, L, be, cpu_legs=True):
         fl = n ** 3 / 3.0
         kname = "chol_resident_kernel" if n <= 448 and os.environ.get("DBA_CHOL_RESIDENT", "1") != "0" else "chol_cluster_kernel"
         out["rooflines"].append({"kernel": "%s (n = %d, fp64)" % (kname, n), "bound": "fp64 issue rate", "achieved": fl / ms / 1e9, "peak": 34.0, "unit": "TFLOP/s", "frac": fl / ms / 1e9 / 34.0,
-                                 "peak_source": "measured fp64 FMA issue rate (profiles/r1_fp64_issue_rate.txt)", "ms": ms, "algorithmic_flops": fl,
+                                 "peak_source": "H100 SXM data sheet fp64 (non-tensor)", "ms": ms, "algorithmic_flops": fl,
                                  "note": "latency bound: a chain of n/32 dependent column steps (potrf -> substitution -> update), the figure of merit is the time"})
     except Exception as e:
         out["rooflines"].append({"kernel": "chol_cluster_kernel", "error": str(e)[:200]})
@@ -731,7 +740,7 @@ def run_reference(args, rank, world, dev):
         "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True, "scaling": SCALING, "vs_baseline": None,
         "dtype": "f32 (CPU solve in f64), %s corr volumes" % args.dtype, "data": "synthetic", "impl": "reference", "update_operator": upd,
         "config": {"workload": "%s: %d edges over a %d-keyframe window at %dx%d, %s + ba(itrs=%d, lm=%g, ep=%g)" % (CFG_NAME, E, FRAMES, HT, WD, ("4-level r=3 corr_index_forward (chunks of %d edges: 32-bit accessors)" % CH) if WITH_CORR else "no lookup", BA_ITERS, LM, EP), "name": CFG_NAME,
-                   "implementation": "unmodified /root/reference/src/*.cu + droid.cpp built for sm_100a (oracle/build_ref.sh); CPU solve = dense fp64 LLT stand-in for Eigen::SimplicialLLT",
+                   "implementation": "unmodified reference src/*.cu + droid.cpp built for sm_90a (oracle/build_ref.sh); CPU solve = dense fp64 LLT stand-in for Eigen::SimplicialLLT",
                    "cpu_solve_ms_per_step": solve_ms, "ms_per_step_without_cpu_solve": ms_step - solve_ms},
         "e2e": {"value": 1e3 / e2e_ms, "unit": unit, "ms_per_step": e2e_ms, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "cpu_baseline": {"value": 1e3 / ms_step, "unit": "iters/s", "cores": os.cpu_count(), "kind": "reference",

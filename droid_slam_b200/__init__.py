@@ -1,7 +1,7 @@
-"""B200-native (sm_100a) dense-BA update hot path of DROID-SLAM behind the reference's `droid_backends` API.
+"""H100-native (sm_90a) dense-BA update hot path of DROID-SLAM behind the reference's `droid_backends` API.
 
     import droid_slam_b200
-    droid_slam_b200.install()        # makes `import droid_backends` resolve to the B200-native extension
+    droid_slam_b200.install()        # makes `import droid_backends` resolve to the native extension
     import droid_backends            # same nine callables as princeton-vl/DROID-SLAM src/droid.cpp:246-259
 
 There is no CPU or PyTorch fallback: if the native extension has not been built (`python -m droid_slam_b200.build`)
@@ -25,7 +25,7 @@ def install():
         sys.path.insert(0, EXT_DIR)
     mod = importlib.import_module("droid_backends")
     if not getattr(mod, "_b200_native", lambda: False)():
-        raise ImportError("a different `droid_backends` module shadows the B200-native one: %r" % (mod,))
+        raise ImportError("a different `droid_backends` module shadows the native one: %r" % (mod,))
     return mod
 
 

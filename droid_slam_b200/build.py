@@ -1,6 +1,6 @@
 """In-tree build of the native code (no JIT cache: the built .so files travel with the repo snapshot).
 
-  lib/libdroid_b200.so                          C-ABI library, hand-written CUDA for sm_100a (nvcc, no torch headers)
+  lib/libdroid_b200.so                          C-ABI library, hand-written CUDA for sm_90a (nvcc, no torch headers)
   _ext/droid_backends.cpython-*.so              pybind11/torch binding exporting the reference's `droid_backends` API
 
 `python -m droid_slam_b200.build` (or `__graft_entry__.build()`) rebuilds what is stale.
@@ -21,7 +21,7 @@ INCLUDE = os.path.join(os.path.dirname(PKG), "include")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.environ.get("NVCC", os.path.join(CUDA_HOME, "bin", "nvcc"))
 CUDA_SOURCES = ["common.cu", "corr_index.cu", "altcorr.cu", "geom.cu", "ba.cu", "chol.cu", "corr_volume.cu", "update_op.cu", "proximity.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-diag-suppress", "177"]
 
 LIB_PATH = os.path.join(LIBDIR, "libdroid_b200.so")
@@ -61,7 +61,7 @@ def build_library(verbose=False):
                 if verbose and out.strip():
                     print(out)
     if jobs or _newer(LIB_PATH, objs):
-        _run([NVCC, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"])
+        _run([NVCC, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"])
     return LIB_PATH
 
 

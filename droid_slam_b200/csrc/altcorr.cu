@@ -1,4 +1,4 @@
-// altcorr_forward / altcorr_backward for sm_100a (on-the-fly correlation, no stored volume).
+// altcorr_forward / altcorr_backward for sm_90a (on-the-fly correlation, no stored volume).
 //
 // Replaces reference src/altcorr_kernel.cu:24-225.  Forward semantics (oracle/corr.py::altcorr_forward):
 //   raw[b,m,a,c,y,x] = sum_ch T(f1[b,ii[m],ch,y,x]/4) * T(f2[b,jj[m],ch,floor(y0)+a-r,floor(x0)+c-r]/4)   (fp32 accumulation,

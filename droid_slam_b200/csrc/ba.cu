@@ -1,4 +1,4 @@
-// Dense bundle adjustment (Gauss-Newton, Schur complement over per-pixel inverse depth) for sm_100a.
+// Dense bundle adjustment (Gauss-Newton, Schur complement over per-pixel inverse depth) for sm_90a.
 //
 // Replaces reference src/droid_kernels.cu:185-433 (K1), :863-1124 (accum / retraction / Schur kernels),
 // :1126-1320 (CPU SparseBlock + schur_block) and the driver :1323-1443.  Same maths, different machine mapping:
@@ -19,7 +19,7 @@
 //   * back-substitution dz = Q (w - E^T dx) keeps the reference quirk Q9 (rows whose pose index is <= 0 are skipped,
 //     src/droid_kernels.cu:1114), then retraction of poses (left-multiplicative Exp, no renormalisation) and disps.
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include <math.h>
 #include <algorithm>
 
@@ -801,30 +801,28 @@ __global__ void __launch_bounds__(kSgThreads, 2) ba_schur_small_kernel(
 //   S[:6R, 6R] = sum E q w  -- one symmetric rank-K update per frame, K = pixels.
 // fp32 accuracy on the tf32 pipe by operand splitting (3xTF32): x = hi + lo with hi = tf32(x), lo = x - hi (exact), and
 //   S = hi hi^T + G + G^T,  G = hi lo^T   (the dropped lo lo^T term is ~2^-22 relative),
-// i.e. TWO tcgen05.mma per 8-pixel K step: G is accumulated once and symmetrised in the epilogue.
-// The tensor core truncates every addend to the accumulator's exponent, so a long accumulation chain drifts (measured: one
-// accumulator over the whole pixel range -> 1e-4 on the depths).  hi hi^T therefore gets a fresh TMEM accumulator per chunk
-// (three 128-column slots in rotation) which the producer warps drain into fp32 registers two chunks later; G is 2^-11 smaller
-// and keeps one accumulator for the whole range.
-// CTA = (frame, pixel range), 288 threads.  Warps 0-7: cp.async their own raw rows of a chunk into a 4-deep warp-private raw ring,
-// split them into the two K-major SWIZZLE_128B operand tiles [128 rows x 32 px] of a 4-deep operand ring (generic-proxy stores +
-// fence.proxy.async), drain accumulators, and finally add the lower triangle into the reduced system with fp64 atomics.
-// Warp 8: one thread issues the MMAs (M = 128, both operands described from the SAME tile) and commits to the mbarriers.
+// i.e. TWO wgmma per 8-pixel K step: G is accumulated once and symmetrised in the epilogue.
+// The tensor core truncates every addend to the accumulator's exponent, so a long accumulation chain drifts (one accumulator over
+// the whole pixel range -> 1e-4 on the depths).  hi hi^T therefore gets a fresh register accumulator per chunk which is added into
+// an fp32 running sum when the next chunk's MMAs are issued; G is 2^-11 smaller and keeps one accumulator for the whole range.
+// CTA = (frame, pixel range), 256 threads = two warpgroups.  Every warp cp.asyncs its own raw rows of a chunk into a 4-deep
+// warp-private raw ring and splits them into the two K-major SWIZZLE_128B operand tiles [128 rows x 32 px] of a 4-deep operand
+// ring (generic-proxy stores + fence.proxy.async); after a CTA barrier warpgroup w issues the chunk's wgmma.m64n128k8 for operand
+// rows 64 w .. 64 w + 63 against all 128 rows (both operands described from the SAME tile) and splits the next chunk while they
+// run.  Finally G goes through shared memory and the lower triangle is added into the reduced system with fp64 atomics.
 // Frames with 6R + 2 <= 64 (R <= 10) run "packed": the two halves of a 64-pixel chunk sit in operand rows 0..63 and 64..127,
-// one M = N = 128 MMA then yields both halves' products on the diagonal blocks (the MMA cost is set by the 128 operand rows
-// it streams whether they are live or not), and the epilogue adds the two blocks.
+// one M = N = 128 product then yields both halves' products on the diagonal blocks (the MMA cost is set by the 128 operand rows
+// it streams whether they are live or not).
 // ---------------------------------------------------------------------------------------------------------
 constexpr int kTcRowsMax = 21;
 constexpr int kPairTileRows = 10;               // pair mode: row tiles of 10 frame rows (60 lines + the w line <= 64 operand rows)
 constexpr int kPairRowsMax = 100;               // pair mode handles 22..100 rows (up to 45 tile pairs over gridDim.z); more rows: SIMT kernel
 constexpr int kPairGridZ = 45;
-constexpr int kTcThreads = 288;
-constexpr int kTcProducers = 256;
+constexpr int kTcThreads = 256;
 constexpr int kTcRawStages = 4;
 constexpr int kTcRawBytes = 128 * 128;          // up to 128 lines (6R rows, w, C; two halves when packed) x 128 bytes
 constexpr int kTcOpBytes = 128 * 128;           // one operand tile (hi or lo)
 constexpr int kTcOpStages = 4;
-constexpr int kTcAccSlots = 3;                  // rotating TMEM accumulators (128 columns each) for hi hi^T; G lives in columns 384..511
 constexpr int kTcCxStride = 129;                // floats per row of the G staging matrix (conflict-free transposed reads)
 constexpr int kTcSmem = kTcRawStages * kTcRawBytes + kTcOpStages * 2 * kTcOpBytes + 1024 /*alignment*/ + 256 /*barriers*/;
 static_assert(128 * kTcCxStride * 4 <= kTcOpStages * 2 * kTcOpBytes, "G staging matrix must fit the operand ring");
@@ -910,18 +908,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   const int nhalf = packed ? 2 : 1;
   const int cpx = 32 * nhalf;                            // pixels per chunk
   const int nchunks = (px_end - px_begin + cpx - 1) / cpx;
-  const int N = two_halves ? 128 : ((R6 + 1 + 15) & ~15);    // MMA N
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t op_base = smem_u32(smem);               // [stage][hi|lo][128 rows][128 B], 1024-byte aligned tiles
   const uint32_t raw_base = op_base + kTcOpStages * 2 * kTcOpBytes;   // [stage][row][128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kTcOpStages * 2 * kTcOpBytes + kTcRawStages * kTcRawBytes);
-  uint64_t* full = bars;                                 // [4] operand stage written (8 producer warps arrive)
-  uint64_t* empty = bars + kTcOpStages;                  // [4] operand stage consumed (tcgen05.commit)
-  uint64_t* acc_full = bars + 2 * kTcOpStages;           // [3] accumulator slot holds one chunk's hi hi^T (tcgen05.commit)
-  uint64_t* acc_empty = acc_full + kTcAccSlots;          // [3] slot drained into registers (8 warps arrive)
-  uint64_t* done = acc_empty + kTcAccSlots;              // every MMA has completed
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(done + 2);
 
   if (tid < 128) {
     if (PAIR) {                                          // operand row -> index in the reduced system, per half
@@ -929,257 +919,199 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
       s_gidx[tid] = (ln < R6x) ? s_pose[row0 + ln / 6] * 6 + (ln % 6) : (ln == R6x ? -1 : -2);
     } else s_gidx[tid] = (tid < R6) ? s_pose[tid / 6] * 6 + (tid % 6) : (tid == R6 ? -1 : -2);
   }
-  if (tid == 0) {
-    for (int s = 0; s < kTcOpStages; s++) { mbar_init(full + s, kTcProducers / 32); mbar_init(empty + s, 1); }
-    for (int s = 0; s < kTcAccSlots; s++) { mbar_init(acc_full + s, 1); mbar_init(acc_empty + s, kTcProducers / 32); }
-    mbar_init(done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_base_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
+  {
     // operand tiles start as zeros: rows that carry no line are never written again
     uint4* z = reinterpret_cast<uint4*>(smem);
-    for (int k = tid; k < kTcOpStages * 2 * kTcOpBytes / 16; k += kTcProducers) z[k] = make_uint4(0u, 0u, 0u, 0u);
+    for (int k = tid; k < kTcOpStages * 2 * kTcOpBytes / 16; k += kTcThreads) z[k] = make_uint4(0u, 0u, 0u, 0u);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_base_smem;
-  const bool dbg = (blockIdx.x == 0 && blockIdx.y == 20);
-  const bool dbg0 = dbg && tid == 0;
+  const bool dbg0 = (blockIdx.x == 0 && blockIdx.y == 20) && tid == 0;
   (void)dbg0;
   TC_STAMP(dbg0, 0);
 #ifdef DBA_TC_TIMING
   if (dbg0) { g_tc_timing[1] = (unsigned long long)nchunks; g_tc_timing[2] = (unsigned long long)R6; }
 #endif
 
-  if (warp == 8) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_tf32(128, N);
-      const uint32_t d_g = tmem_base + 3 * 128;
-      for (int c = 0; c < nchunks; c++) {
-        const int os = c % kTcOpStages, slot = c % kTcAccSlots;
-        TC_STAMP(dbg, 4096 + 4 * c + 0);
-        mbar_wait(full + os, (c / kTcOpStages) & 1);
-        TC_STAMP(dbg, 4096 + 4 * c + 1);
-        if (c >= kTcAccSlots) mbar_wait(acc_empty + slot, ((c / kTcAccSlots) - 1) & 1);
-        TC_STAMP(dbg, 4096 + 4 * c + 2);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t hi0 = op_base + (uint32_t)os * 2 * kTcOpBytes, lo0 = hi0 + kTcOpBytes;
-        const uint32_t d = tmem_base + (uint32_t)(slot * 128);
+  // ================= raw rows -> split operands =================
+  // Every warp stages and splits its OWN lines (line = warp + 8 i); the operand stage is shared by both warpgroups' MMAs.
+  // Warp-private raw slab: 16 rows x 128 B per stage; slab row li = i (not packed) or hf * 8 + i (packed: half hf of the chunk).
+  // A thread owns four (slab row, 16-byte piece) copy slots: li = 4 s + lane / 8, piece = lane % 8.
+  const float* src[4];
+  uint32_t dst[4];
+  int pxo[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
-          const uint64_t dh = umma_desc_k_sw128(hi0 + k * 32, 1024), dl = umma_desc_k_sw128(lo0 + k * 32, 1024);
-          umma_tf32(d, dh, dh, idesc, k > 0 ? 1u : 0u);
-          umma_tf32(d_g, dh, dl, idesc, (c > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(empty + os);          // the operand stage may be overwritten once these MMAs have read it
-        umma_commit(acc_full + slot);     // ... and the chunk's hi hi^T is ready to be drained
-        TC_STAMP(dbg, 4096 + 4 * c + 3);
-      }
-      umma_commit(done);
+  for (int i = 0; i < 4; i++) {
+    const int li = 4 * i + (lane >> 3), piece = lane & 7;
+    const int hf = two_halves ? (li >> 3) : 0, line = warp + 8 * (two_halves ? (li & 7) : li);
+    const int R6x = PAIR ? (hf ? R6b : R6a) : R6, row0 = PAIR ? kPairTileRows * (hf ? tb : ta) : 0;
+    // slots without a line copy zero bytes (cp.async zero-fills) into their unused slab row: no branch in the copy loop
+    src[i] = Cin; pxo[i] = 1 << 30;
+    dst[i] = raw_base + warp * 2048 + li * 128 + piece * 16;
+    if (line <= R6x) {
+      const float* base = (line < R6x) ? s_ptr[row0 + line / 6] + (size_t)(line % 6) * HW : win + (size_t)m * HW;
+      pxo[i] = (packed ? hf * 32 : 0) + piece * 4;
+      src[i] = base + pxo[i];
     }
-    __syncwarp();
-  } else {
-    // ================= producers: raw rows -> split operands =================
-    // Every warp stages and splits its OWN lines (line = warp + 8 i), so the only CTA-wide coupling is through the mbarriers.
-    // Warp-private raw slab: 16 rows x 128 B per stage; slab row li = i (not packed) or hf * 8 + i (packed: half hf of the chunk).
-    // A thread owns four (slab row, 16-byte piece) copy slots: li = 4 s + lane / 8, piece = lane % 8.
-    const float* src[4];
-    uint32_t dst[4];
-    int pxo[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int li = 4 * i + (lane >> 3), piece = lane & 7;
-      const int hf = two_halves ? (li >> 3) : 0, line = warp + 8 * (two_halves ? (li & 7) : li);
-      const int R6x = PAIR ? (hf ? R6b : R6a) : R6, row0 = PAIR ? kPairTileRows * (hf ? tb : ta) : 0;
-      // slots without a line copy zero bytes (cp.async zero-fills) into their unused slab row: no branch in the copy loop
-      src[i] = Cin; pxo[i] = 1 << 30;
-      dst[i] = raw_base + warp * 2048 + li * 128 + piece * 16;
-      if (line <= R6x) {
-        const float* base = (line < R6x) ? s_ptr[row0 + line / 6] + (size_t)(line % 6) * HW : win + (size_t)m * HW;
-        pxo[i] = (packed ? hf * 32 : 0) + piece * 4;
-        src[i] = base + pxo[i];
-      }
-    }
-    const float* Cm = Cin + (size_t)m * HW;
-    // this thread's share of S: operand row q*32 + lane; column blocks of 32: packed -> the one block of its own half,
-    // otherwise half_w*32 and 64 + half_w*32
-    const int q = warp & 3, half_w = warp >> 2;
-    const int row = q * 32 + lane;
-    const int lrow = packed ? (row & 63) : row;                     // line of this row
-    const int lq = two_halves ? (q & 1) : q;                        // 32-row group inside the half
-    const int ncb = packed ? 1 : 2;
-    const int cb0 = packed ? ((q >> 1) * 64 + half_w * 32) : half_w * 32;
-    const int R6q = PAIR ? ((q >> 1) ? R6b : R6a) : R6;             // lines of this row's half
-    // PAIR: which of this thread's two column blocks are wanted: rows of tile a only need S_aa (block 0, if this CTA emits it);
-    // rows of tile b need S_ba (block 0) and S_bb (block 1, if emitted)
-    const bool need0 = !PAIR || ((q >> 1) ? true : emit_a);
-    const bool need1 = !PAIR || ((q >> 1) ? emit_b : false);
-    float acc[2][32];
-#pragma unroll
-    for (int h = 0; h < 2; h++)
-#pragma unroll
-      for (int j = 0; j < 32; j++) acc[h][j] = 0.f;
-    auto drain = [&](int cd) {
-      const int slot = cd % kTcAccSlots;
-      mbar_wait(acc_full + slot, (cd / kTcAccSlots) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int cb = cb0 + h * 64;
-        if (h < ncb && cb < N && lq * 32 < R6q && (h ? need1 : need0)) {     // warp-uniform: groups without live rows skip the TMEM read
-          uint32_t r[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * 128 + cb), r);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int j = 0; j < 32; j++) acc[h][j] += __uint_as_float(r[j]);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty + slot);
-    };
-    auto issue = [&](int c) {
-      if (c < nchunks) {
-        const int p0 = px_begin + c * cpx;
-        const uint32_t stage_off = (uint32_t)(c % kTcRawStages) * kTcRawBytes;
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const bool ok = p0 + pxo[i] < px_end;            // false for slots without a line (pxo = 2^30)
-          cp_async16_zfill(dst[i] + stage_off, ok ? (const void*)(src[i] + p0) : (const void*)Cin, ok ? 16u : 0u);
-        }
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-#pragma unroll
-    for (int s = 0; s < kTcRawStages - 1; s++) issue(s);
-
-    // A thread splits exactly the 16-byte pieces it copied (slot i: slab row 4 i + lane / 8, pixels 4 (lane % 8) .. + 3): one
-    // 128-bit shared load, four scale / round / subtract chains, two 128-bit swizzled stores per slot.  A 16-byte piece stays
-    // contiguous under the 128-byte swizzle (chunk index ^ row % 8).
-    const int piece = lane & 7;
-    uint32_t op_off[4];                                      // byte offset of the slot's piece inside an operand tile
-    bool live[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int li = 4 * i + (lane >> 3);
-      const int hf = two_halves ? (li >> 3) : 0, line = warp + 8 * (two_halves ? (li & 7) : li);
-      const uint32_t rr = (uint32_t)(hf * 64 + line);
-      live[i] = line <= (PAIR ? (hf ? R6b : R6a) : R6);
-      op_off[i] = rr * 128 + (((uint32_t)piece ^ (rr & 7u)) << 4);
-    }
-    auto load_c4 = [&](int c, int hf) -> float4 {          // C of this thread's four pixels in half hf of chunk c (0 beyond the range)
-      const int px = px_begin + c * cpx + hf * 32 + 4 * piece;
-      return (c < nchunks && px < px_end) ? __ldg(reinterpret_cast<const float4*>(Cm + px)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    };
-    auto rsq4 = [](float4 v) -> float4 {                     // sqrt(Q); pixels beyond the range stay zero
-      return make_float4(v.x > 0.f ? rsqrtf(v.x) : 0.f, v.y > 0.f ? rsqrtf(v.y) : 0.f, v.z > 0.f ? rsqrtf(v.z) : 0.f, v.w > 0.f ? rsqrtf(v.w) : 0.f);
-    };
-    float4 Cn0 = load_c4(0, 0), Cn1 = packed ? load_c4(0, 1) : make_float4(0.f, 0.f, 0.f, 0.f);
-    TC_STAMP(dbg0, 3);
-    for (int c = 0; c < nchunks; c++) {
-      TC_STAMP(dbg0, 16 + 8 * c + 0);
-      asm volatile("cp.async.wait_group %0;" ::"n"(kTcRawStages - 2) : "memory");
-      __syncwarp();                                          // this warp's copies of chunk c have landed
-      TC_STAMP(dbg0, 16 + 8 * c + 1);
-      const int os = c % kTcOpStages;
-      if (c >= kTcOpStages) mbar_wait(empty + os, ((c / kTcOpStages) - 1) & 1);
-      TC_STAMP(dbg0, 16 + 8 * c + 2);
-      const uint32_t raw = raw_base + (uint32_t)(c % kTcRawStages) * kTcRawBytes + (uint32_t)warp * 2048 + (uint32_t)(lane >> 3) * 128 +
-                           (uint32_t)piece * 16;
-      const uint32_t ophi = op_base + (uint32_t)os * 2 * kTcOpBytes;
-      const float4 sq0 = rsq4(Cn0), sq1 = rsq4(Cn1);
-      Cn0 = load_c4(c + 1, 0); Cn1 = packed ? load_c4(c + 1, 1) : Cn1;      // one chunk ahead
-      float4 xv[4];
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(xv[i].x), "=f"(xv[i].y), "=f"(xv[i].z), "=f"(xv[i].w) : "r"(raw + (uint32_t)i * 512) : "memory");
+  }
+  const float* Cm = Cin + (size_t)m * HW;
+  auto issue = [&](int c) {
+    if (c < nchunks) {
+      const int p0 = px_begin + c * cpx;
+      const uint32_t stage_off = (uint32_t)(c % kTcRawStages) * kTcRawBytes;
 #pragma unroll
       for (int i = 0; i < 4; i++) {
-        const float4 q = (packed && i >= 2) ? sq1 : sq0;
-        const float x[4] = {xv[i].x * q.x, xv[i].y * q.y, xv[i].z * q.z, xv[i].w * q.w};
-        float hi[4], lo[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) {                        // tf32 round-to-nearest (ties away), as cvt.rna.tf32.f32 for finite x
-          hi[k] = __uint_as_float((__float_as_uint(x[k]) + 0x1000u) & 0xffffe000u);
-          lo[k] = x[k] - hi[k];
-        }
-        if (live[i]) {
-          asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ophi + op_off[i]), "f"(hi[0]), "f"(hi[1]), "f"(hi[2]), "f"(hi[3]) : "memory");
-          asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ophi + kTcOpBytes + op_off[i]), "f"(lo[0]), "f"(lo[1]), "f"(lo[2]), "f"(lo[3]) : "memory");
-        }
-      }
-      TC_STAMP(dbg0, 16 + 8 * c + 3);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // generic-proxy stores -> visible to the tensor core
-      __syncwarp();
-      if (lane == 0) mbar_arrive(full + os);
-      TC_STAMP(dbg0, 16 + 8 * c + 4);
-      issue(c + kTcRawStages - 1);
-      TC_STAMP(dbg0, 16 + 8 * c + 5);
-      if (c >= 2) drain(c - 2);
-      TC_STAMP(dbg0, 16 + 8 * c + 6);
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    if (nchunks >= 2) drain(nchunks - 2);
-    drain(nchunks - 1);
-    TC_STAMP(dbg0, 4);
-
-    // ================= G = hi lo^T: through shared memory (the operand ring is idle now) so that G + G^T can be formed
-    mbar_wait(done, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const int cb = cb0 + h * 64;
-      if (h < ncb && cb < N && lq * 32 <= R6q) {                     // PAIR: all four blocks of G (the lower-left block needs G^T from the upper right)
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(3 * 128 + cb), r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 32; j++) sts_f32(op_base + (uint32_t)(row * kTcCxStride + cb + j) * 4, __uint_as_float(r[j]));
+        const bool ok = p0 + pxo[i] < px_end;            // false for slots without a line (pxo = 2^30)
+        cp_async16_zfill(dst[i] + stage_off, ok ? (const void*)(src[i] + p0) : (const void*)Cin, ok ? 16u : 0u);
       }
     }
-    asm volatile("bar.sync 1, %0;" ::"n"(kTcProducers) : "memory");
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+#pragma unroll
+  for (int s = 0; s < kTcRawStages - 1; s++) issue(s);
 
-    // ================= epilogue: lower triangle of S (and the rhs column) into the reduced system =================
+  // A thread splits exactly the 16-byte pieces it copied (slot i: slab row 4 i + lane / 8, pixels 4 (lane % 8) .. + 3): one
+  // 128-bit shared load, four scale / round / subtract chains, two 128-bit swizzled stores per slot.  A 16-byte piece stays
+  // contiguous under the 128-byte swizzle (chunk index ^ row % 8).
+  const int piece = lane & 7;
+  uint32_t op_off[4];                                      // byte offset of the slot's piece inside an operand tile
+  bool live[4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    const int li = 4 * i + (lane >> 3);
+    const int hf = two_halves ? (li >> 3) : 0, line = warp + 8 * (two_halves ? (li & 7) : li);
+    const uint32_t rr = (uint32_t)(hf * 64 + line);
+    live[i] = line <= (PAIR ? (hf ? R6b : R6a) : R6);
+    op_off[i] = rr * 128 + (((uint32_t)piece ^ (rr & 7u)) << 4);
+  }
+  auto load_c4 = [&](int c, int hf) -> float4 {          // C of this thread's four pixels in half hf of chunk c (0 beyond the range)
+    const int px = px_begin + c * cpx + hf * 32 + 4 * piece;
+    return (c < nchunks && px < px_end) ? __ldg(reinterpret_cast<const float4*>(Cm + px)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  };
+  auto rsq4 = [](float4 v) -> float4 {                     // sqrt(Q); pixels beyond the range stay zero
+    return make_float4(v.x > 0.f ? rsqrtf(v.x) : 0.f, v.y > 0.f ? rsqrtf(v.y) : 0.f, v.z > 0.f ? rsqrtf(v.z) : 0.f, v.w > 0.f ? rsqrtf(v.w) : 0.f);
+  };
+  float4 Cn0 = load_c4(0, 0), Cn1 = packed ? load_c4(0, 1) : make_float4(0.f, 0.f, 0.f, 0.f);
+  const int wg = warp >> 2;
+  float acc[64], D[64], G[64];                              // running hi hi^T, this chunk's hi hi^T, hi lo^T (m64n128 fragments)
+#pragma unroll
+  for (int j = 0; j < 64; j++) acc[j] = 0.f;
+  TC_STAMP(dbg0, 3);
+  // Operand stage c % 4 is rewritten at chunk c: the MMAs of chunk c - 4 that read it are complete, because each warpgroup waits
+  // for its chunk c - 2 before issuing chunk c - 1, and both passed the CTA barrier of chunk c - 1.
+  for (int c = 0; c < nchunks; c++) {
+    TC_STAMP(dbg0, 16 + 8 * c + 0);
+    asm volatile("cp.async.wait_group %0;" ::"n"(kTcRawStages - 2) : "memory");
+    __syncwarp();                                          // this warp's copies of chunk c have landed
+    TC_STAMP(dbg0, 16 + 8 * c + 1);
+    const int os = c % kTcOpStages;
+    const uint32_t raw = raw_base + (uint32_t)(c % kTcRawStages) * kTcRawBytes + (uint32_t)warp * 2048 + (uint32_t)(lane >> 3) * 128 +
+                         (uint32_t)piece * 16;
+    const uint32_t ophi = op_base + (uint32_t)os * 2 * kTcOpBytes;
+    const float4 sq0 = rsq4(Cn0), sq1 = rsq4(Cn1);
+    Cn0 = load_c4(c + 1, 0); Cn1 = packed ? load_c4(c + 1, 1) : Cn1;      // one chunk ahead
+    float4 xv[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+      asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(xv[i].x), "=f"(xv[i].y), "=f"(xv[i].z), "=f"(xv[i].w) : "r"(raw + (uint32_t)i * 512) : "memory");
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const float4 q = (packed && i >= 2) ? sq1 : sq0;
+      const float x[4] = {xv[i].x * q.x, xv[i].y * q.y, xv[i].z * q.z, xv[i].w * q.w};
+      float hi[4], lo[4];
+#pragma unroll
+      for (int k = 0; k < 4; k++) {                        // tf32 round-to-nearest (ties away), as cvt.rna.tf32.f32 for finite x
+        hi[k] = __uint_as_float((__float_as_uint(x[k]) + 0x1000u) & 0xffffe000u);
+        lo[k] = x[k] - hi[k];
+      }
+      if (live[i]) {
+        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ophi + op_off[i]), "f"(hi[0]), "f"(hi[1]), "f"(hi[2]), "f"(hi[3]) : "memory");
+        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ophi + kTcOpBytes + op_off[i]), "f"(lo[0]), "f"(lo[1]), "f"(lo[2]), "f"(lo[3]) : "memory");
+      }
+    }
+    TC_STAMP(dbg0, 16 + 8 * c + 3);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // generic-proxy stores -> visible to the tensor core
+    __syncthreads();
+    if (c > 0) {                                                         // chunk c - 1's hi hi^T into the running sum
+      wgmma_wait<0>();
+      wgmma_fence_regs(D);
+#pragma unroll
+      for (int j = 0; j < 64; j++) acc[j] += D[j];
+    }
+    wgmma_fence();
+    {
+      const uint32_t hi0 = ophi, lo0 = ophi + kTcOpBytes;
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const uint64_t da = gmma_desc_sw128(hi0 + wg * 64 * 128 + k * 32, 16, 1024);
+        wgmma_tf32_n128(D, da, gmma_desc_sw128(hi0 + k * 32, 16, 1024), k > 0 ? 1 : 0);
+        wgmma_tf32_n128(G, da, gmma_desc_sw128(lo0 + k * 32, 16, 1024), (c > 0 || k > 0) ? 1 : 0);
+      }
+    }
+    wgmma_commit();
+    TC_STAMP(dbg0, 16 + 8 * c + 4);
+    issue(c + kTcRawStages - 1);
+  }
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  wgmma_wait<0>();
+  wgmma_fence_regs(D);
+  wgmma_fence_regs(G);
+#pragma unroll
+  for (int j = 0; j < 64; j++) acc[j] += D[j];
+  TC_STAMP(dbg0, 4);
+
+  // ================= G = hi lo^T: through shared memory (the operand ring is idle now) so that G + G^T can be formed
+  __syncthreads();                                         // both warpgroups' MMAs have completed: the ring may be overwritten
+  const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2), c_base = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 16; j++)
+#pragma unroll
+    for (int e = 0; e < 4; e++)
+      sts_f32(op_base + (uint32_t)((r_base + 8 * (e >> 1)) * kTcCxStride + 8 * j + c_base + (e & 1)) * 4, G[4 * j + e]);
+  __syncthreads();
+
+  // ================= epilogue: lower triangle of S (and the rhs column) into the reduced system =================
+#pragma unroll
+  for (int ih = 0; ih < 2; ih++) {
+    const int row = r_base + 8 * ih;
+    const int lrow = packed ? (row & 63) : row;                       // line of this row
     const int gr = PAIR ? s_gidx[row] : ((lrow < R6) ? s_gidx[lrow] : -2);
-    if (gr >= 0) {
-      const int cofs = packed ? (row & 64) : 0;                     // first operand column of this row's half
+    if (gr < 0) continue;
+    const bool rb = row >= 64;
 #pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int cb = cb0 + h * 64;
-        if (h < ncb && cb < N && (h ? need1 : need0)) {
-          const bool cross = PAIR && ((row >> 6) != (cb >> 6));     // lower-left block S_ba: every unordered row pair appears once
+    for (int j = 0; j < 16; j++) {
 #pragma unroll
-          for (int j = 0; j < 32; j++) {
-            const int col = cb + j;
-            const int gc = s_gidx[col - cofs];
-            if (gc == -2) continue;
-            const float g = lds_f32(op_base + (uint32_t)(row * kTcCxStride + col) * 4) + lds_f32(op_base + (uint32_t)(col * kTcCxStride + row) * 4);
-            const double v = -(double)(acc[h][j] + g);
-            if (cross) {
-              if (gc < 0) continue;                                 // the rhs comes from the diagonal blocks
-              if (gr > gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
-              else if (gr < gc) atomicAdd(&Hsys[(size_t)gc * n + gr], v);
-              else atomicAdd(&Hsys[(size_t)gr * n + gr], 2.0 * v);  // two different rows with the same pose: (r,c) and (c,r) land on one entry
-            } else if (gc >= 0) {
-              if (gr >= gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
-            } else {
-              atomicAdd(&bsys[gr], v);
-            }
-          }
+      for (int e = 0; e < 2; e++) {
+        const int col = 8 * j + c_base + e;
+        const bool cbk = col >= 64;
+        int gc;
+        if (PAIR) {          // rows of tile a need S_aa (if this CTA emits it); rows of tile b need S_ba and S_bb (if emitted)
+          if (!rb && (cbk || !emit_a)) continue;
+          if (rb && cbk && !emit_b) continue;
+          gc = s_gidx[col];
+        } else if (packed) {  // the diagonal block of this row's half
+          if (cbk != rb) continue;
+          gc = s_gidx[col & 63];
+        } else {
+          gc = s_gidx[col];
+        }
+        if (gc == -2) continue;
+        const float g = lds_f32(op_base + (uint32_t)(row * kTcCxStride + col) * 4) + lds_f32(op_base + (uint32_t)(col * kTcCxStride + row) * 4);
+        const double v = -(double)(acc[4 * j + 2 * ih + e] + g);
+        if (PAIR && rb != cbk) {                                     // lower-left block S_ba: every unordered row pair appears once
+          if (gc < 0) continue;                                      // the rhs comes from the diagonal blocks
+          if (gr > gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
+          else if (gr < gc) atomicAdd(&Hsys[(size_t)gc * n + gr], v);
+          else atomicAdd(&Hsys[(size_t)gr * n + gr], 2.0 * v);       // two different rows with the same pose: (r,c) and (c,r) land on one entry
+        } else if (gc >= 0) {
+          if (gr >= gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
+        } else {
+          atomicAdd(&bsys[gr], v);
         }
       }
     }
   }
   TC_STAMP(dbg0, 5);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  TC_STAMP(dbg0, 6);
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1350,8 +1282,10 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
   if (L.P == 0) return DBA_OK;
   // frames that can own edges on this rank (edge-sharded runs own a sub-range): size the pixel chunks so the grid fills the GPU
   const int eff_frames = std::max(1, std::min(a->n_frames, a->own_hi - a->own_lo));
-  const int ppt = (eff_frames * ((HW + 4 * kBuildThreads - 1) / (4 * kBuildThreads)) >= 148) ? 4
-                : (eff_frames * ((HW + 2 * kBuildThreads - 1) / (2 * kBuildThreads)) >= 148) ? 2 : 1;
+  static int sms = 0;
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
+  const int ppt = (eff_frames * ((HW + 4 * kBuildThreads - 1) / (4 * kBuildThreads)) >= sms) ? 4
+                : (eff_frames * ((HW + 2 * kBuildThreads - 1) / (2 * kBuildThreads)) >= sms) ? 2 : 1;
 #define LAUNCH_BUILD(PPT)                                                                                                               \
   ba_build_kernel<PPT><<<dim3((HW + PPT * kBuildThreads - 1) / (PPT * kBuildThreads), a->n_frames), kBuildThreads, 0, st>>>(             \
       a->poses, a->disps, a->intrinsics, a->disps_sens, a->targets, a->weights, a->eta, a->eta_rows, a->eta_by_frame, a->jj, WS(int, L.off_hdr),  \
@@ -1364,13 +1298,13 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
     const size_t smem2 = (size_t)2 * kSgK * kSgStride * sizeof(float);
     // small frames: about 2.5 CTAs per SM worth of (frame, chunk) work items of whole 64-pixel tiles
     const int tiles1 = (HW + kSgK - 1) / kSgK;
-    const int chunks1 = std::max(1, std::min(tiles1, (5 * 148 / 2 + eff_frames - 1) / eff_frames));
+    const int chunks1 = std::max(1, std::min(tiles1, (5 * sms / 2 + eff_frames - 1) / eff_frames));
     const int px_per_cta1 = ((tiles1 + chunks1 - 1) / chunks1) * kSgK;
     const int gx1 = (HW + px_per_cta1 - 1) / px_per_cta1;
     // the SGEMM-style kernel keeps its accumulators in registers over the whole pixel chunk: few long chunks, tile pairs over z
     const int px_per_cta2 = ((HW + 2) / 3 + kSgK - 1) / kSgK * kSgK;
     const int gx2 = (HW + px_per_cta2 - 1) / px_per_cta2;
-    const int zsplit2 = std::max(1, std::min(32, (6 * 148 + eff_frames * gx2 - 1) / (eff_frames * gx2)));
+    const int zsplit2 = std::max(1, std::min(32, (6 * sms + eff_frames * gx2 - 1) / (eff_frames * gx2)));
     static bool attr_set = false;
     if (!attr_set) {
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2), "schur gemm smem attr");
@@ -1385,7 +1319,7 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
     int pair_rows_max = kTcRowsMax;                  // frames with more rows than this go to the SIMT kernel
     if (use_tc) {
       const int tiles64 = (HW + 63) / 64;
-      const int chunks_tc = std::max(1, std::min(tiles64, (148 + eff_frames / 2) / eff_frames));     // one CTA per SM
+      const int chunks_tc = std::max(1, std::min(tiles64, (sms + eff_frames / 2) / eff_frames));     // one CTA per SM
       const int px_per_cta_tc = ((tiles64 + chunks_tc - 1) / chunks_tc) * 64;
       const int gx_tc = (HW + px_per_cta_tc - 1) / px_per_cta_tc;
       ba_schur_tc_kernel<false><<<dim3(gx_tc, a->n_frames, 1), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),

@@ -1,7 +1,7 @@
 // `droid_backends` -- drop-in Python extension exporting the reference's nine callables
 // (reference src/droid.cpp:93-259: ba, frame_distance, projmap, depth_filter, iproj, altcorr_forward,
 // altcorr_backward, corr_index_forward, corr_index_backward) with identical positional signatures and return
-// shapes, implemented on the C ABI of include/droid_b200.h (libdroid_b200.so, hand-written sm_100a kernels).
+// shapes, implemented on the C ABI of include/droid_b200.h (libdroid_b200.so, hand-written sm_90a kernels).
 //
 // torch is used here for what the reference binding uses it for: tensor handles, the caching allocator, the current
 // stream.  Differences from the reference binding, all strictly safer: a CUDAGuard on the tensors' device, launches on
@@ -413,7 +413,7 @@ torch::Tensor proximity_edges(torch::Tensor d, int64_t t0, int64_t t1, int64_t t
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "B200-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
+  m.doc() = "H100-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
   // bundle adjustment kernels
   m.def("ba", &ba, "bundle adjustment");
   m.def("frame_distance", &frame_distance, "frame_distance");
@@ -425,15 +425,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("altcorr_backward", &altcorr_backward, "ALTCORR backward");
   m.def("corr_index_forward", &corr_index_forward, "INDEX forward");
   m.def("corr_index_backward", &corr_index_backward, "INDEX backward");
-  m.def("corr_volume_pyramid", &corr_volume_pyramid, "all-pairs correlation + 4-level pyramid (tcgen05), B200 extension", pybind11::arg("fmap1"), pybind11::arg("fmap2"),
+  m.def("corr_volume_pyramid", &corr_volume_pyramid, "all-pairs correlation + 4-level pyramid (wgmma), native extension", pybind11::arg("fmap1"), pybind11::arg("fmap2"),
         pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("tiled") = false);
-  m.def("corr_lookup_pyramid", &corr_lookup_pyramid, "4-level radius-3 lookup in one launch -> [E,196,H,W], B200 extension", pybind11::arg("pyramid"), pybind11::arg("coords"),
+  m.def("corr_lookup_pyramid", &corr_lookup_pyramid, "4-level radius-3 lookup in one launch -> [E,196,H,W], native extension", pybind11::arg("pyramid"), pybind11::arg("coords"),
         pybind11::arg("tiled") = false);
   m.def("corr_volume_supported", [](int dim, int ht, int wd) { return dba_corr_volume_supported(dim, ht, wd, DBA_F16) != 0; }, "does corr_volume_pyramid have a kernel for f16 [.,dim,ht,wd] feature maps");
-  m.def("reproject", &reproject, "fused pops.projective_transform(jacobian=False), B200 extension");
-  m.def("update_forward", &update_forward, "update operator (ConvGRU + heads + GraphAgg) on tcgen05, B200 extension");
-  m.def("conv_nhwc", &conv_nhwc, "channels-last 1x1/3x3 convolution on tcgen05, B200 extension");
-  m.def("cvx_upsample", &cvx_upsample, "convex upsampling of inverse depth maps (droid_net.cvx_upsample, dim = 1), B200 extension");
-  m.def("proximity_edges", &proximity_edges, "edge selection of FactorGraph.add_proximity_factors (factor_graph.py:357-411), B200 extension");
+  m.def("reproject", &reproject, "fused pops.projective_transform(jacobian=False), native extension");
+  m.def("update_forward", &update_forward, "update operator (ConvGRU + heads + GraphAgg) on wgmma, native extension");
+  m.def("conv_nhwc", &conv_nhwc, "channels-last 1x1/3x3 convolution on wgmma, native extension");
+  m.def("cvx_upsample", &cvx_upsample, "convex upsampling of inverse depth maps (droid_net.cvx_upsample, dim = 1), native extension");
+  m.def("proximity_edges", &proximity_edges, "edge selection of FactorGraph.add_proximity_factors (factor_graph.py:357-411), native extension");
   m.def("_b200_native", []() { return true; });
 }

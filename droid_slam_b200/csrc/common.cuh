@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels of the dense-BA update path.
+// Shared device helpers for the sm_90a kernels of the dense-BA update path.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

@@ -1,4 +1,4 @@
-// corr_index_forward / corr_index_backward for sm_100a.
+// corr_index_forward / corr_index_backward for sm_90a.
 //
 // Replaces reference src/correlation_kernels.cu:20-185.  Semantics (checked against oracle/corr.py):
 //   out[n][i][j][y][x] = bilinear sample of volume[n][y][x][.][.] at (y0-r+j, x0-r+i), taps outside the plane

@@ -1,27 +1,28 @@
-// All-pairs correlation volume + 4-level pooled pyramid in ONE pass on the 5th-gen tensor cores (tcgen05 + TMEM + TMA).
+// All-pairs correlation volume + 4-level pooled pyramid in ONE pass on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 // Replaces CorrBlock.__init__ / CorrBlock.corr (reference droid_slam/modules/corr.py:24-38, 63-71): a cuBLAS batched GEMM
 // writing the [E,HW,HW] level-0 volume followed by three avg_pool2d passes that re-read it.  Here, per edge e:
-//     L0[m][n]  = fp16( (1/16) * sum_c f1[ii[e]][c][m] * f2[jj[e]][c][n] )           (fp32 accumulation in TMEM)
+//     L0[m][n]  = fp16( (1/16) * sum_c f1[ii[e]][c][m] * f2[jj[e]][c][n] )           (fp32 accumulation in registers)
 //     L1..L3    = 2x2 average pooling over n = (y2,x2) (ATen rounds every level to fp16 before pooling the next; here the
 //                 cascade runs in fp32 on the accumulator and each level is rounded once -- closer to exact, within fp16 ulp)
 // are produced by one kernel: the GEMM is write bound (2*HW^2*128 flop vs 1.33*HW^2*2 bytes per edge, ~150 flop/B, far
-// below the B200 ridge), so the pyramid is computed in the epilogue from the accumulator while it is still on chip and the
+// below the H100 ridge), so the pyramid is computed in the epilogue from the accumulator while it is still on chip and the
 // volume is written exactly once (25.1 MB/edge at 48x64 instead of ~50 MB of traffic for GEMM + 3 pooling passes).
 //
-// CTA = (edge, 128 source pixels m).  Warp 0: TMA producer (cp.async.bulk.tensor, 128B swizzle) -- the A tile
-// [128 ch x 128 px] once, then B chunks [128 ch x 256 px] (= 4 image rows of frame j), double buffered.  Warp 1: MMA issuer,
-// tcgen05.mma.cta_group::1.kind::f16, M=128, N=256, K=16 x 8, both operands MN-major straight from the [C,H,W] feature
-// layout (no transposes anywhere), two 256-column fp32 accumulators in TMEM so the MMA of chunk c+1 overlaps the epilogue of
-// chunk c.  Warps 2-9: epilogue, tcgen05.ld 32 lanes x 32 columns, thread = one source pixel row m x half an image row, which
-// makes every pooling window thread-local (registers only); outputs leave as 256-bit stores.
+// CTA = (edge, 128 source pixels m), 288 threads.  Warp 8: TMA producer (cp.async.bulk.tensor, 128B swizzle) -- the A tile
+// [128 ch x 128 px] once, then B chunks [128 ch x 256 px] (= 4 image rows of frame j), double buffered.  Warps 0-7: two
+// consumer warpgroups, warpgroup w owns source pixels 64 w .. 64 w + 63; per chunk it runs wgmma.m64n128k16 x 8 (K = 128) on
+// each half of the chunk (2 image rows), both operands MN-major straight from the [C,H,W] feature layout (no transposes), and
+// pools the register accumulator.  A thread holds two source pixels x (8-column groups, 2 adjacent columns each); 2x2 windows are
+// thread-local, 4x4 / 8x8 windows combine lanes of a quad by shuffles, and a 4x4 word transpose inside the quad turns the
+// fragment into 16-byte row pieces before the stores.
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 
 namespace dba {
 
-constexpr int kCvThreads = 320;          // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
+constexpr int kCvThreads = 288;          // warps 0..7 consumers (two warpgroups), warp 8 TMA
 constexpr int kCvM = 128;                // source pixels per CTA
 constexpr int kCvN = 256;                // target pixels per chunk (4 image rows at wd = 64)
 constexpr int kCvK = 128;                // channels
@@ -35,36 +36,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
                ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 
-// shared-memory matrix descriptor, MN-major, SWIZZLE_128B (cute::UMMA::SmemDescriptor): start>>4 | LBO>>4 <<16 | SBO>>4 <<32 |
-// version 1 <<46 | layout_type 2 <<61.  LBO = byte distance between 64-element MN atoms, SBO = between 8-row K groups.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): c=f32, a=b=f16, both MN-major, N>>3 at bit 17, M>>4 at bit 24
-__device__ __forceinline__ uint32_t umma_idesc_f16(int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                 // c_format = F32
-  d |= 1u << 15;                // a_major = MN
-  d |= 1u << 16;                // b_major = MN
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
-}
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 struct CvParams {
   const int64_t* ii; const int64_t* jj;
   __half* out0; __half* out1; __half* out2; __half* out3;
@@ -76,10 +47,17 @@ __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
   const __half2 t = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<const uint32_t*>(&t);
 }
-// 256-bit global store (sm_100: st.global.v8.b32): one full 32-byte sector per thread per instruction
-__device__ __forceinline__ void st_v8(__half* dst, const uint32_t* w) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]),
-               "r"(w[6]), "r"(w[7]) : "memory");
+__device__ __forceinline__ uint32_t sel4(const uint32_t (&w)[4], int i) { return i == 0 ? w[0] : i == 1 ? w[1] : i == 2 ? w[2] : w[3]; }
+// 4x4 transpose of 32-bit words inside a quad of lanes: on return lane q of the quad holds o[j] = (word q of lane j)
+__device__ __forceinline__ void quad_transpose(const uint32_t (&w)[4], uint32_t (&o)[4], int lane) {
+  const int q = lane & 3;
+#pragma unroll
+  for (int s = 0; s < 4; s++) {
+    const int src = (q + s) & 3;
+    const uint32_t v = __shfl_sync(0xffffffffu, sel4(w, (q - s) & 3), (lane & ~3) | src);
+#pragma unroll
+    for (int j = 0; j < 4; j++) if (j == src) o[j] = v;
+  }
 }
 
 __global__ void __launch_bounds__(kCvThreads, 1) corr_volume_pyramid_kernel(const __grid_constant__ CUtensorMap tmA,
@@ -92,9 +70,6 @@ __global__ void __launch_bounds__(kCvThreads, 1) corr_volume_pyramid_kernel(cons
   uint64_t* bar_a = bars + 0;
   uint64_t* full_b = bars + 1;       // [2]
   uint64_t* empty_b = bars + 3;      // [2]
-  uint64_t* tmem_full = bars + 5;    // [2]
-  uint64_t* tmem_empty = bars + 7;   // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 10);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int e = blockIdx.y;
@@ -103,19 +78,12 @@ __global__ void __launch_bounds__(kCvThreads, 1) corr_volume_pyramid_kernel(cons
 
   if (threadIdx.x == 0) {
     mbar_init(bar_a, 1);
-    for (int s = 0; s < 2; s++) { mbar_init(full_b + s, 1); mbar_init(empty_b + s, 1); mbar_init(tmem_full + s, 1); mbar_init(tmem_empty + s, 8); }
+    for (int s = 0; s < 2; s++) { mbar_init(full_b + s, 1); mbar_init(empty_b + s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM: 512 columns = two 128x256 fp32 accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_base_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================= TMA producer =================
     if (lane == 0) {
       mbar_expect_tx(bar_a, kSmemA);
@@ -128,111 +96,112 @@ __global__ void __launch_bounds__(kCvThreads, 1) corr_volume_pyramid_kernel(cons
         for (int b = 0; b < 4; b++) tma_load_3d(sB + s * kSmemB + b * kBoxBytes, &tmB, full_b + s, c * kCvN + 64 * b, 0, fj);
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = umma_idesc_f16(kCvM, kCvN);
-    mbar_wait(bar_a, 0);
-    for (int c = 0; c < p.n_chunks; c++) {
-      const int s = c & 1;
-      mbar_wait(full_b + s, (c >> 1) & 1);
-      if (c >= 2) mbar_wait(tmem_empty + s, ((c >> 1) - 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB + s * kSmemB);
+    return;
+  }
+  // ================= consumers: warpgroup wg = source pixels 64 wg .. 64 wg + 63 =================
+  const int wg = warp >> 2, qd = lane & 3;
+  const int wd = p.wd;                                                 // 64
+  const float sc = 0.0625f;                                            // (f1/4).(f2/4)
+  const uint32_t a0 = smem_u32(sA + wg * kBoxBytes);
+  size_t rowoff[2];                                                    // this thread's two source pixels (fragment rows)
 #pragma unroll
-        for (int k = 0; k < kCvK / 16; k++) {
-          const uint64_t ad = umma_desc_mn_sw128(a0 + k * 2048, kBoxBytes, 1024);
-          const uint64_t bd = umma_desc_mn_sw128(b0 + k * 2048, kBoxBytes, 1024);
-          umma_f16(tmem_base + s * kCvN, ad, bd, idesc, k > 0 ? 1u : 0u);
-        }
-        umma_commit(empty_b + s);     // smem stage may be refilled when these MMAs have read it
-        umma_commit(tmem_full + s);   // accumulator ready for the epilogue
+  for (int i = 0; i < 2; i++) rowoff[i] = (size_t)e * p.HW + m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+  float acc[64];
+  float l1h0[2][8], l2prev[2][8];
+  mbar_wait(bar_a, 0);
+  for (int c = 0; c < p.n_chunks; c++) {
+    const int s = c & 1;
+    mbar_wait(full_b + s, (c >> 1) & 1);
+    const uint32_t b0 = smem_u32(sB + s * kSmemB);
+#pragma unroll 1
+    for (int h = 0; h < 2; h++) {                                      // image rows 4c + 2h, 4c + 2h + 1 = columns 128 h .. 128 h + 127
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kCvK / 16; k++)
+        wgmma_f16<128>(acc, gmma_desc_sw128(a0 + k * 2048, kBoxBytes, 1024), gmma_desc_sw128(b0 + 2 * h * kBoxBytes + k * 2048, kBoxBytes, 1024),
+                       k > 0 ? 1 : 0, 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (h == 1) {                                                    // the smem stage may be refilled
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_b + s);
       }
-      __syncwarp();
-    }
-  } else {
-    // ================= epilogue: warps 2..9.  TMEM lane quarter q = warp % 4 (hardware rule); the two warps of a quarter
-    // split every image row of frame j into its left / right 32 columns, so all 2x2 / 4x4 / 8x8 pooling windows stay
-    // thread-local.  Pooling runs in fp32 on the accumulator values and is rounded once per level. =================
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;                                  // 0: columns 0..31, 1: columns 32..63 of each image row
-    const int m = m0 + q * 32 + lane;                                  // this thread's source pixel
-    const int wd = p.wd;                                               // 64
-    __half* o0 = p.out0 + ((size_t)e * p.HW + m) * (size_t)p.HW + half * 32;
-    __half* o1 = p.out1 + ((size_t)e * p.HW + m) * (size_t)(p.HW / 4) + half * 16;
-    __half* o2 = p.out2 + ((size_t)e * p.HW + m) * (size_t)(p.HW / 16) + half * 8;
-    __half* o3 = p.out3 + ((size_t)e * p.HW + m) * (size_t)(p.HW / 64) + half * 4;
-    const float sc = 0.0625f;                                          // (f1/4).(f2/4)
-    float l2prev[8];
-    for (int c = 0; c < p.n_chunks; c++) {
-      const int s = c & 1;
-      mbar_wait(tmem_full + s, (c >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tbase = tmem_base + s * kCvN + ((uint32_t)(q * 32) << 16) + half * 32;
-      float l1f[2][16];
 #pragma unroll
-      for (int rp = 0; rp < 2; rp++) {                                 // image rows 4c + 2rp, 4c + 2rp + 1
-        uint32_t ra[32], rb[32];
-        tmem_ld32(tbase + (2 * rp) * 64, ra);
-        tmem_ld32(tbase + (2 * rp + 1) * 64, rb);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        uint32_t wa[16], wb[16];
+      for (int i = 0; i < 2; i++) {
+        // level 0: per image row, two blocks of four 8-column groups -> one 16-byte piece (8 columns) per lane
 #pragma unroll
-        for (int k = 0; k < 16; k++) {
-          wa[k] = pack_h2(__uint_as_float(ra[2 * k]) * sc, __uint_as_float(ra[2 * k + 1]) * sc);
-          wb[k] = pack_h2(__uint_as_float(rb[2 * k]) * sc, __uint_as_float(rb[2 * k + 1]) * sc);
-          l1f[rp][k] = ((__uint_as_float(ra[2 * k]) + __uint_as_float(ra[2 * k + 1])) + (__uint_as_float(rb[2 * k]) + __uint_as_float(rb[2 * k + 1]))) * (0.25f * sc);
-        }
-        if (!p.tiled) {
-          // level 0: 32 halves = 64 contiguous bytes per image row, as 256-bit stores (one full 32-byte sector each)
-          st_v8(o0 + (size_t)c * kCvN + (2 * rp) * 64, wa);      st_v8(o0 + (size_t)c * kCvN + (2 * rp) * 64 + 16, wa + 8);
-          st_v8(o0 + (size_t)c * kCvN + (2 * rp + 1) * 64, wb);  st_v8(o0 + (size_t)c * kCvN + (2 * rp + 1) * 64 + 16, wb + 8);
-          // level 1 row 2c + rp: 16 halves = 32 bytes
-          uint32_t w1[8];
+        for (int ry = 0; ry < 2; ry++) {
 #pragma unroll
-          for (int k = 0; k < 8; k++) w1[k] = pack_h2(l1f[rp][2 * k], l1f[rp][2 * k + 1]);
-          st_v8(o1 + (size_t)(2 * c + rp) * (wd / 2), w1);
-        } else {
-          // tiled level 0: chunk c = tile row c; this thread's 32 columns = tiles 4*half .. 4*half+3; rows 2rp, 2rp+1 of a tile are
-          // adjacent 16-byte pieces -> one 32-byte sector per tile
-          __half* t0 = p.out0 + ((size_t)e * p.HW + m) * (size_t)p.HW + ((size_t)c * 8 + 4 * half) * 32 + (2 * rp) * 8;
+          for (int b = 0; b < 2; b++) {
+            uint32_t w[4], o[4];
 #pragma unroll
-          for (int t = 0; t < 4; t++) {
-            const uint32_t w8[8] = {wa[4 * t], wa[4 * t + 1], wa[4 * t + 2], wa[4 * t + 3], wb[4 * t], wb[4 * t + 1], wb[4 * t + 2], wb[4 * t + 3]};
-            st_v8(t0 + t * 32, w8);
+            for (int g = 0; g < 4; g++) {
+              const int j = ry * 8 + b * 4 + g;
+              w[g] = pack_h2(acc[4 * j + 2 * i] * sc, acc[4 * j + 2 * i + 1] * sc);
+            }
+            quad_transpose(w, o, lane);
+            const int gx = b * 4 + qd, row = 2 * h + ry;                // 8-column group of image row 4c + row
+            __half* dst = p.tiled ? p.out0 + rowoff[i] * (size_t)p.HW + ((size_t)c * 8 + gx) * 32 + row * 8
+                                  : p.out0 + rowoff[i] * (size_t)p.HW + (size_t)c * kCvN + row * 64 + gx * 8;
+            *reinterpret_cast<uint4*>(dst) = make_uint4(o[0], o[1], o[2], o[3]);
           }
-          // tiled level 1 (24 x 32 plane, 4 tiles per tile row): row 2c+rp -> tile row c/2, row 2(c&1)+rp inside; tiles 2*half, 2*half+1
-          __half* t1 = p.out1 + ((size_t)e * p.HW + m) * (size_t)(p.HW / 4) + ((size_t)(c >> 1) * 4 + 2 * half) * 32 + (2 * (c & 1) + rp) * 8;
-#pragma unroll
-          for (int t = 0; t < 2; t++)
-            *reinterpret_cast<uint4*>(t1 + t * 32) = make_uint4(pack_h2(l1f[rp][8 * t], l1f[rp][8 * t + 1]), pack_h2(l1f[rp][8 * t + 2], l1f[rp][8 * t + 3]),
-                                                               pack_h2(l1f[rp][8 * t + 4], l1f[rp][8 * t + 5]), pack_h2(l1f[rp][8 * t + 6], l1f[rp][8 * t + 7]));
         }
-      }
-      // accumulator drained: hand the TMEM stage back to the MMA warp
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty + s);
-      // level 2 row c: 8 halves = 16 bytes
-      float l2f[8];
+        // level 1 row 2c + h: column 4 gx + qd of this lane
+        float l1[8];
 #pragma unroll
-      for (int k = 0; k < 8; k++) l2f[k] = ((l1f[0][2 * k] + l1f[0][2 * k + 1]) + (l1f[1][2 * k] + l1f[1][2 * k + 1])) * 0.25f;
-      *reinterpret_cast<uint4*>(o2 + (size_t)c * (wd / 4)) =
-          make_uint4(pack_h2(l2f[0], l2f[1]), pack_h2(l2f[2], l2f[3]), pack_h2(l2f[4], l2f[5]), pack_h2(l2f[6], l2f[7]));
-      if (c & 1) {   // level 3 row c/2: 4 halves = 8 bytes
-        float l3f[4];
+        for (int gx = 0; gx < 8; gx++)
+          l1[gx] = ((acc[4 * gx + 2 * i] + acc[4 * gx + 2 * i + 1]) + (acc[4 * (8 + gx) + 2 * i] + acc[4 * (8 + gx) + 2 * i + 1])) * (0.25f * sc);
+        {
+          uint32_t w[4], r[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++) l3f[k] = ((l2prev[2 * k] + l2prev[2 * k + 1]) + (l2f[2 * k] + l2f[2 * k + 1])) * 0.25f;
-        *reinterpret_cast<uint2*>(o3 + (size_t)(c >> 1) * (wd / 8)) = make_uint2(pack_h2(l3f[0], l3f[1]), pack_h2(l3f[2], l3f[3]));
-      } else {
+          for (int k = 0; k < 4; k++) w[k] = pack_h2(l1[2 * k], l1[2 * k + 1]);
+          quad_transpose(w, r, lane);                                  // lane qd: columns 8 qd + {0..3} (low halves), 8 qd + 4 + {0..3} (high)
+          const uint4 v = make_uint4(__byte_perm(r[0], r[1], 0x5410), __byte_perm(r[2], r[3], 0x5410), __byte_perm(r[0], r[1], 0x7632),
+                                     __byte_perm(r[2], r[3], 0x7632));
+          __half* dst = p.tiled ? p.out1 + rowoff[i] * (size_t)(p.HW / 4) + ((size_t)(c >> 1) * 4 + qd) * 32 + (2 * (c & 1) + h) * 8
+                                : p.out1 + rowoff[i] * (size_t)(p.HW / 4) + (size_t)(2 * c + h) * (wd / 2) + qd * 8;
+          *reinterpret_cast<uint4*>(dst) = v;
+        }
+        if (h == 0) {
 #pragma unroll
-        for (int k = 0; k < 8; k++) l2prev[k] = l2f[k];
+          for (int gx = 0; gx < 8; gx++) l1h0[i][gx] = l1[gx];
+          continue;
+        }
+        // level 2 row c: column 2 gx + qd / 2 (lanes qd, qd ^ 1 hold the same value)
+        float l2[8], ot[8];
+#pragma unroll
+        for (int gx = 0; gx < 8; gx++) {
+          const float s0 = l1h0[i][gx] + __shfl_xor_sync(0xffffffffu, l1h0[i][gx], 1);
+          const float s1 = l1[gx] + __shfl_xor_sync(0xffffffffu, l1[gx], 1);
+          l2[gx] = (s0 + s1) * 0.25f;
+        }
+#pragma unroll
+        for (int gx = 0; gx < 8; gx++) ot[gx] = __shfl_xor_sync(0xffffffffu, l2[gx], 2);
+        if (qd == 0)
+          *reinterpret_cast<uint4*>(p.out2 + rowoff[i] * (size_t)(p.HW / 16) + (size_t)c * (wd / 4)) =
+              make_uint4(pack_h2(l2[0], ot[0]), pack_h2(l2[1], ot[1]), pack_h2(l2[2], ot[2]), pack_h2(l2[3], ot[3]));
+        else if (qd == 2)
+          *reinterpret_cast<uint4*>(p.out2 + rowoff[i] * (size_t)(p.HW / 16) + (size_t)c * (wd / 4) + 8) =
+              make_uint4(pack_h2(ot[4], l2[4]), pack_h2(ot[5], l2[5]), pack_h2(ot[6], l2[6]), pack_h2(ot[7], l2[7]));
+        if (c & 1) {   // level 3 row c/2: column gx (lanes 0 and 2 of the quad hold the two level-2 columns 2 gx, 2 gx + 1)
+          float l3[8];
+#pragma unroll
+          for (int gx = 0; gx < 8; gx++) {
+            const float a = l2prev[i][gx] + __shfl_xor_sync(0xffffffffu, l2prev[i][gx], 2);
+            const float b = l2[gx] + ot[gx];
+            l3[gx] = (a + b) * 0.25f;
+          }
+          if (qd == 0)
+            *reinterpret_cast<uint4*>(p.out3 + rowoff[i] * (size_t)(p.HW / 64) + (size_t)(c >> 1) * (wd / 8)) =
+                make_uint4(pack_h2(l3[0], l3[1]), pack_h2(l3[2], l3[3]), pack_h2(l3[4], l3[5]), pack_h2(l3[6], l3[7]));
+        } else {
+#pragma unroll
+          for (int gx = 0; gx < 8; gx++) l2prev[i][gx] = l2[gx];
+        }
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
 }
 
 // ---- host: tensor maps through the driver entry point (no link-time dependency on libcuda) ------------------------------

@@ -1,4 +1,4 @@
-// Streaming geometry ops for sm_100a: projmap, frame_distance, depth_filter, iproj.
+// Streaming geometry ops for sm_90a: projmap, frame_distance, depth_filter, iproj.
 // Replace reference src/droid_kernels.cu:436-859 (kernels) and :1447-1550 (drivers).
 // All four are HBM-streaming (4-16 B per pixel); one CTA computes the edge transform once into shared memory,
 // pixels are thread-strided so every global access is warp-coalesced, outputs are written once (no memset, and

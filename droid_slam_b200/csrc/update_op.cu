@@ -1,9 +1,9 @@
-// The update operator of DROID-SLAM (SURVEY section 8a row A6) as hand-written sm_100a kernels:
+// The update operator of DROID-SLAM (SURVEY section 8a row A6) as hand-written sm_90a kernels:
 //   UpdateModule.forward   reference droid_slam/droid_net.py:111-143  (encoders :83-93, heads :95-106)
 //   ConvGRU.forward        reference droid_slam/modules/gru.py:19-32
 //   GraphAgg.forward       reference droid_slam/droid_net.py:59-75
 //
-// Every convolution is an implicit GEMM on the 5th-generation tensor cores -- no im2col buffer, no library call:
+// Every convolution is an implicit GEMM on the Hopper tensor cores (wgmma) -- no im2col buffer, no library call:
 //   * activations live channels-last ([image, y, x, C], f16), so a tile of 128 pixels x 64 channels is a K-major operand
 //     with 128-byte rows; a 3x3 tap (dy,dx) is the same tile shifted by one pixel, which TMA delivers with the zero padding
 //     for free (cp.async.bulk.tensor.4d with out-of-bounds fill at negative / beyond-the-edge coordinates);
@@ -11,16 +11,17 @@
 //     shared-memory buffer at +dy*TW*128 bytes (a multiple of the 1024-byte swizzle atom), so a 3x3 convolution reads its
 //     input 3x (not 9x) from L2;
 //   * weights are pre-packed [tap][N][K] f16 (K contiguous) and stream through a second TMA ring;
-//   * tcgen05.mma.cta_group::1.kind::f16, M = 128 (x MT tiles sharing every weight stage), N up to 384, fp32 accumulators in
-//     TMEM; persistent CTAs (one per SM) with a static tile schedule: warp 0 = TMA producer (runs ahead across tiles),
-//     warp 1 = MMA issuer, warps 2..9 = epilogue (tcgen05.ld 32 lanes x 32 columns, thread = one output pixel);
-//     accumulators are double-buffered in TMEM whenever MT*N <= 256 so the epilogue of tile i overlaps the MMAs of tile i+1;
+//   * wgmma.m64nNk16 (f16 operands from shared memory, fp32 accumulators in registers), N = the output channels of the tile
+//     (up to 256; 384 outputs run as two 192-wide N tiles), M = 128 pixels per tile (x MT tiles sharing every weight stage);
+//     persistent CTAs (one per SM) with a static tile schedule: warp 8 = TMA producer (runs ahead across tiles), warps 0..7 =
+//     two consumer warpgroups, warpgroup w computing pixels 64 w .. 64 w + 63 of every M tile and running its own epilogue
+//     straight from the register fragment while the producer already streams the next tile's operands;
 //   * the epilogues fuse everything elementwise: bias, ReLU, the GRU gates (z, r*h, tanh, (1-z)h + zq), the gated global
 //     context sum, sigmoid / softplus of the heads and the NCHW layout of the upsampling mask.
 // Segment mean (GraphAgg's scatter_mean), the 7x7 flow encoder's im2col (4 input channels: 49 taps x 4 = one 196-wide K),
 // the global-context mat-vec and the NCHW -> channels-last transposes are small SIMT kernels around it.
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <string.h>
 #include <stdlib.h>
@@ -29,8 +30,8 @@ namespace dba {
 
 enum { EPI_STORE = 0, EPI_GATE = 1, EPI_ZR = 2, EPI_Q = 3, EPI_F32 = 4, EPI_NCHW = 5 };
 
-constexpr int kUpThreads = 320;   // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr bool kPairDefault = false;   // cta_group::2 kernel by default
+constexpr int kUpThreads = 288;   // warps 0..7 two consumer warpgroups, warp 8 TMA
+constexpr int kSlotsPerMTile = 8;  // EPI_GATE partial-sum slots per 128-pixel M tile (one per consumer warp)
 
 struct ConvParams {
   int E, HT, WD;                    // images (edges or frames), image height / width
@@ -38,18 +39,17 @@ struct ConvParams {
   int tiles_x, tiles_y, n_ntiles;   // CTA tiles per image, N tiles (output-channel blocks)
   int KS;                           // kernel size 1 or 3
   int nk0, nk1;                     // 64-channel K blocks taken from source 0 / source 1
-  int N;                            // accumulator columns per M tile
+  int N;                            // output channels per N tile (<= 256)
   int w_rows;                       // rows per tap of the packed weight tensor (0: n_ntiles * N); larger when only the first N rows are used
   int boxn;                         // weight rows per TMA box
   int a_stages, b_stages, a_bytes, b_bytes;
-  int nbuf;                         // TMEM accumulator buffers (2 when MT * N <= 256)
   const float* bias;                // [n_ntiles * N]
   int relu;
   __half* out; int out_stride;      // EPI_STORE / EPI_Q: channels-last f16, out[pix * out_stride + n]
   const __half* h; int h_stride;    // hidden state, channels-last (EPI_GATE, EPI_ZR, EPI_Q)
   const float* glo;                 // [E][384] global-context terms: z | r | q
   __half* z; __half* rh;            // EPI_ZR outputs [pix][128]; EPI_Q reads z
-  float* partial; int slots;        // EPI_GATE: [E][slots][128] column sums of sigmoid(.) * h over 32-pixel groups
+  float* partial; int slots;        // EPI_GATE: [E][slots][128] column sums of sigmoid(.) * h over 16-pixel groups
   float* f32a; int f32_cols, f32_stride;      // EPI_F32: f32 out[pix * f32_stride + n] for n < f32_cols (per-tap partial sums of the narrow heads)
   __half* nchw; int nchw_C;         // EPI_NCHW: out[(img * nchw_C + n) * HT*WD + pixel]
 };
@@ -62,17 +62,6 @@ __device__ __forceinline__ void tma_load_3d_w(void* smem_dst, const CUtensorMap*
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// instruction descriptor: D = f32, A = B = f16, both K-major
-__device__ __forceinline__ uint32_t umma_idesc_f16_kk(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
@@ -81,145 +70,89 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
 }
 __device__ __forceinline__ float2 unpack2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
 
-// 32 consecutive f16 (64 bytes) of one pixel row
-__device__ __forceinline__ void load32h(const __half* p, float (&f)[32]) {
-  const uint4* q = reinterpret_cast<const uint4*>(p);
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    const uint4 u = __ldg(q + i);
-    float2 a = unpack2(u.x), b = unpack2(u.y), c = unpack2(u.z), d = unpack2(u.w);
-    f[8 * i + 0] = a.x; f[8 * i + 1] = a.y; f[8 * i + 2] = b.x; f[8 * i + 3] = b.y;
-    f[8 * i + 4] = c.x; f[8 * i + 5] = c.y; f[8 * i + 6] = d.x; f[8 * i + 7] = d.y;
-  }
-}
-__device__ __forceinline__ void store32h(__half* p, const float (&f)[32]) {
-  uint4* q = reinterpret_cast<uint4*>(p);
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-    q[i] = make_uint4(pack2(f[8 * i], f[8 * i + 1]), pack2(f[8 * i + 2], f[8 * i + 3]), pack2(f[8 * i + 4], f[8 * i + 5]), pack2(f[8 * i + 6], f[8 * i + 7]));
-}
+__device__ __forceinline__ float2 ldh2(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
 
-// column sums over the 32 lanes of a warp: on return lane l holds sum_lanes v[l] (31 shuffles instead of 160)
-__device__ __forceinline__ float warp_column_sums(float (&v)[32], int lane) {
-#pragma unroll
-  for (int j = 0; j < 16; j++) {
-    const bool up = lane & 16;
-    const float send = up ? v[j] : v[j + 16];
-    const float keep = up ? v[j + 16] : v[j];
-    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-  }
-#pragma unroll
-  for (int j = 0; j < 8; j++) {
-    const bool up = lane & 8;
-    const float send = up ? v[j] : v[j + 8];
-    const float keep = up ? v[j + 8] : v[j];
-    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-  }
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    const bool up = lane & 4;
-    const float send = up ? v[j] : v[j + 4];
-    const float keep = up ? v[j + 4] : v[j];
-    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-  }
-#pragma unroll
-  for (int j = 0; j < 2; j++) {
-    const bool up = lane & 2;
-    const float send = up ? v[j] : v[j + 2];
-    const float keep = up ? v[j + 2] : v[j];
-    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  }
-  {
-    const bool up = lane & 1;
-    const float send = up ? v[0] : v[1];
-    const float keep = up ? v[1] : v[0];
-    v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
-  }
-  return v[0];
-}
+// M tiles per CTA tile a consumer warpgroup can hold in registers: MT * N / 2 <= 128 fp32 accumulators per thread
+constexpr int conv_max_mt(int nw) { return 256 / nw < 4 ? 256 / nw : 4; }
 
-// epilogue of one CTA tile (MT x 128 pixels x this warp's column range) out of the TMEM accumulator buffer `buf`; `store` = false
-// for the duplicated tile a CTA pair computes when the tile count is odd (everything is computed, nothing is written)
-template <int EPI>
-__device__ __forceinline__ void conv_epilogue_tile(const ConvParams& p, uint32_t tmem_base, uint32_t buf, int q, int lane, int c_begin, int c_end, int my, int mx,
-                                                   int nt, int e, int ty, int tx, bool store) {
-  for (int t = 0; t < p.MT; t++) {
+// epilogue of one 64-pixel x N fragment (M tile t of the CTA tile) of consumer warpgroup wg: this thread holds pixels r, r + 8
+// (r = 16 (warp % 4) + lane / 4) and columns 8 j + 2 (lane % 4) + {0, 1}
+template <int EPI, int NW>
+__device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (&acc)[NW / 2], int t, int wg, int warp, int lane, int nt, int e, int ty,
+                                              int tx) {
+  const int qd = lane & 3;
+  const float* bias = p.bias + nt * p.N;
+  float csum[NW / 4];                                                  // EPI_GATE: per-column sums over this thread's two pixels
+#pragma unroll
+  for (int i = 0; i < 2; i++) {
+    const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+    const int my = m / p.TW, mx = m - my * p.TW;
     const int y = ty * (p.MT * p.RM) + t * p.RM + my, x = tx * p.TW + mx;
-    const bool valid = store && y < p.HT && x < p.WD;
+    const bool valid = y < p.HT && x < p.WD;
     const size_t pix = ((size_t)e * p.HT + (valid ? y : 0)) * p.WD + (valid ? x : 0);
-    for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-      uint32_t raw[32];
-      tmem_ld32(tmem_base + buf * 256 + t * p.N + c0 + ((uint32_t)(q * 32) << 16), raw);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      float v[32];
-      const float* bias = p.bias + nt * p.N + c0;
 #pragma unroll
-      for (int j = 0; j < 32; j++) v[j] = __uint_as_float(raw[j]) + __ldg(bias + j);
-
+    for (int j = 0; j < NW / 8; j++) {
+      const int c = 8 * j + 2 * qd;
+      float v0 = acc[4 * j + 2 * i] + __ldg(bias + c), v1 = acc[4 * j + 2 * i + 1] + __ldg(bias + c + 1);
       if (EPI == EPI_STORE) {
-        if (p.relu) {
-#pragma unroll
-          for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j], 0.f);
-        }
-        if (valid) store32h(p.out + pix * p.out_stride + c0, v);
+        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + nt * p.N + c) = pack2(v0, v1);
       } else if (EPI == EPI_GATE) {
-        float hh[32];
-        if (valid) load32h(p.h + pix * p.h_stride + c0, hh);
-#pragma unroll
-        for (int j = 0; j < 32; j++) v[j] = valid ? sigmoid_fast(v[j]) * hh[j] : 0.f;
-        const float s = warp_column_sums(v, lane);
-        const int slot = ((ty * p.tiles_x + tx) * p.MT + t) * 4 + q;
-        if (store) p.partial[((size_t)e * p.slots + slot) * 128 + c0 + lane] = s;
+        float g0 = 0.f, g1 = 0.f;
+        if (valid) { const float2 hh = ldh2(p.h + pix * p.h_stride + c); g0 = sigmoid_fast(v0) * hh.x; g1 = sigmoid_fast(v1) * hh.y; }
+        if (i == 0) { csum[2 * j] = g0; csum[2 * j + 1] = g1; }
+        else { csum[2 * j] += g0; csum[2 * j + 1] += g1; }
       } else if (EPI == EPI_ZR) {
-        const float* g = p.glo + (size_t)e * 384 + c0;
-#pragma unroll
-        for (int j = 0; j < 32; j++) v[j] = sigmoid_fast(v[j] + __ldg(g + j));
-        if (c0 < 128) {
-          if (valid) store32h(p.z + pix * 128 + c0, v);
-        } else {
-          float hh[32];
-          if (valid) {
-            load32h(p.h + pix * p.h_stride + (c0 - 128), hh);
-#pragma unroll
-            for (int j = 0; j < 32; j++) v[j] *= hh[j];
-            store32h(p.rh + pix * 128 + (c0 - 128), v);
+        const float* g = p.glo + (size_t)e * 384 + c;
+        v0 = sigmoid_fast(v0 + __ldg(g)); v1 = sigmoid_fast(v1 + __ldg(g + 1));
+        if (valid) {
+          if (c < 128) {
+            *reinterpret_cast<uint32_t*>(p.z + pix * 128 + c) = pack2(v0, v1);
+          } else {
+            const float2 hh = ldh2(p.h + pix * p.h_stride + (c - 128));
+            *reinterpret_cast<uint32_t*>(p.rh + pix * 128 + (c - 128)) = pack2(v0 * hh.x, v1 * hh.y);
           }
         }
       } else if (EPI == EPI_Q) {
-        const float* g = p.glo + (size_t)e * 384 + 256 + c0;
+        const float* g = p.glo + (size_t)e * 384 + 256 + c;
         if (valid) {
-          float hh[32], zz[32];
-          load32h(p.h + pix * p.h_stride + c0, hh);
-          load32h(p.z + pix * 128 + c0, zz);
-#pragma unroll
-          for (int j = 0; j < 32; j++) {
-            const float qq = tanh_fast(v[j] + __ldg(g + j));
-            v[j] = (1.f - zz[j]) * hh[j] + zz[j] * qq;
-          }
-          store32h(p.out + pix * p.out_stride + c0, v);
+          const float2 hh = ldh2(p.h + pix * p.h_stride + c), zz = ldh2(p.z + pix * 128 + c);
+          const float q0 = tanh_fast(v0 + __ldg(g)), q1 = tanh_fast(v1 + __ldg(g + 1));
+          *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack2((1.f - zz.x) * hh.x + zz.x * q0, (1.f - zz.y) * hh.y + zz.y * q1);
         }
       } else if (EPI == EPI_F32) {
-        if (valid) {
-          float* o = p.f32a + pix * p.f32_stride + c0;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            if (c0 + j < p.f32_cols) *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);     // f32_cols, f32_stride: multiples of 4
-        }
+        if (valid && c < p.f32_cols) *reinterpret_cast<float2*>(p.f32a + pix * p.f32_stride + c) = make_float2(v0, v1);   // f32_cols even
       } else if (EPI == EPI_NCHW) {
         if (valid) {
           const size_t HW = (size_t)p.HT * p.WD;
-          __half* o = p.nchw + ((size_t)e * p.nchw_C + nt * p.N + c0) * HW + (size_t)y * p.WD + x;
-#pragma unroll
-          for (int j = 0; j < 32; j++) o[j * HW] = __float2half_rn(v[j]);
+          __half* o = p.nchw + ((size_t)e * p.nchw_C + nt * p.N + c) * HW + (size_t)y * p.WD + x;
+          o[0] = __float2half_rn(v0);
+          o[HW] = __float2half_rn(v1);
         }
       }
     }
   }
+  if (EPI == EPI_GATE) {
+    // column sums over the warp's 16 pixels (lanes with equal lane % 4 hold the same columns), one slot per warp and M tile
+#pragma unroll
+    for (int k = 0; k < NW / 4; k++) {
+      csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 4);
+      csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 8);
+      csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 16);
+    }
+    if (lane < 4) {
+      const int slot = ((ty * p.tiles_x + tx) * p.MT + t) * kSlotsPerMTile + wg * 4 + (warp & 3);
+      float* dst = p.partial + ((size_t)e * p.slots + slot) * 128;
+#pragma unroll
+      for (int j = 0; j < NW / 8; j++) *reinterpret_cast<float2*>(dst + 8 * j + 2 * qd) = make_float2(csum[2 * j], csum[2 * j + 1]);
+    }
+  }
 }
 
-template <int EPI>
+template <int EPI, int NW>
 __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                                                                const __grid_constant__ CUtensorMap tmW, const ConvParams p) {
+  constexpr int kMT = conv_max_mt(NW);
   extern __shared__ uint8_t up_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(up_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = smem;
@@ -229,9 +162,6 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
   uint64_t* a_empty = bars + 4;         // [4]
   uint64_t* b_full = bars + 8;          // [8]
   uint64_t* b_empty = bars + 16;        // [8]
-  uint64_t* tmem_full = bars + 24;      // [2]
-  uint64_t* tmem_empty = bars + 26;     // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 28);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
@@ -240,21 +170,13 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
   const int pad = p.KS >> 1;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.a_stages; s++) { mbar_init(a_full + s, 1); mbar_init(a_empty + s, 1); }
-    for (int s = 0; s < p.b_stages; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, 1); }
-    for (int s = 0; s < 2; s++) { mbar_init(tmem_full + s, 1); mbar_init(tmem_empty + s, 8); }
+    for (int s = 0; s < p.a_stages; s++) { mbar_init(a_full + s, 1); mbar_init(a_empty + s, 8); }
+    for (int s = 0; s < p.b_stages; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_base_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ================= TMA producer (one thread) =================
     if (lane == 0) {
       uint32_t ac = 0, bc = 0;
@@ -286,283 +208,69 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    const int n_c0 = p.N > 256 ? 256 : p.N, n_c1 = p.N - n_c0;
-    const uint32_t idesc0 = umma_idesc_f16_kk(128, n_c0);
-    const uint32_t idesc1 = n_c1 ? umma_idesc_f16_kk(128, n_c1) : 0u;
-    const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-    uint32_t ac = 0, bc = 0, it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it++) {
-      const uint32_t buf = it % p.nbuf;
-      mbar_wait(tmem_empty + buf, ((it / p.nbuf) & 1) ^ 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tcol = tmem_base + buf * 256;
-      bool first = true;
-      for (int kb = 0; kb < nk; kb++) {
-        for (int dx = 0; dx < p.KS; dx++) {
-          const int as = ac % p.a_stages;
-          mbar_wait(a_full + as, (ac / p.a_stages) & 1);
-          for (int dy = 0; dy < p.KS; dy++) {
-            const int bs = bc % p.b_stages;
-            mbar_wait(b_full + bs, (bc / p.b_stages) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (lane == 0) {
-              const uint32_t b_base = sB_u + bs * p.b_bytes;
-              for (int t = 0; t < p.MT; t++) {
-                const uint32_t a_base = sA_u + as * p.a_bytes + (uint32_t)((t * p.RM + dy) * p.TW) * 128u;
+    return;
+  }
+  // ================= consumers: warpgroup wg = pixels 64 wg .. 64 wg + 63 of every M tile =================
+  // A stage is released (one arrival per warp) when the wgmma batch after the last one reading it has been issued and the
+  // batch reading it has completed (wgmma.wait_group 1), so one batch is always in flight.
+  const int wg = warp >> 2;
+  const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
+  float acc[kMT][NW / 2];
+  uint32_t ac = 0, bc = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int nt = tile / (p.E * tiles_per_img);
+    const int r0 = tile - nt * (p.E * tiles_per_img);
+    const int e = r0 / tiles_per_img;
+    const int r1 = r0 - e * tiles_per_img;
+    const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
+    bool first = true;
+    int pend_a = -1, pend_b = -1;
+    for (int kb = 0; kb < nk; kb++) {
+      for (int dx = 0; dx < p.KS; dx++) {
+        const int as = ac % p.a_stages;
+        mbar_wait(a_full + as, (ac / p.a_stages) & 1);
+        for (int dy = 0; dy < p.KS; dy++) {
+          const int bs = bc % p.b_stages;
+          mbar_wait(b_full + bs, (bc / p.b_stages) & 1);
+          const uint32_t b_base = sB_u + bs * p.b_bytes;
+          wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 4; k++) {
-                  const uint32_t acc = (first && k == 0) ? 0u : 1u;
-                  const uint64_t ad = umma_desc_k_sw128(a_base + k * 32, 1024);
-                  umma_f16_ss(tcol + t * p.N, ad, umma_desc_k_sw128(b_base + k * 32, 1024), idesc0, acc);
-                  if (n_c1) umma_f16_ss(tcol + t * p.N + 256, ad, umma_desc_k_sw128(b_base + 256 * 128 + k * 32, 1024), idesc1, acc);
-                }
-              }
-              umma_commit(b_empty + bs);
+          for (int t = 0; t < kMT; t++) {
+            if (t < p.MT) {
+              const uint32_t a_base = sA_u + as * p.a_bytes + (uint32_t)((t * p.RM + dy) * p.TW + wg * 64) * 128u;
+#pragma unroll
+              for (int k = 0; k < 4; k++)
+                wgmma_f16<NW>(acc[t], gmma_desc_sw128(a_base + k * 32, 16, 1024), gmma_desc_sw128(b_base + k * 32, 16, 1024), (first && k == 0) ? 0 : 1, 0);
             }
-            __syncwarp();
-            first = false;
-            bc++;
           }
-          if (lane == 0) umma_commit(a_empty + as);
+          wgmma_commit();
+          wgmma_wait<1>();
           __syncwarp();
-          ac++;
+          if (lane == 0) {
+            if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
+            if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
+          }
+          pend_a = -1;
+          pend_b = bs;
+          first = false;
+          bc++;
         }
+        pend_a = as;
+        ac++;
       }
-      if (lane == 0) umma_commit(tmem_full + buf);
-      __syncwarp();
     }
-  } else {
-    // ================= epilogue: warps 2..9; TMEM lane quarter q = warp % 4, the two warps of a quarter split the columns =================
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int cols_per_half = p.N >= 64 ? p.N / 2 : p.N;
-    const int c_begin = half * cols_per_half;
-    const int c_end = (p.N >= 64 || half == 0) ? c_begin + cols_per_half : c_begin;
-    const int m = q * 32 + lane;
-    const int my = m / p.TW, mx = m - my * p.TW;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, it++) {
-      const int nt = tile / (p.E * tiles_per_img);
-      const int r0 = tile - nt * (p.E * tiles_per_img);
-      const int e = r0 / tiles_per_img;
-      const int r1 = r0 - e * tiles_per_img;
-      const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
-      const uint32_t buf = it % p.nbuf;
-      mbar_wait(tmem_full + buf, (it / p.nbuf) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      conv_epilogue_tile<EPI>(p, tmem_base, buf, q, lane, c_begin, c_end, my, mx, nt, e, ty, tx, true);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty + buf);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): two CTAs of a cluster (one SM pair) work on two CTA tiles at once and SHARE every weight
-// stage -- each CTA loads only half of the N weight rows, the pair-wide MMA (M = 256: CTA 0's 128 pixels + CTA 1's 128 pixels,
-// N = all output channels) reads both halves.  Per MMA a CTA's tensor core now fetches 4 KB of A + half of B from shared memory
-// instead of all of B (the single-CTA form is shared-memory-operand bound: 128 B/clk at N = 128), and the L2 -> SM weight traffic
-// per MAC halves.  The leader CTA (rank 0) issues all MMAs; both CTAs run their own TMA producer and their own epilogue on their
-// own TMEM lanes.  Barrier protocol (the usual 2-SM pipeline): "full" barriers live in the leader and collect both CTAs' loads
-// (the peer's TMA signals the leader's barrier; count 2 = leader arrive.expect_tx + peer arrive), "empty" / "tmem_full" barriers
-// live in each CTA and are released by one multicast tcgen05.commit, "tmem_empty" lives in the leader and collects all 16
-// epilogue warps.
-// ---------------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank)); return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma2_load_3d(void* smem_dst, const CUtensorMap* map, uint32_t bar_cluster_addr, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar) {      // arrive on this barrier in BOTH CTAs of the pair when the MMAs issued so far are done
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma2_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-template <int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kUpThreads, 1) conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                                                                                         const __grid_constant__ CUtensorMap tmW, const ConvParams p) {
-  extern __shared__ uint8_t up_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(up_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + p.a_stages * p.a_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + p.b_stages * p.b_bytes);       // b_bytes = this CTA's half of a weight stage
-  uint64_t* a_full = bars;              // [4]  used in the leader
-  uint64_t* a_empty = bars + 4;         // [4]
-  uint64_t* b_full = bars + 8;          // [8]  used in the leader
-  uint64_t* b_empty = bars + 16;        // [8]
-  uint64_t* tmem_full = bars + 24;      // [2]
-  uint64_t* tmem_empty = bars + 26;     // [2]  used in the leader
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 28);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
-  const int tpn = p.E * tiles_per_img;                 // CTA tiles per N tile
-  const int ppn = (tpn + 1) >> 1;                      // pair tiles per N tile
-  const int total_pairs = p.n_ntiles * ppn;
-  const int npairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
-  const int nk = p.nk0 + p.nk1;
-  const int pad = p.KS >> 1;
-  const int n_c0 = p.N > 256 ? 256 : p.N, n_c1 = p.N - n_c0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.a_stages; s++) { mbar_init(a_full + s, 2); mbar_init(a_empty + s, 1); }
-    for (int s = 0; s < p.b_stages; s++) { mbar_init(b_full + s, 2); mbar_init(b_empty + s, 1); }
-    for (int s = 0; s < 2; s++) { mbar_init(tmem_full + s, 1); mbar_init(tmem_empty + s, 16); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_base_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  cluster_sync_all();                                   // barriers of both CTAs initialised, TMEM of both allocated
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_base_smem;
-
-  if (warp == 0) {
-    // ================= TMA producer (one thread per CTA): own halo tiles, own half of the weight rows =================
+    wgmma_wait<0>();
+    __syncwarp();
     if (lane == 0) {
-      uint32_t ac = 0, bc = 0;
-      const int h0 = n_c0 >> 1, h1 = n_c1 >> 1;          // this CTA's rows of the two N chunks
-      for (int T = pair; T < total_pairs; T += npairs) {
-        const int nt = T / ppn;
-        int r0 = 2 * (T - nt * ppn) + (int)rank;
-        if (r0 >= tpn) r0 = tpn - 1;                     // odd tile count: the pair's second CTA recomputes the last tile (not stored)
-        const int e = r0 / tiles_per_img;
-        const int r1 = r0 - e * tiles_per_img;
-        const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
-        const int y0 = ty * (p.MT * p.RM), x0 = tx * p.TW;
-        for (int kb = 0; kb < nk; kb++) {
-          const CUtensorMap* am = kb < p.nk0 ? &tmA0 : &tmA1;
-          const int ch = (kb < p.nk0 ? kb : kb - p.nk0) * 64;
-          for (int dx = 0; dx < p.KS; dx++) {
-            const int as = ac % p.a_stages;
-            mbar_wait(a_empty + as, ((ac / p.a_stages) & 1) ^ 1);
-            const uint32_t fa = mapa_rank(smem_u32(a_full + as), 0);
-            tma2_load_4d(sA + as * p.a_bytes, am, fa, ch, x0 + dx - pad, y0 - pad, e);
-            if (leader) mbar_expect_tx(a_full + as, 2 * p.a_bytes); else mbar_arrive_cluster(fa);
-            ac++;
-            for (int dy = 0; dy < p.KS; dy++) {
-              const int bs = bc % p.b_stages;
-              mbar_wait(b_empty + bs, ((bc / p.b_stages) & 1) ^ 1);
-              const uint32_t fb = mapa_rank(smem_u32(b_full + bs), 0);
-              uint8_t* dstb = sB + bs * p.b_bytes;
-              const int tap = dy * p.KS + dx;
-              for (int n = 0; n < h0; n += p.boxn) tma2_load_3d(dstb + n * 128, &tmW, fb, kb * 64, nt * p.N + (int)rank * h0 + n, tap);
-              for (int n = 0; n < h1; n += p.boxn) tma2_load_3d(dstb + (h0 + n) * 128, &tmW, fb, kb * 64, nt * p.N + n_c0 + (int)rank * h1 + n, tap);
-              if (leader) mbar_expect_tx(b_full + bs, 2 * p.b_bytes); else mbar_arrive_cluster(fb);
-              bc++;
-            }
-          }
-        }
-      }
+      if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
+      if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer: leader CTA only, M = 256 across the pair =================
-    if (leader) {
-      const uint32_t idesc0 = umma_idesc_f16_kk(256, n_c0);
-      const uint32_t idesc1 = n_c1 ? umma_idesc_f16_kk(256, n_c1) : 0u;
-      const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-      uint32_t ac = 0, bc = 0, it = 0;
-      for (int T = pair; T < total_pairs; T += npairs, it++) {
-        const uint32_t buf = it % p.nbuf;
-        mbar_wait(tmem_empty + buf, ((it / p.nbuf) & 1) ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tcol = tmem_base + buf * 256;
-        bool first = true;
-        for (int kb = 0; kb < nk; kb++) {
-          for (int dx = 0; dx < p.KS; dx++) {
-            const int as = ac % p.a_stages;
-            mbar_wait(a_full + as, (ac / p.a_stages) & 1);
-            for (int dy = 0; dy < p.KS; dy++) {
-              const int bs = bc % p.b_stages;
-              mbar_wait(b_full + bs, (bc / p.b_stages) & 1);
-              asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-              if (lane == 0) {
-                const uint32_t b_base = sB_u + bs * p.b_bytes;
-                for (int t = 0; t < p.MT; t++) {
-                  const uint32_t a_base = sA_u + as * p.a_bytes + (uint32_t)((t * p.RM + dy) * p.TW) * 128u;
 #pragma unroll
-                  for (int k = 0; k < 4; k++) {
-                    const uint32_t acc = (first && k == 0) ? 0u : 1u;
-                    const uint64_t ad = umma_desc_k_sw128(a_base + k * 32, 1024);
-                    umma2_f16_ss(tcol + t * p.N, ad, umma_desc_k_sw128(b_base + k * 32, 1024), idesc0, acc);
-                    if (n_c1) umma2_f16_ss(tcol + t * p.N + 256, ad, umma_desc_k_sw128(b_base + (n_c0 >> 1) * 128 + k * 32, 1024), idesc1, acc);
-                  }
-                }
-                umma2_commit_mc(b_empty + bs);
-              }
-              __syncwarp();
-              first = false;
-              bc++;
-            }
-            if (lane == 0) umma2_commit_mc(a_empty + as);
-            __syncwarp();
-            ac++;
-          }
-        }
-        if (lane == 0) umma2_commit_mc(tmem_full + buf);
-        __syncwarp();
-      }
-    }
-  } else {
-    // ================= epilogue: every CTA drains its own 128 TMEM lanes =================
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int cols_per_half = p.N >= 64 ? p.N / 2 : p.N;
-    const int c_begin = half * cols_per_half;
-    const int c_end = (p.N >= 64 || half == 0) ? c_begin + cols_per_half : c_begin;
-    const int m = q * 32 + lane;
-    const int my = m / p.TW, mx = m - my * p.TW;
-    uint32_t it = 0;
-    for (int T = pair; T < total_pairs; T += npairs, it++) {
-      const int nt = T / ppn;
-      int r0 = 2 * (T - nt * ppn) + (int)rank;
-      const bool store = r0 < tpn;
-      if (!store) r0 = tpn - 1;
-      const int e = r0 / tiles_per_img;
-      const int r1 = r0 - e * tiles_per_img;
-      const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
-      const uint32_t buf = it % p.nbuf;
-      mbar_wait(tmem_full + buf, (it / p.nbuf) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      conv_epilogue_tile<EPI>(p, tmem_base, buf, q, lane, c_begin, c_end, my, mx, nt, e, ty, tx, store);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(mapa_rank(smem_u32(tmem_empty + buf), 0));
+    for (int t = 0; t < kMT; t++) {
+      wgmma_fence_regs(acc[t]);
+      if (t < p.MT) conv_epilogue<EPI, NW>(p, acc[t], t, wg, warp, lane, nt, e, ty, tx);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  cluster_sync_all();                                   // nobody leaves while the peer may still read its shared memory / signal its barriers
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -793,6 +501,29 @@ struct ConvSrc { const void* base; int C; int stride; };
 
 static int g_num_sms = 0;
 
+template <int EPI>
+constexpr bool conv_width_used(int nw) {
+  return EPI == EPI_STORE || (EPI == EPI_GATE && nw == 128) || (EPI == EPI_ZR && nw == 256) || (EPI == EPI_Q && nw == 128) ||
+         (EPI == EPI_F32 && (nw == 32 || nw == 64)) || (EPI == EPI_NCHW && nw == 192);
+}
+
+template <int EPI, int NW>
+static int launch_conv_nw(const ConvParams& p, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tW, int grid, int smem, cudaStream_t st) {
+  if constexpr (!conv_width_used<EPI>(NW)) {
+    set_error("update operator: no convolution kernel for this epilogue with %d output channels", NW);
+    return DBA_ERR_INVALID;
+  } else {
+    static bool attr_set = false;
+    if (!attr_set) {
+      DBA_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<EPI, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), "conv_tc smem attr");
+      attr_set = true;
+    }
+    conv_tc_kernel<EPI, NW><<<grid, kUpThreads, smem, st>>>(tA0, tA1, tW, p);
+    DBA_CHECK_LAUNCH("conv_tc_kernel");
+    return DBA_OK;
+  }
+}
+
 // one convolution launch.  src0 (+ optional src1) = channels-last sources concatenated along K; wpk = packed weights
 // [KS*KS][n_ntiles*N][Kpad] with Kpad = 64 * (kblocks(src0) + kblocks(src1)).
 template <int EPI>
@@ -802,30 +533,31 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
     cudaDeviceProp prop; DBA_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties");
     g_num_sms = prop.multiProcessorCount;
   }
+  if (p.N > 256) {                // 384 outputs: two 192-wide N tiles (the register accumulator holds at most 256 columns)
+    if (p.w_rows == 0) p.w_rows = p.n_ntiles * p.N;
+    p.n_ntiles *= p.N / 192;
+    p.N = 192;
+  }
+  if (p.N % 32 != 0 || p.N < 32) { set_error("update operator: %d output channels per tile", p.N); return DBA_ERR_INVALID; }
   p.TW = (p.WD % 64 == 0) ? 64 : 32;
   p.RM = 128 / p.TW;
   // M tiles per CTA tile: every weight stage is shared by MT tiles (and every halo row by 3 taps), so larger is better for the
-  // L2 -> SM traffic per MAC; bounded by TMEM (MT * N <= 512 columns) and by the image height
-  p.MT = (p.N <= 256 && p.HT >= 2 * p.RM) ? 2 : 1;
-  // N <= 128 with a long K loop (the q convolution): 4 tiles per weight stage beat the overlapped epilogue of 2 (measured:
-  // profiles/r2_conv_pipeline_experiments.txt); short K loops keep the double-buffered accumulators
-  if (p.N <= 128 && p.HT >= 4 * p.RM && (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0) >= 4 && p.KS == 3) p.MT = 4;
+  // L2 -> SM traffic per MAC; bounded by the register accumulators (MT * N <= 256 columns) and by the image height
+  p.MT = (p.HT >= 2 * p.RM) ? 2 : 1;
+  if (p.N <= 64 && p.HT >= 4 * p.RM && (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0) >= 4 && p.KS == 3) p.MT = 4;
   static const int ov_mt = getenv("DBA_CONV_MT") ? atoi(getenv("DBA_CONV_MT")) : 0;          // experiment switches (tools/conv_bench.py)
   static const int ov_as = getenv("DBA_CONV_ASTAGES") ? atoi(getenv("DBA_CONV_ASTAGES")) : 0;
   static const int ov_bs = getenv("DBA_CONV_BSTAGES") ? atoi(getenv("DBA_CONV_BSTAGES")) : 0;
-  if (ov_mt > 0 && ov_mt * p.N <= 512 && ov_mt <= 4) p.MT = ov_mt;
+  if (ov_mt > 0) p.MT = ov_mt;
+  if (p.MT > conv_max_mt(p.N)) p.MT = conv_max_mt(p.N);
   p.tiles_x = (p.WD + p.TW - 1) / p.TW;
   p.tiles_y = (p.HT + p.MT * p.RM - 1) / (p.MT * p.RM);
   p.nk0 = (s0.C + 63) / 64;
   p.nk1 = s1.base ? (s1.C + 63) / 64 : 0;
-  // CTA pairs (cta_group::2) share every weight stage: each CTA holds half of the N rows (DBA_CONV_2CTA=0 selects the single-CTA kernel)
-  static const int ov_pair = getenv("DBA_CONV_2CTA") ? atoi(getenv("DBA_CONV_2CTA")) : -1;
-  const bool use_pair = (ov_pair < 0 ? kPairDefault : ov_pair != 0) && (p.N % 32 == 0) && g_num_sms >= 2;
-  p.boxn = use_pair ? (p.N <= 256 ? p.N / 2 : 64) : (p.N <= 256 ? p.N : 128);
-  p.nbuf = (p.MT * p.N <= 256) ? 2 : 1;
+  p.boxn = p.N;
   const int box_rows = p.MT * p.RM + p.KS - 1;
   p.a_bytes = box_rows * p.TW * 128;
-  p.b_bytes = (use_pair ? p.N / 2 : p.N) * 128;
+  p.b_bytes = p.N * 128;
   // shared memory: at least 2 halo stages and 3 weight stages; what is left goes to more halo stages (up to 4: with narrow N the
   // MMAs of a stage are short and the TMA latency of the next halo tile is what the pipeline has to cover), then weight stages
   const int budget = 227 * 1024 - 2048;
@@ -836,7 +568,7 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   if (p.b_stages > 8) p.b_stages = 8;
   if (ov_bs > 0 && ov_bs <= 8 && p.a_stages * p.a_bytes + ov_bs * p.b_bytes <= budget) p.b_stages = ov_bs;
   if (p.b_stages < 2) { set_error("update operator: tile does not fit shared memory"); return DBA_ERR_INVALID; }
-  p.slots = p.tiles_x * p.tiles_y * p.MT * 4;
+  p.slots = p.tiles_x * p.tiles_y * p.MT * kSlotsPerMTile;
   if (slots_out) *slots_out = p.slots;
   const int smem = p.a_stages * p.a_bytes + p.b_stages * p.b_bytes + 1024 + 256;
   CUtensorMap tA0, tA1, tW;
@@ -844,26 +576,19 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   if (s1.base) { rc = make_act_map(&tA1, s1.base, s1.C, s1.stride, p.WD, p.HT, p.E, p.TW, box_rows); if (rc) return rc; }
   else tA1 = tA0;
   rc = make_weight_map(&tW, wpk, 64 * (p.nk0 + p.nk1), p.w_rows > 0 ? p.w_rows : p.n_ntiles * p.N, p.KS * p.KS, p.boxn); if (rc) return rc;
-  static int attr_set = 0;
-  if (attr_set < smem) {
-    DBA_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), "conv_tc smem attr");
-    DBA_CHECK_CUDA(cudaFuncSetAttribute(conv_tc2_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), "conv_tc2 smem attr");
-    attr_set = 227 * 1024;
-  }
   const long long total = (long long)p.n_ntiles * p.E * p.tiles_x * p.tiles_y;
   if (total <= 0) return DBA_OK;
-  if (use_pair) {
-    const long long tpn = (long long)p.E * p.tiles_x * p.tiles_y;
-    const long long pairs = (long long)p.n_ntiles * ((tpn + 1) / 2);
-    const int npairs = (int)(pairs < g_num_sms / 2 ? pairs : g_num_sms / 2);
-    conv_tc2_kernel<EPI><<<2 * npairs, kUpThreads, smem, st>>>(tA0, tA1, tW, p);
-    DBA_CHECK_LAUNCH("conv_tc2_kernel");
-    return DBA_OK;
-  }
   const int grid = (int)(total < g_num_sms ? total : g_num_sms);
-  conv_tc_kernel<EPI><<<grid, kUpThreads, smem, st>>>(tA0, tA1, tW, p);
-  DBA_CHECK_LAUNCH("conv_tc_kernel");
-  return DBA_OK;
+  switch (p.N) {
+    case 32: return launch_conv_nw<EPI, 32>(p, tA0, tA1, tW, grid, smem, st);
+    case 64: return launch_conv_nw<EPI, 64>(p, tA0, tA1, tW, grid, smem, st);
+    case 96: return launch_conv_nw<EPI, 96>(p, tA0, tA1, tW, grid, smem, st);
+    case 128: return launch_conv_nw<EPI, 128>(p, tA0, tA1, tW, grid, smem, st);
+    case 160: return launch_conv_nw<EPI, 160>(p, tA0, tA1, tW, grid, smem, st);
+    case 192: return launch_conv_nw<EPI, 192>(p, tA0, tA1, tW, grid, smem, st);
+    case 224: return launch_conv_nw<EPI, 224>(p, tA0, tA1, tW, grid, smem, st);
+    default: return launch_conv_nw<EPI, 256>(p, tA0, tA1, tW, grid, smem, st);
+  }
 }
 
 static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -875,7 +600,7 @@ static UpWs up_layout(int E, int n_src, int ht, int wd) {
   UpWs w;
   const size_t px = (size_t)E * ht * wd, spx = (size_t)(n_src > 0 ? n_src : 1) * ht * wd;
   const int tw = (wd % 64 == 0) ? 64 : 32, rm = 128 / tw;
-  const size_t slots = (size_t)((wd + tw - 1) / tw) * ((ht + rm - 1) / rm) * 4 * 2;   // upper bound over MT
+  const size_t slots = (size_t)((wd + tw - 1) / tw) * ((ht + rm - 1) / rm) * kSlotsPerMTile * 2;   // upper bound over MT
   size_t o = 0;
   w.hin = o; o += al256(px * 128 * 2);
   w.x320 = o; o += al256(px * 320 * 2);

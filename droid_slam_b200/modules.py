@@ -5,7 +5,7 @@ drop-in callables); nothing of it is restated here.  What the reference computes
 kernel for is offered as a hook:
 
   * `install_corr_volume_hook(corr_module)`: `CorrBlock.__init__` (modules/corr.py:24-38, 63-71: torch.matmul + 3x avg_pool2d) builds
-    its four pyramid levels with the one-pass tcgen05 kernel `droid_backends.corr_volume_pyramid` instead.  Only the constructor is
+    its four pyramid levels with the one-pass wgmma kernel `droid_backends.corr_volume_pyramid` instead.  Only the constructor is
     replaced; lookups, `cat` and `__getitem__` stay the reference's code.
   * `reproject(...)`: `DepthVideo.reproject` (depth_video.py:171-179 -> geom/projective_ops.py:165-198) as one kernel.
   * `add_proximity_factors(graph, ...)` / `install_proximity_hook(FactorGraph)`: the edge selection of

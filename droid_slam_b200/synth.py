@@ -16,7 +16,7 @@ CONFIGS = {
     "metric": dict(E=512, N=72, ht=48, wd=64, stereo=False, itrs=2, lm=1e-4, ep=0.1),
     "c3_global": dict(E=2048, N=400, ht=48, wd=64, stereo=False, itrs=10, lm=1e-5, ep=1e-2),
     "c4_stereo": dict(E=256, N=64, ht=48, wd=64, stereo=True, itrs=2, lm=1e-4, ep=0.1),
-    "c5_stress": dict(E=8192, N=1000, ht=72, wd=96, stereo=False, itrs=2, lm=1e-4, ep=0.1),
+    "c5_stress": dict(E=4096, N=500, ht=72, wd=96, stereo=False, itrs=2, lm=1e-4, ep=0.1),
 }
 
 

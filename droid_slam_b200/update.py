@@ -134,7 +134,7 @@ class UpdateModule(nn.Module):
 
     def forward(self, net, inp, corr, flow=None, ii=None, jj=None):
         if not net.is_cuda:
-            raise RuntimeError("droid_slam_b200.UpdateModule runs on CUDA tensors only (hand-written sm_100a kernels, no CPU path)")
+            raise RuntimeError("droid_slam_b200.UpdateModule runs on CUDA tensors only (hand-written sm_90a kernels, no CPU path)")
         from . import install
         be = install()
         batch, num, ch, ht, wd = net.shape

@@ -1,5 +1,5 @@
 /*
- * droid_b200.h -- C ABI of the B200-native (sm_100a) dense-BA update hot path of DROID-SLAM.
+ * droid_b200.h -- C ABI of the H100-native (sm_90a) dense-BA update hot path of DROID-SLAM.
  *
  * This is the drop-in boundary: every entry point takes plain device pointers, extents, a dtype code and a
  * CUDA stream, and returns an int status (0 = ok).  No torch types cross it.  The Python extension
@@ -54,7 +54,7 @@ int dba_corr_index_backward(const float* coords, const void* corr_grad, void* vo
  * replaces CorrBlock.__init__ / CorrBlock.corr (reference droid_slam/modules/corr.py:24-38,63-71: torch.matmul of the
  * /4-scaled feature maps + 3x avg_pool2d).  fmap1 [n_frames1,C,ht,wd], fmap2 [n_frames2,C,ht,wd] (f16, C = 128),
  * ii,jj [E] int64 frame indices into fmap1 / fmap2;  out_l [E,ht,wd,ht/2^l,wd/2^l] f16 for l = 0..3, fully overwritten.
- * One tcgen05/TMEM/TMA kernel writes all four levels in a single pass over the accumulator.
+ * One wgmma/TMA kernel writes all four levels in a single pass over the accumulator.
  * Implemented for wd = 64, ht % 8 == 0 (DBA_ERR_INVALID otherwise). */
 /* 1 when dba_corr_volume_pyramid has a kernel for this shape / dtype (f16, 128 channels, wd = 64, ht % 8 == 0), else 0 */
 int dba_corr_volume_supported(int channels, int ht, int wd, int dtype);
@@ -193,7 +193,7 @@ int dba_ba_read_info(const dba_ba_args* a, int* n_depth_frames, int* device_stat
 /* ---- update operator (ConvGRU + heads + GraphAgg) on the tensor cores -----------------------------------
  * replaces UpdateModule.forward (reference droid_slam/droid_net.py:111-143), ConvGRU.forward (droid_slam/modules/gru.py:19-32) and
  * GraphAgg.forward (droid_net.py:59-75) -- in the reference a chain of 19 cuDNN convolutions + ~25 elementwise launches.
- * Every convolution runs as an implicit GEMM (tcgen05 / TMEM / TMA, f16 operands, fp32 accumulation) on channels-last
+ * Every convolution runs as an implicit GEMM (wgmma / TMA, f16 operands, fp32 accumulation) on channels-last
  * activations; gates, activations, the global-context sum and output layouts are fused into the epilogues.
  *
  * Packed weights (device memory, made once per checkpoint by the host side, droid_slam_b200/update.py:pack_update_weights):

@@ -10,7 +10,7 @@ reference file:line it follows.
 
 Parity pinning: the reference ships NO golden vectors or unit tests for this path (SURVEY.md
 section 4 / 8c).  The oracle is pinned instead against the reference's own CUDA build run on a
-B200 (``oracle/build_ref.sh`` -> ``oracle/_ref/droid_backends_ref``; fixtures under
+H100 (``oracle/build_ref.sh`` -> ``oracle/_ref/droid_backends_ref``; fixtures under
 ``tests/golden/`` made by ``tests/golden/make_golden.py``) -- see DESIGN.md "Oracle pinning".
 """
 from .se3 import *      # noqa: F401,F403

@@ -1,6 +1,6 @@
 #!/usr/bin/env bash
 # Build the UNMODIFIED reference droid_backends (src/*.cu, src/droid.cpp read in place from
-# /root/reference) for sm_100a as `droid_backends_ref`, against the Eigen stand-in in
+# /root/reference) for sm_90a as `droid_backends_ref`, against the Eigen stand-in in
 # oracle/eigen_standin (Eigen itself is an absent submodule).  Output only into oracle/_ref/.
 # This is measurement/test infrastructure: the product never links or imports it.
 set -euo pipefail
@@ -20,7 +20,7 @@ NAME=droid_backends_ref
 TARGET="$OUT/$NAME$EXT"
 COMMON=(-O3 -std=c++17 -DTORCH_EXTENSION_NAME=$NAME -DTORCH_API_INCLUDE_EXTENSION_H -D_GLIBCXX_USE_CXX11_ABI=1
         -I"$HERE/eigen_standin" -I"$TORCH_INC" -I"$TORCH_INC/torch/csrc/api/include" -I"$PY_INC" -I/usr/local/cuda/include)
-NVCC=(/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC --expt-relaxed-constexpr
+NVCC=(/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC --expt-relaxed-constexpr
       -D__CUDA_NO_HALF_OPERATORS__ -D__CUDA_NO_HALF_CONVERSIONS__ -D__CUDA_NO_BFLOAT16_CONVERSIONS__ -D__CUDA_NO_HALF2_OPERATORS__)
 stale() { [ ! -f "$1" ] || [ "$2" -nt "$1" ]; }
 pids=()

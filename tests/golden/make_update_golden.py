@@ -38,6 +38,10 @@ def _stub_missing_packages():
     sys.modules.setdefault("torch_scatter", ts)
 
 
+def upmask_sample_index(n):
+    return torch.randperm(n, generator=torch.Generator().manual_seed(0))[:n // 4]
+
+
 def main(out_path):
     from droid_slam_b200 import synth
     _stub_missing_packages()
@@ -56,6 +60,9 @@ def main(out_path):
             o = mod(net, inp, corr, flow, ii)
             for k, t in zip(("net", "delta", "weight", "eta", "upmask"), o):
                 G["%s_%s" % (name, k)] = t.clone()
+            up = G.pop("%s_upmask" % name)                             # the largest output: a seeded quarter of it (file < 1 MB)
+            G["%s_upmask_shape" % name] = tuple(up.shape)
+            G["%s_upmask_sample" % name] = up.reshape(-1)[upmask_sample_index(up.numel())].clone()
             o2 = mod(net, inp, corr, None, None)                       # no flow, no aggregation
             for k, t in zip(("net", "delta", "weight"), o2):
                 G["%s_noflow_%s" % (name, k)] = t.clone()

@@ -1,5 +1,5 @@
-"""Pin the CPU oracle against outputs of the UNMODIFIED reference CUDA build run on a B200
-(tests/golden/reference_b200.pt, produced by tests/golden/make_golden.py; the reference ships no golden vectors of
+"""Pin the CPU oracle against outputs of the UNMODIFIED reference CUDA build run on an H100
+(tests/golden/reference_h100.pt, produced by tests/golden/make_golden.py; the reference ships no golden vectors of
 its own for this path, SURVEY.md section 8c)."""
 import os
 import sys
@@ -12,7 +12,7 @@ import oracle
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
 import cases  # noqa: E402
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_b200.pt")
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_h100.pt")
 
 
 @pytest.fixture(scope="module")
@@ -26,7 +26,7 @@ def _rel(a, b, floor=1.0):
 
 def test_golden_file_describes_reference(gold):
     m = gold["_meta"]
-    assert "B200" in m["gpu"] and "unmodified" in m["note"]
+    assert "H100" in m["gpu"] and "unmodified" in m["note"]
     # our kernels vs the reference on the same GPU, recorded when the file was made
     for k, v in m["ours_vs_reference"].items():
         if k.startswith(("corr_", "altcorr_", "projmap", "iproj", "depth_filter")):

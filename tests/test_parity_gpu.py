@@ -1,4 +1,4 @@
-"""GPU parity tests: the hand-written sm_100a kernels, called through the C ABI (ctypes) and through the
+"""GPU parity tests: the hand-written sm_90a kernels, called through the C ABI (ctypes) and through the
 `droid_backends` pybind surface, against the CPU oracle on the same seeded inputs.
 
 Tolerances (BASELINE.json north_star): fp32 outputs within 1e-4 relative (with an absolute floor of 1e-4*scale),
@@ -315,7 +315,7 @@ def test_cluster_cholesky_envelope_banded_systems(capi, n, band, far):
 
 # ---------------------------------------------------------------------------------------------------
 def test_corr_volume_pyramid_tcgen05_matches_reference_formula(backends):
-    """CorrBlock.__init__ (reference modules/corr.py:24-38,63-71) in one tcgen05/TMEM/TMA kernel vs matmul + avg_pool2d"""
+    """CorrBlock.__init__ (reference modules/corr.py:24-38,63-71) in one wgmma/TMA kernel vs matmul + avg_pool2d"""
     g = torch.Generator().manual_seed(31)
     N, C, ht, wd = 5, 128, 16, 64
     fmaps = torch.randn(N, C, ht, wd, generator=g).half()

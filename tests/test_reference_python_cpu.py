@@ -39,7 +39,8 @@ def test_oracle_corr_classes_match_reference_classes(gold):
     (f1, f2, coords), (fm, ca, ii, jj) = mk.corr_cases()
     pyr = oracle.corr_pyramid(f1, f2, 3)
     for l, v in enumerate(pyr):
-        assert torch.equal(v, gold["corrblock_pyr%d" % l])
+        g = gold["corrblock_pyr%d" % l]
+        assert mk.digest(v) == g if isinstance(g, str) else torch.equal(v, g), l
     assert torch.equal(oracle.corr_block_lookup(pyr, coords, 3), gold["corrblock_lookup"])
     assert torch.equal(oracle.altcorr_block_lookup(oracle.fmap_pyramid(fm, 3), ca, ii, jj, 3), gold["altcorrblock_lookup"])
 
@@ -51,7 +52,7 @@ def test_reference_python_imports_unmodified_and_reproduces_the_fixture(gold, tm
     regen = torch.load(str(out))
     assert sorted(regen.keys()) == sorted(gold.keys())
     for k in gold:
-        assert torch.equal(regen[k], gold[k]), k
+        assert (regen[k] == gold[k]) if isinstance(gold[k], str) else torch.equal(regen[k], gold[k]), k
 
 
 @pytest.mark.skipif(not REF_PRESENT, reason="reference tree not present (GPU box)")

@@ -7,6 +7,8 @@ import sys
 import pytest
 import torch
 
+import oracle
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import make_reference_python_golden as mk  # noqa: E402
@@ -54,7 +56,7 @@ class _RefShapedCorrBlock:
 def test_corrblock_lookups_match_reference_classes(backends, gold):
     """CorrBlock / AltCorrBlock results of the reference classes (oracle-backed on CPU) vs the native ops called the same way"""
     (f1, f2, coords), (fm, ca, ii, jj) = mk.corr_cases()
-    pyr = [gold["corrblock_pyr%d" % l].to(dev) for l in range(3)]
+    pyr = [v.to(dev) for v in oracle.corr_pyramid(f1, f2, 3)]          # bit-identical to the reference's (test_reference_python_cpu.py)
     c = coords.permute(0, 1, 4, 2, 3).contiguous().view(5, 2, 8, 16).to(dev)
     outs = [backends.corr_index_forward(pyr[l], (c / 2 ** l).contiguous(), 3)[0].view(1, 5, -1, 8, 16) for l in range(3)]
     assert torch.equal(torch.cat(outs, 2).cpu(), gold["corrblock_lookup"])

@@ -14,6 +14,8 @@ from droid_slam_b200.update import UpdateModule, pack_update_weights, PACKED_ORD
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from update_emul import emulate  # noqa: E402
+sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+import make_update_golden as mk  # noqa: E402
 CASES = (("a", dict(E=5, ht=6, wd=8, seed=0, n_src=3)), ("b", dict(E=7, ht=5, wd=9, seed=1, n_src=4)))
 NAMES = ("net", "delta", "weight", "eta", "upmask")
 
@@ -33,7 +35,11 @@ def test_update_oracle_matches_reference_module(gold, weights, name, kw):
     net, inp, corr, flow, ii = synth.make_update_inputs(**kw)
     out = oracle.update_module_forward(weights, net, inp, corr, flow, ii)
     for k, t in zip(NAMES, out):
-        g = gold["%s_%s" % (name, k)]
+        if k == "upmask":                                                   # stored as a seeded quarter of the elements
+            assert tuple(t.shape) == gold["%s_upmask_shape" % name]
+            t, g = t.reshape(-1)[mk.upmask_sample_index(t.numel())], gold["%s_upmask_sample" % name]
+        else:
+            g = gold["%s_%s" % (name, k)]
         assert t.shape == g.shape
         assert torch.allclose(t, g, rtol=1e-5, atol=1e-6), (k, float((t - g).abs().max()))      # observed: bit-identical
     out = oracle.update_module_forward(weights, net, inp, corr, None, None)

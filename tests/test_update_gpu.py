@@ -24,7 +24,7 @@ DEV = "cuda:0"
 
 @pytest.mark.parametrize("E,ht,wd,c0,c1,ks,n,relu", [
     (3, 16, 64, 128, 0, 3, 128, True),       # TW = 64, MT = 2, double-buffered accumulators
-    (2, 16, 64, 128, 320, 3, 256, False),    # two sources, N = 256 (single TMEM buffer)
+    (2, 16, 64, 128, 320, 3, 256, False),    # two sources, N = 256 (one M tile per CTA tile)
     (2, 8, 64, 128, 0, 3, 384, True),        # N = 384: two MMAs per K step
     (3, 16, 32, 200, 0, 1, 128, True),       # 1x1, channel remainder (196 of a 200-pitch row) -> TMA out-of-bounds fill along K
     (2, 24, 96, 128, 0, 3, 64, True),        # TW = 32 (wd = 96), N = 64

@@ -1,4 +1,4 @@
-"""time corr_volume_pyramid (tcgen05) against the reference formula on the GPU (cuBLAS fp16 matmul + 3x avg_pool2d)"""
+"""time corr_volume_pyramid (wgmma) against the reference formula on the GPU (cuBLAS fp16 matmul + 3x avg_pool2d)"""
 import os, sys, json, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import droid_slam_b200
