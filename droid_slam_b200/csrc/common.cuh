@@ -45,6 +45,12 @@ __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
 }
+// same, allocated in L1: another load of the same 32-byte sector by the SM is served from L1 instead of L2
+__device__ __forceinline__ uint4 ldg_nc_v4_l1(const void* p) {
+  uint4 r;
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+  return r;
+}
 
 // ---- SE3 helpers, same arithmetic as the reference device functions ---------------------------------------
 // (reference src/droid_kernels.cu:67-116; double-literal `2.0 *` there promotes to fp64 and rounds once, which

@@ -11,7 +11,8 @@
 //     warp-coalesced rows of the [n][i][j][y][x] output, coords loads are coalesced;
 //   * the 8x8 tap window is fetched as 16-byte aligned vector loads (2 per window row for f16, 3 for f32),
 //     all 16/24 loads of a pixel issued before first use (memory-level parallelism), streamed past L1
-//     (ld.global.nc.L1::no_allocate);  window alignment inside the vectors is resolved in registers with a
+//     (ld.global.nc.L1::no_allocate), except in the fused lookup on tiled volumes, where the two loads that share a 32-byte
+//     sector meet in L1 (corr_lookup_pyramid_f16_kernel);  window alignment inside the vectors is resolved in registers with a
 //     3-level select / funnel-shift network (no local memory, no shared memory);
 //   * out-of-plane rows / 16-byte chunks are predicated off and zero filled: for finite coordinates a zero tap
 //     contributes exactly +-0, identical to the reference's skip.  Non-finite coordinates take the exact
@@ -205,9 +206,13 @@ __device__ __forceinline__ void align_row_f16(const uint4& A, const uint4& B, in
 // plane); the arithmetic and therefore every output bit is the same.
 // T16 = __half (reference arithmetic: product and sum rounded in f16, two taps per half2 instruction) or __nv_bfloat16 (extension:
 // fp32 FMA chain on the bf16 inputs, rounded once -- the same function as the generic bf16 path, with the vector loads of the f16 one)
-template <bool TILED, typename T16 = __half>
-__device__ __forceinline__ void corr_pixel_f16_r3(const T16* __restrict__ plane, T16* __restrict__ out_px, size_t out_stride,
-                                                  float x0, float y0, int h2, int w2) {
+//
+// The window comes from fetch(y1, cx): the 16-byte chunk holding taps (y1, 8cx .. 8cx+7) of the plane, called only for chunks
+// inside the plane (the others are zero).  Chunk B (taps a0+8 ..) is not fetched when the window starts on a chunk boundary (o == 0):
+// all 8 taps are then in chunk A.  `plane` (global memory, layout TILED) is read only by the slow path for non-finite coordinates.
+template <bool TILED, typename T16, typename Fetch>
+__device__ __forceinline__ void corr_pixel_f16_r3_from(Fetch fetch, const T16* __restrict__ plane, T16* __restrict__ out_px,
+                                                       size_t out_stride, float x0, float y0, int h2, int w2) {
   constexpr bool kHalf = sizeof(T16) == 2 && std::is_same<T16, __half>::value;
   if (!(isfinite(x0) && isfinite(y0))) {   // exact reference semantics for NaN/inf coordinates (slow path)
     if constexpr (TILED && !kHalf) return;                                       // (tiled planes exist for f16 only)
@@ -219,18 +224,17 @@ __device__ __forceinline__ void corr_pixel_f16_r3(const T16* __restrict__ plane,
   const int x1s = floor_to_int_sat(fxf) - 3, y1s = floor_to_int_sat(fyf) - 3;
   const int a0 = x1s & ~7;
   const int o = x1s - a0;
-  const bool okA = (unsigned)a0 < (unsigned)w2, okB = (unsigned)(a0 + 8) < (unsigned)w2;
-  const int tpr = w2 >> 3;                                   // tiles per tile row
+  const bool okA = (unsigned)a0 < (unsigned)w2, okB = o != 0 && (unsigned)(a0 + 8) < (unsigned)w2;
+  const int cx = a0 >> 3;
 
   uint4 A[8], B[8];
 #pragma unroll
   for (int b = 0; b < 8; b++) {
     const int y1 = y1s + b;
     const bool rowok = (unsigned)y1 < (unsigned)h2;
-    const T16* row = TILED ? plane + ((size_t)(y1 >> 2) * tpr + (a0 >> 3)) * 32 + (y1 & 3) * 8 : plane + (size_t)y1 * w2 + a0;
     A[b] = make_uint4(0, 0, 0, 0); B[b] = make_uint4(0, 0, 0, 0);
-    if (rowok && okA) A[b] = ldg_nc_v4(row);
-    if (rowok && okB) B[b] = ldg_nc_v4(row + (TILED ? 32 : 8));
+    if (rowok && okA) A[b] = fetch(y1, cx);
+    if (rowok && okB) B[b] = fetch(y1, cx + 1);
   }
   const float f00 = (1.0f - dx) * (1.0f - dy), f01 = (1.0f - dx) * dy, f10 = dx * (1.0f - dy), f11 = dx * dy;
   const __half2 w00 = __half2half2(__float2half_rn(f00));
@@ -271,6 +275,22 @@ __device__ __forceinline__ void corr_pixel_f16_r3(const T16* __restrict__ plane,
   }
 }
 
+// chunk (y1, cx) of a plane in global memory, row-major or 4x8-tiled
+template <bool TILED, typename T16>
+__device__ __forceinline__ const T16* plane_chunk(const T16* plane, int y1, int cx, int w2) {
+  return TILED ? plane + ((size_t)(y1 >> 2) * (w2 >> 3) + cx) * 32 + (y1 & 3) * 8 : plane + (size_t)y1 * w2 + cx * 8;
+}
+
+template <bool TILED, typename T16 = __half, bool L1 = false>
+__device__ __forceinline__ void corr_pixel_f16_r3(const T16* __restrict__ plane, T16* __restrict__ out_px, size_t out_stride,
+                                                  float x0, float y0, int h2, int w2) {
+  auto fetch = [&](int y1, int cx) {
+    const T16* chunk = plane_chunk<TILED>(plane, y1, cx, w2);
+    return L1 ? ldg_nc_v4_l1(chunk) : ldg_nc_v4(chunk);
+  };
+  corr_pixel_f16_r3_from<TILED, T16>(fetch, plane, out_px, out_stride, x0, y0, h2, w2);
+}
+
 template <typename T16>
 __global__ void __launch_bounds__(128) corr_index_fwd_f16_r3_kernel(const T16* __restrict__ vol, const float* __restrict__ coords,
                                                                     T16* __restrict__ out, long long total, int hw1, int h2, int w2) {
@@ -287,8 +307,12 @@ __global__ void __launch_bounds__(128) corr_index_fwd_f16_r3_kernel(const T16* _
 // coordinates are read once, the level-l lookup uses coords / 2^l (exact in fp32, like the reference's `coords/2**i`), and the four
 // [49,H,W] results land directly in the concatenated [E,196,H,W] tensor the update operator consumes (the reference allocates four
 // tensors and copies them with torch.cat).  tiled_levels: bit l set = level l is stored in the 4x8-tile layout.
-template <int TILED_MASK>
-__global__ void __launch_bounds__(128) corr_lookup_pyramid_f16_kernel(const __half* __restrict__ v0, const __half* __restrict__ v1,
+// L1: window loads allocate in L1.  A 32-byte sector holds two rows of a 4x8 tile (levels 0-1), one whole 16-wide row (level 2, both
+// chunks A and B) or two 8-wide rows (level 3); the pixel loads each row separately, so without L1 every sector crosses L2 -> SM twice.
+// With L1 the second load of a sector hits: on an H100 SXM (400 W) the tiled lookup at 512 edges, 48x64 goes from 1.214 to 0.706 ms.
+// It is compiled with minBlocks = 1 (136 registers, 3 CTAs per SM, no spills); capping it at 80 registers for 6 CTAs measured ~9 % slower.
+template <int TILED_MASK, bool L1>
+__global__ void __launch_bounds__(128, L1 ? 1 : 0) corr_lookup_pyramid_f16_kernel(const __half* __restrict__ v0, const __half* __restrict__ v1,
                                                                       const __half* __restrict__ v2, const __half* __restrict__ v3,
                                                                       const float* __restrict__ coords, __half* __restrict__ out,
                                                                       long long total, int hw1, int h1, int w1) {
@@ -300,10 +324,10 @@ __global__ void __launch_bounds__(128) corr_lookup_pyramid_f16_kernel(const __ha
   const float y0 = coords[((size_t)n * 2 + 1) * hw1 + pin];
   __half* o = out + (size_t)n * 196 * hw1 + pin;
   // coarse levels first: their planes are small and their loads return while the level-0 window (the expensive one) is being issued
-  corr_pixel_f16_r3<(TILED_MASK & 8) != 0>(v3 + (size_t)p * (h1 >> 3) * (w1 >> 3), o + (size_t)147 * hw1, (size_t)hw1, x0 * 0.125f, y0 * 0.125f, h1 >> 3, w1 >> 3);
-  corr_pixel_f16_r3<(TILED_MASK & 4) != 0>(v2 + (size_t)p * (h1 >> 2) * (w1 >> 2), o + (size_t)98 * hw1, (size_t)hw1, x0 * 0.25f, y0 * 0.25f, h1 >> 2, w1 >> 2);
-  corr_pixel_f16_r3<(TILED_MASK & 2) != 0>(v1 + (size_t)p * (h1 >> 1) * (w1 >> 1), o + (size_t)49 * hw1, (size_t)hw1, x0 * 0.5f, y0 * 0.5f, h1 >> 1, w1 >> 1);
-  corr_pixel_f16_r3<(TILED_MASK & 1) != 0>(v0 + (size_t)p * h1 * w1, o, (size_t)hw1, x0, y0, h1, w1);
+  corr_pixel_f16_r3<(TILED_MASK & 8) != 0, __half, L1>(v3 + (size_t)p * (h1 >> 3) * (w1 >> 3), o + (size_t)147 * hw1, (size_t)hw1, x0 * 0.125f, y0 * 0.125f, h1 >> 3, w1 >> 3);
+  corr_pixel_f16_r3<(TILED_MASK & 4) != 0, __half, L1>(v2 + (size_t)p * (h1 >> 2) * (w1 >> 2), o + (size_t)98 * hw1, (size_t)hw1, x0 * 0.25f, y0 * 0.25f, h1 >> 2, w1 >> 2);
+  corr_pixel_f16_r3<(TILED_MASK & 2) != 0, __half, L1>(v1 + (size_t)p * (h1 >> 1) * (w1 >> 1), o + (size_t)49 * hw1, (size_t)hw1, x0 * 0.5f, y0 * 0.5f, h1 >> 1, w1 >> 1);
+  corr_pixel_f16_r3<(TILED_MASK & 1) != 0, __half, L1>(v0 + (size_t)p * h1 * w1, o, (size_t)hw1, x0, y0, h1, w1);
 }
 
 __global__ void __launch_bounds__(128) corr_index_fwd_f32_r3_kernel(const float* __restrict__ vol, const float* __restrict__ coords,
@@ -466,9 +490,9 @@ extern "C" int dba_corr_lookup_pyramid(const void* v0, const void* v1, const voi
   const unsigned blocks = (unsigned)((total + 127) / 128);
   cudaStream_t st = (cudaStream_t)stream;
   if (tiled_mask == 3)
-    corr_lookup_pyramid_f16_kernel<3><<<blocks, 128, 0, st>>>((const __half*)v0, (const __half*)v1, (const __half*)v2, (const __half*)v3, coords, (__half*)out, total, h1 * w1, h1, w1);
+    corr_lookup_pyramid_f16_kernel<3, true><<<blocks, 128, 0, st>>>((const __half*)v0, (const __half*)v1, (const __half*)v2, (const __half*)v3, coords, (__half*)out, total, h1 * w1, h1, w1);
   else
-    corr_lookup_pyramid_f16_kernel<0><<<blocks, 128, 0, st>>>((const __half*)v0, (const __half*)v1, (const __half*)v2, (const __half*)v3, coords, (__half*)out, total, h1 * w1, h1, w1);
+    corr_lookup_pyramid_f16_kernel<0, false><<<blocks, 128, 0, st>>>((const __half*)v0, (const __half*)v1, (const __half*)v2, (const __half*)v3, coords, (__half*)out, total, h1 * w1, h1, w1);
   DBA_CHECK_LAUNCH("corr_lookup_pyramid");
   return DBA_OK;
 }
