@@ -837,15 +837,6 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
 }
 __device__ __forceinline__ void sts_f32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
 
-// debug timeline (DBA_TC_TIMING build only): globaltimer stamps of one CTA's warp 0 / MMA thread
-#ifdef DBA_TC_TIMING
-__device__ unsigned long long g_tc_timing[8192];
-__device__ __forceinline__ unsigned long long tc_gtimer() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define TC_STAMP(cond, idx) do { if (cond) g_tc_timing[(idx)] = tc_gtimer(); } while (0)
-#else
-#define TC_STAMP(cond, idx) do {} while (0)
-#endif
-
 // PAIR mode (frames with 22..100 rows: dense graphs, edge-sharded ranks): the rows are cut into tiles of 10; CTA (frame, pair z) stacks
 // tile a in operand rows 0..63 and tile b in rows 64..127 over the SAME 32 pixels (the packed layout with a zero pixel offset for the
 // second half), so the one M = N = 128 product holds S_ba in its lower-left block and S_aa / S_bb on the diagonal (emitted only by
@@ -902,7 +893,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   const int R6a = PAIR ? 6 * min(kPairTileRows, nrows - kPairTileRows * ta) : 6 * nrows;
   const int R6b = PAIR ? 6 * min(kPairTileRows, nrows - kPairTileRows * tb) : 6 * nrows;
   const int R6 = R6a;                                    // operand rows 0..R6-1: E rows, row R6: w  (PAIR: of the half, see R6h)
-  TC_STAMP(blockIdx.x == 0 && blockIdx.y == 20 && threadIdx.x == 0, 7);
   const bool packed = !PAIR && (R6 + 2 <= 64);          // two PIXEL halves of a 64-pixel chunk in operand rows 0..63 / 64..127
   const bool two_halves = PAIR || packed;                // operand rows 64..127 carry a second set of lines
   const int nhalf = packed ? 2 : 1;
@@ -926,12 +916,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
-  const bool dbg0 = (blockIdx.x == 0 && blockIdx.y == 20) && tid == 0;
-  (void)dbg0;
-  TC_STAMP(dbg0, 0);
-#ifdef DBA_TC_TIMING
-  if (dbg0) { g_tc_timing[1] = (unsigned long long)nchunks; g_tc_timing[2] = (unsigned long long)R6; }
-#endif
 
   // ================= raw rows -> split operands =================
   // Every warp stages and splits its OWN lines (line = warp + 8 i); the operand stage is shared by both warpgroups' MMAs.
@@ -996,14 +980,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   float acc[64], D[64], G[64];                              // running hi hi^T, this chunk's hi hi^T, hi lo^T (m64n128 fragments)
 #pragma unroll
   for (int j = 0; j < 64; j++) acc[j] = 0.f;
-  TC_STAMP(dbg0, 3);
   // Operand stage c % 4 is rewritten at chunk c: the MMAs of chunk c - 4 that read it are complete, because each warpgroup waits
   // for its chunk c - 2 before issuing chunk c - 1, and both passed the CTA barrier of chunk c - 1.
   for (int c = 0; c < nchunks; c++) {
-    TC_STAMP(dbg0, 16 + 8 * c + 0);
     asm volatile("cp.async.wait_group %0;" ::"n"(kTcRawStages - 2) : "memory");
     __syncwarp();                                          // this warp's copies of chunk c have landed
-    TC_STAMP(dbg0, 16 + 8 * c + 1);
     const int os = c % kTcOpStages;
     const uint32_t raw = raw_base + (uint32_t)(c % kTcRawStages) * kTcRawBytes + (uint32_t)warp * 2048 + (uint32_t)(lane >> 3) * 128 +
                          (uint32_t)piece * 16;
@@ -1029,7 +1010,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
         asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ophi + kTcOpBytes + op_off[i]), "f"(lo[0]), "f"(lo[1]), "f"(lo[2]), "f"(lo[3]) : "memory");
       }
     }
-    TC_STAMP(dbg0, 16 + 8 * c + 3);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // generic-proxy stores -> visible to the tensor core
     __syncthreads();
     if (c > 0) {                                                         // chunk c - 1's hi hi^T into the running sum
@@ -1049,7 +1029,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
       }
     }
     wgmma_commit();
-    TC_STAMP(dbg0, 16 + 8 * c + 4);
     issue(c + kTcRawStages - 1);
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -1058,7 +1037,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   wgmma_fence_regs(G);
 #pragma unroll
   for (int j = 0; j < 64; j++) acc[j] += D[j];
-  TC_STAMP(dbg0, 4);
 
   // ================= G = hi lo^T: through shared memory (the operand ring is idle now) so that G + G^T can be formed
   __syncthreads();                                         // both warpgroups' MMAs have completed: the ring may be overwritten
@@ -1111,7 +1089,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
       }
     }
   }
-  TC_STAMP(dbg0, 5);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1313,10 +1290,10 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc pair smem attr");
       attr_set = true;
     }
-    // frames with at most 21 rows go to the tensor cores (needs 16-byte aligned pixel rows); DBA_SCHUR_SIMT=1 keeps the CUDA-core path
-    static const bool force_simt = (getenv("DBA_SCHUR_SIMT") != nullptr && getenv("DBA_SCHUR_SIMT")[0] == '1');
-    const bool use_tc = (HW % 4 == 0) && !force_simt;
-    int pair_rows_max = kTcRowsMax;                  // frames with more rows than this go to the SIMT kernel
+    // the tensor-core kernels need 16-byte aligned pixel rows: frames with at most 21 rows go to the packed / single kernel, 22..100 rows
+    // to the pair kernel, more to ba_schur_gemm_kernel.  Otherwise ba_schur_small_kernel takes frames with at most 16 rows and
+    // ba_schur_gemm_kernel the rest.
+    const bool use_tc = (HW % 4 == 0);
     if (use_tc) {
       const int tiles64 = (HW + 63) / 64;
       const int chunks_tc = std::max(1, std::min(tiles64, (sms + eff_frames / 2) / eff_frames));     // one CTA per SM
@@ -1326,14 +1303,12 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
                                                            WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta_tc, WS(float, L.off_Eij),
                                                            WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
       // frames with 22..100 rows (dense graphs, edge-sharded ranks): tile pairs over gridDim.z, whole pixel range per CTA; CTAs of
-      // frames outside that range (and pair indices beyond a frame's count) exit after the row-list build.  DBA_SCHUR_PAIR=0: SIMT kernel.
-      static const bool no_pair = (getenv("DBA_SCHUR_PAIR") != nullptr && getenv("DBA_SCHUR_PAIR")[0] == '0');
+      // frames outside that range (and pair indices beyond a frame's count) exit after the row-list build.
       const int max_big = std::min(a->n_frames, a->n_edges / kTcRowsMax);     // a frame with 22+ rows has 21+ out-edges
-      if (!no_pair && max_big > 0)
+      if (max_big > 0)
         ba_schur_tc_kernel<true><<<dim3(1, max_big, kPairGridZ), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
                                                            WS(int, L.off_edgeidx), HW, a->t0, L.P, ((HW + 31) / 32) * 32, WS(float, L.off_Eij),
                                                            WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
-      pair_rows_max = no_pair ? kTcRowsMax : kPairRowsMax;
     } else {
       ba_schur_small_kernel<<<dim3(gx1, a->n_frames, 1), kSgThreads, smem2, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
                                                            WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta1, WS(float, L.off_Eij),
@@ -1341,7 +1316,7 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
     }
     DBA_CHECK_LAUNCH("ba_schur<single>");
     ba_schur_gemm_kernel<<<dim3(gx2, a->n_frames, zsplit2), kSgThreads, smem2, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta2, use_tc ? pair_rows_max : kSgRows, WS(float, L.off_Eij),
+                                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta2, use_tc ? kPairRowsMax : kSgRows, WS(float, L.off_Eij),
                                                                          WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys);
     DBA_CHECK_LAUNCH("ba_schur<multi>");
   }
@@ -1407,13 +1382,6 @@ extern "C" int dba_ba_p2p_signal(const dba_ba_args* a) {
   DBA_CHECK_LAUNCH("ba_p2p_signal");
   return DBA_OK;
 }
-
-#ifdef DBA_TC_TIMING
-extern "C" int dba_debug_tc_timing(unsigned long long* out, int n) {
-  cudaDeviceSynchronize();
-  return (int)cudaMemcpyFromSymbol(out, dba::g_tc_timing, sizeof(unsigned long long) * (size_t)std::min(n, 8192));
-}
-#endif
 
 extern "C" int dba_ba(const dba_ba_args* a, int iterations) {
   int rc = dba_ba_prepare(a);

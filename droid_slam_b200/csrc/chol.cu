@@ -7,8 +7,9 @@
 //  * chol_resident_kernel (n <= 448, i.e. <= 14 tile rows: frontend windows, the 72-keyframe metric window) -- every tile has one owner
 //    warp for the whole factorisation and lives in its registers; tiles are handed over through global memory (L2) WITHOUT flags, fences
 //    or barriers: every output location is pre-filled with a NaN bit pattern no arithmetic produces and a consumer re-reads a tile until no
-//    element is that sentinel.  See the comment block above the kernel and DESIGN.md 4.4 for the measurements that led there (every
-//    acquire ends in CCTL.IVALL and makes the next global loads ~10x slower; the unrolled potrf was bound by instruction delivery).
+//    element is that sentinel.  See DESIGN.md §4.3 and the comment block above the kernel for the measurements that led there (measured
+//    on B200, not re-measured on H100: every acquire ends in CCTL.IVALL and makes the next global loads ~10x slower; an unrolled potrf
+//    was bound by instruction delivery).
 //  * chol_cluster_kernel (larger systems) -- right-looking tiled Cholesky with the tiles in global memory (L2 resident).  Per panel k:
 //     TRSM of the column-k tiles (one warp per tile, lane = row, forward substitution against L_kk in shared memory)
 //       -- cluster barrier --
@@ -27,15 +28,13 @@
 // O(n^3) to O(n b^2) -- what Eigen's sparse LLT does for the reference.
 // The right-hand side rides along as an extra tile row, so L^-1 b comes out of the factorisation for free; the
 // backward substitution uses the inverted diagonal tiles and runs in CTA 0.
-// (B200 note, measured: a dependent fp64 op costs ~9 cycles, the fp64 pipe issues one warp instruction per ~2.3 cycles per SM
-//  sub-partition, and a 64-bit warp shuffle pair is slower than a shared-memory broadcast, which is why the pivot column goes through
-//  shared memory and the pivot uses an fp32 rsqrt seed + one Newton step -- 3e-14 relative, far below the fp32 rounding of the result.)
+// (Measured on B200, not re-measured on H100: a dependent fp64 op costs ~9 cycles, the fp64 pipe issues one warp instruction per ~2.3
+//  cycles per SM sub-partition, and a 64-bit warp shuffle pair is slower than a shared-memory broadcast, which is why the pivot column
+//  goes through shared memory and the pivot uses an rsqrt seed + one correction step, see fast_rsqrt.)
 #include "common.cuh"
 #include <cooperative_groups.h>
 #include <math.h>
 #include <stdint.h>
-#include <stdlib.h>
-#include <string.h>
 
 namespace cg = cooperative_groups;
 
@@ -46,13 +45,11 @@ constexpr int kTP = kT + 1;            // padded row length in shared memory
 constexpr int kCholThreads = 256;      // 8 warps per CTA
 constexpr int kCholWarps = kCholThreads / 32;
 
-__device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define CHOL_STAMP(slot) do { if (p.timing && cta == 0 && tid == 0) p.timing[(slot)] = gtimer(); } while (0)
 __device__ __forceinline__ double ldcg(const double* p) { return __ldcg(p); }
 __device__ __forceinline__ void stcg(double* p, double v) { __stcg(p, v); }
 
 // 1/sqrt(d): MUFU.RSQ64H seed (~2^-22) + one third-order correction r += r t (1/2 + 3/8 t), t = 1 - d r^2 (error ~ t^3: full fp64).
-// Deliberately branch-free: a branch here splits warp_potrf into basic blocks and stops ptxas from scheduling the rank-1 update
+// Deliberately branch-free: a branch here splits the potrf loop into basic blocks and stops ptxas from scheduling the rank-1 update
 // under the latency of this chain.  d <= 0 yields NaN/inf, which the caller flags through its pivot test.
 __device__ __forceinline__ double fast_rsqrt(double d) {
   double r;
@@ -61,9 +58,11 @@ __device__ __forceinline__ double fast_rsqrt(double d) {
   return fma(fma(0.375, t, 0.5), r * t, r);
 }
 
-// Cholesky of a 32x32 tile, one row per lane in registers; the pivot column is broadcast through `col` (2 x 32 doubles
-// of shared memory private to the warp).  rdiag_out receives 1/L[k][k] (lane k's value).  Returns false on a
-// non-positive pivot.
+// Cholesky of a 32x32 tile, one row per lane in registers; the pivot column is broadcast through `col` (2 x 32 doubles of shared memory
+// private to the warp).  rdiag_out receives 1/L[k][k] (lane k's value).  Returns false on a non-positive pivot.  Fully unrolled (~1800
+// straight-line instructions): used only for tile (0,0) of chol_cluster_kernel, which every other warp of the cluster waits for.  There
+// it is faster than warp_potrf_compact (measured on H100: the compact routine made banded n = 2394 solves 3-10 us slower) with the
+// same bits.
 __device__ __forceinline__ bool warp_potrf(double (&a)[kT], int lane, double* col, double& rdiag_out) {
   bool ok = true;
   rdiag_out = 0.0;
@@ -91,14 +90,14 @@ __device__ __forceinline__ bool warp_potrf(double (&a)[kT], int lane, double* co
   return ok;
 }
 
-// Cholesky of a 32x32 tile, one row per lane, in ~300 instructions instead of the ~1800 straight-line ones of warp_potrf.  ncu on the
-// resident kernel (profiles/r2_chol_resident_stalls.txt): 40 % of the samples inside the unrolled potrf are "no instruction" -- the code is
-// executed once per SM and its delivery from the GPC-level instruction cache, not its dependent chain, sets the pace (2.9 us on an idle
-// GPC, 5.3 us while the other 15 SMs fetch code of their own).  Here the row is shifted down one register per column, so a[0] is always
-// the pivot column and all register indices are static inside a rolled loop; four loops of eight columns with widths 32/24/16/8 keep
-// the extra arithmetic at 608 instead of 496 DFMAs.  The pivot column is published twice (offset by one double) so that the operands
-// of the rank-1 update can be fetched with aligned 16-byte loads whatever the parity of the column.  Per element the operations and
-// their order are those of warp_potrf: identical bits.  out[lane][k] receives L (zeros above the diagonal).
+// The same factorisation in ~300 instructions.  The unrolled warp_potrf is bound by instruction delivery, not by its dependent chain,
+// when all SMs of a GPC run it at once (measured on B200, not re-measured on H100: 40 % of the samples inside it were "no instruction";
+// the code comes from the GPC-level instruction cache: 2.9 us on an idle GPC, 5.3 us while the other 15 SMs fetch code of their own).
+// Here the row is shifted down one register per column, so a[0] is always the pivot column and all register indices are static inside
+// a rolled loop; four loops of eight columns with widths 32/24/16/8 keep the extra arithmetic at 608 instead of 496 DFMAs.  The pivot
+// column is published twice (offset by one double) so that the operands of the rank-1 update can be fetched with aligned 16-byte loads
+// whatever the parity of the column.  Per element the operations and their order are those of warp_potrf: identical bits.
+// out[lane][k] receives L (zeros above the diagonal).
 template <int W>
 __device__ __forceinline__ void potrf_phase(double (&a)[kT], int lane, int k0, double* cx, double* cy, double (*out)[kTP], double& d, double& r, bool& ok,
                                             double& rdiag_out) {
@@ -150,19 +149,48 @@ struct CholParams {
   double* L;         // [(nt+1)*32][nt*32] row-major working matrix (tile row nt carries b^T in its row 0)
   double* Linv;      // [nt][32][32] inverses of the diagonal tiles
   double* rdiag;     // [nt*32] reciprocals of diag(L)
-  int* first;        // [nt+1] envelope: first nonzero tile column of each tile row (rhs row nt: 0)
-  int* flags;        // (unused)
-  unsigned sleep_urgent, sleep_idle;   // resident-tile kernel: ns between polls of a warp on / off the critical path
-  int warm;                            // bit 1: the diagonal owner substitutes tile (j, j-1) itself (default; DBA_CHOL_FUSED_SUBST=0 turns it off)
-  double* Cs;                          // resident-tile kernel: [nt][32][32] tiles (j+1, j) BEFORE the substitution (for mode 2)
+  int* first;        // [nt+2] envelope: first nonzero tile column of each tile row (rhs row nt: 0); word nt+1: store-drain target
+  double* Cs;        // resident-tile kernel: [nt][32][32] tiles (j+1, j) BEFORE the substitution
   unsigned char map_i[128], map_j[128];   // resident-tile kernel: tile (i, j) of warp slot cta*8 + warp; 0xFF = none
   int* fail;         // sticky flag: non-positive pivot
   float* x;          // [n] result (fp32 like the reference's dx)
   int n, nt;
   double lm, ep;
-  unsigned long long* timing;   // debug (DBA_CHOL_TIMING=1): globaltimer stamps of CTA 0 / the potrf warp, else nullptr
-  CholPeers peers;              // world <= 1: plain local system
+  CholPeers peers;   // world <= 1: plain local system
 };
+
+// Multi-GPU (world > 1): thread 0 of every CTA waits until every rank has published its partial system for this epoch.  CTA 0 clears
+// the fail flag, or sets it to 2 when a peer never arrived: the solve gives up loudly (dx = 0) instead of hanging.
+__device__ __forceinline__ void wait_for_peers(const CholPeers& peers, int world, int cta, int tid, int* fail) {
+  if (world > 1) {
+    __shared__ int s_timeout;
+    if (tid == 0) {
+      int bad = 0;
+      const unsigned long long want = peers.epoch_dev ? *peers.epoch_dev : peers.epoch;
+      for (int r = 0; r < world; r++) {
+        unsigned long long v = 0;
+        long long spins = 0;
+        do {
+          asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(peers.flags + r) : "memory");
+        } while (v < want && ++spins < (1ll << 24));
+        if (v < want) bad = 1;
+      }
+      s_timeout = bad;
+    }
+    __syncthreads();
+    if (cta == 0 && tid == 0) *fail = s_timeout ? 2 : 0;
+  } else if (cta == 0 && tid == 0) *fail = 0;
+}
+
+// index of entry (r, c) of the padded working matrix in the [n*n | n] system (H row-major, lower triangle valid; diagonal tiles are kept
+// fully symmetric), or -1 for an entry that is not read from it (identity padding, zeros above the diagonal tiles)
+__device__ __forceinline__ size_t sys_index(int r, int c, int n, bool diag_tile) {
+  if (r < n && c < n) {
+    if (c <= r) return (size_t)r * n + c;
+    if (diag_tile) return (size_t)c * n + r;
+  }
+  return (size_t)-1;
+}
 
 // one warp: C (32x32 at Ct) -= A (at At) * B^T (at Bt); lane (rg = lane>>3, cg = lane&7) owns rows 8rg..8rg+7, cols 4cg..4cg+3
 __device__ __forceinline__ void warp_tile_update(const double* At, const double* Bt, double* Ct, int ld, int lane,
@@ -245,26 +273,9 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
   double (*s_D)[kTP] = reinterpret_cast<double (*)[kTP]>(s_dyn + (size_t)2 * kCholWarps * kT * kTP);
   double (*s_T)[kTP] = reinterpret_cast<double (*)[kTP]>(s_dyn + (size_t)2 * kCholWarps * kT * kTP + kT * kTP);
 
-  // ---- fused peer-to-peer reduction: wait until every rank has published its partial system for this epoch ------------
+  // ---- fused peer-to-peer reduction: wait for the peers' partial systems
   const int world = p.peers.world;
-  if (world > 1) {
-    __shared__ int s_timeout;
-    if (tid == 0) {
-      int bad = 0;
-      const unsigned long long want = p.peers.epoch_dev ? *p.peers.epoch_dev : p.peers.epoch;
-      for (int r = 0; r < world; r++) {
-        unsigned long long v = 0;
-        long long spins = 0;
-        do {
-          asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p.peers.flags + r) : "memory");
-        } while (v < want && ++spins < (1ll << 24));
-        if (v < want) bad = 1;
-      }
-      s_timeout = bad;
-    }
-    __syncthreads();
-    if (cta == 0 && tid == 0) *p.fail = s_timeout ? 2 : 0;   // a peer never arrived: give up loudly (dx = 0), never hang
-  } else if (cta == 0 && tid == 0) *p.fail = 0;
+  wait_for_peers(p.peers, world, cta, tid, p.fail);
   // ---- envelope: first[i] starts at the diagonal, the load below lowers it to the first nonzero tile of the row
   const bool envelope = nt < kCholThreads;             // one thread per tile row in the per-panel scan below
   for (int i = cta * kCholThreads + tid; i <= nt; i += ncta * kCholThreads) p.first[i] = (i < nt && envelope) ? i : 0;
@@ -294,10 +305,8 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
         if (idx < total) {
           const int r = (int)(idx / ld), c = (int)(idx - (size_t)r * ld);
           if (r < nt * kT) {
-            if (r < n && c < n) {
-              if (c <= r) srcs[u] = (size_t)r * n + c;
-              else if ((r >> 5) == (c >> 5)) srcs[u] = (size_t)c * n + r;     // diagonal tiles are kept fully symmetric
-            } else if (r == c) vals[u] = 1.0;
+            if (r < n && c < n) srcs[u] = sys_index(r, c, n, (r >> 5) == (c >> 5));
+            else if (r == c) vals[u] = 1.0;                   // identity padding
           } else if (r == nt * kT && c < n) srcs[u] = nn + c;
         }
         if (srcs[u] != (size_t)-1) {                      // element of the [n*n | n] system feeding this entry
@@ -333,9 +342,7 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
       }
     }
   }
-  CHOL_STAMP(0);
   cluster.sync();
-  CHOL_STAMP(1);
 
   // ---- potrf of tile (0,0) --------------------------------------------------------------------------------------
   if (gw == 0) {
@@ -348,7 +355,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
     stcg(p.rdiag + lane, rd);
   }
   cluster_sync_light(mbar, mphase, ncta, tid, drain);
-  CHOL_STAMP(2);
 
   for (int k = 0; k < nt; k++) {
     // ---- every CTA: L_kk and its reciprocal diagonal into shared memory
@@ -371,7 +377,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
     }
     __syncthreads();
     const int nact = envelope ? s_nact : (nt - k);       // >= 1: the rhs row
-    CHOL_STAMP(8 + 8 * k + 0);
     // ---- TRSM: tiles (i,k) of the active rows (tile row nt is the right-hand side)
     for (int ta = gw; ta < nact; ta += nwarps) {
       const int i = envelope ? s_act[ta] : k + 1 + ta;
@@ -398,9 +403,7 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
       for (int r = 0; r < kT; r++) stcg(tile + (size_t)r * ld + lane, s_A[warp][r][lane]);
       __syncwarp();
     }
-    CHOL_STAMP(8 + 8 * k + 1);
     cluster_sync_light(mbar, mphase, ncta, tid, drain);
-    CHOL_STAMP(8 + 8 * k + 2);
     // ---- trailing update with panel k
     const int rem = nt - k - 1;                       // remaining tile columns
     const int m1 = nact - 1;                          // active rows without the rhs row
@@ -434,13 +437,11 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
       }
       __syncthreads();
       if (warp == 0) {
-        if (p.timing && lane == 0) p.timing[8 + 8 * k + 5] = gtimer();
         double a[kT], rd;
 #pragma unroll
         for (int c = 0; c < kT; c++) a[c] = s_T[lane][c];
         __syncwarp();
         if (!warp_potrf_compact(a, lane, s_col, s_T, rd) && lane == 0) *p.fail = 1;   // writes L into s_T
-        if (p.timing && lane == 0) p.timing[8 + 8 * k + 6] = gtimer();
         __syncwarp();
 #pragma unroll 8
         for (int r = 0; r < kT; r++) stcg(Ct + (size_t)r * ld + lane, s_T[r][lane]);
@@ -462,7 +463,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
                          s_A[warp], s_B[warp]);
       }
     }
-    CHOL_STAMP(8 + 8 * k + 3);
     // inverse of L_kk (for the backward substitution) by the last warp of the cluster: lane j owns column j
     if (gw == nwarps - 1) {
       double xcol[kT];
@@ -477,7 +477,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
       for (int i = 0; i < kT; i++) stcg(p.Linv + ((size_t)k * kT + i) * kT + lane, xcol[i]);
     }
     cluster_sync_light(mbar, mphase, ncta, tid, drain);
-    CHOL_STAMP(8 + 8 * k + 4);
   }
 
   if (cta != 0) return;
@@ -503,7 +502,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
     }
     __syncthreads();
   }
-  CHOL_STAMP(3);
   const bool failed = (*reinterpret_cast<volatile int*>(p.fail)) != 0;
   for (int i = tid; i < n; i += kCholThreads) {
     const double v = ldcg(y + i);
@@ -516,8 +514,9 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
 // Resident-tile dataflow variant for nt <= 14 (n <= 448: every frontend window, the 72-keyframe metric window).
 //
 // The barrier version above spends a panel on  L_kk reload -> TRSM -> cluster barrier -> trailing update -> cluster barrier.  Measured
-// (in-kernel %globaltimer): the arithmetic is ~3 us of that; the rest is synchronisation -- in particular every acquire (cluster barrier,
-// ld.acquire, fence) ends in CCTL.IVALL, after which the next global loads of the warp take ~3 us instead of ~0.3.
+// on B200, not re-measured on H100 (in-kernel %globaltimer): the arithmetic is ~3 us of that; the rest is synchronisation -- in
+// particular every acquire (cluster barrier, ld.acquire, fence) ends in CCTL.IVALL, after which the next global loads of the warp take
+// ~3 us instead of ~0.3.
 // Here every lower tile (i,j) and every 32-entry piece of the right-hand side has ONE owner warp for the whole factorisation (105 + 14
 // tiles <= 128 warps of the 16-CTA cluster) and lives in that warp's registers.  An owner applies  C -= L_ik L_jk^T  for k = 0..j-1 as
 // soon as the two operand tiles exist, then finalises its tile (potrf on the diagonal, a substitution against L_jj below it) and writes it
@@ -529,14 +528,15 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_cluster_kernel(CholParam
 // Waits are bounded; a wait that expires marks the solve failed (dx = 0) instead of hanging.
 constexpr int kResMaxNt = 14;
 constexpr unsigned long long kSentinel = 0xFFF7DEADBEEF5A5Aull;
-
+constexpr unsigned kSleepUrgent = 300;   // ns between the polls of a warp on the critical path
+constexpr unsigned kSleepIdle = 4000;    // ns between the polls of a warp off it
 
 __device__ __forceinline__ bool is_sentinel(double v) { return __double2hiint(v) == (int)(kSentinel >> 32); }   // arithmetic NaNs are canonical
 __device__ __forceinline__ double sentinel() { return __longlong_as_double((long long)kSentinel); }
 
 // wait until the 32x32 tile at src is completely written, then stage it in the warp's padded slab.  false on time-out.
-// `urgent` (the consumer sits on the critical path): no probe stage, short back-off; otherwise a one-row probe with a long back-off so
-// that the ~100 waiting warps take neither issue slots nor L2 bandwidth from the working ones.
+// A one-row probe polls every sleep_ns (kSleepIdle off the critical path, so that the ~100 waiting warps take neither issue slots nor
+// L2 bandwidth from the working ones), the whole tile is re-read every sleep_retry.
 __device__ __forceinline__ bool tile_fetch(const double* src, int ld, int lane, double (*slab)[kTP], unsigned sleep_ns, unsigned sleep_retry) {
   int tries = 0;
   while (true) {                                             // cheap probe: the row that is stored last
@@ -590,17 +590,6 @@ __device__ __forceinline__ void slab_mac(double (&acc)[8][4], const double (*sA)
   }
 }
 
-// one entry of the damped, padded working matrix straight from H / b (or from the peers' partial systems, summed in rank order)
-__device__ __forceinline__ size_t sys_index(int r, int c, int n, bool diag_tile) {
-  if (r < n && c < n) {
-    if (c <= r) return (size_t)r * n + c;
-    if (diag_tile) return (size_t)c * n + r;
-  }
-  return (size_t)-1;
-}
-
-#define RES_STAMP(col, slot) do { if (p.timing && lane == 0) p.timing[8 + 16 * (col) + (slot)] = gtimer(); } while (0)
-
 template <bool PEERS>
 __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholParams p) {
   cg::cluster_group cluster = cg::this_cluster();
@@ -623,24 +612,7 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
 
   // ---- prologue: wait for the peers' systems (multi-GPU), dense envelope for the backward pass
   for (int i = cta * kCholThreads + tid; i <= nt; i += ncta * kCholThreads) p.first[i] = 0;
-  if (PEERS) {
-    __shared__ int s_timeout;
-    if (tid == 0) {
-      int bad = 0;
-      const unsigned long long want = p.peers.epoch_dev ? *p.peers.epoch_dev : p.peers.epoch;
-      for (int r = 0; r < world; r++) {
-        unsigned long long v = 0;
-        long long spins = 0;
-        do {
-          asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p.peers.flags + r) : "memory");
-        } while (v < want && ++spins < (1ll << 24));
-        if (v < want) bad = 1;
-      }
-      s_timeout = bad;
-    }
-    __syncthreads();
-    if (cta == 0 && tid == 0) *p.fail = s_timeout ? 2 : 0;
-  } else if (cta == 0 && tid == 0) *p.fail = 0;
+  wait_for_peers(p.peers, world, cta, tid, p.fail);
 
   // ---- tile of this warp: placed by the host (resident_tile_map below) so that a potrf never shares its SM with a working warp
   const int slot = cta * kCholWarps + warp;
@@ -679,7 +651,7 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
     double* tile = L + (size_t)(i * kT) * ld + j * kT;
 #pragma unroll 8
     for (int r = 0; r < kT; r++) stcg(tile + (size_t)r * ld + lane, sentinel());
-    if (i == j + 1 && (p.warm & 2)) {
+    if (i == j + 1) {
 #pragma unroll 8
       for (int r = 0; r < kT; r++) stcg(p.Cs + ((size_t)j * kT + r) * kT + lane, sentinel());
     }
@@ -703,7 +675,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
   }
   __threadfence();
   cluster.sync();
-  if (p.timing && cta == 0 && tid == 0) p.timing[0] = p.timing[1] = p.timing[2] = gtimer();
 
   if (has_tile) {
     double (*sA)[kTP] = s_A[warp];
@@ -713,19 +684,16 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
     if (i < nt) {
       // ---------------- matrix tile (i, j): updates with the finished columns k < j
       for (int k = 0; k < j && alive; k++) {
-        const bool last = (i == j && k == j - 1);
-        if (last) RES_STAMP(j, 8);
-        if (last && (p.warm & 2)) {
-          // mode 2: the diagonal owner does not wait for tile (j, j-1) to come back from its owner; it takes that tile as it was BEFORE
-          // the substitution (published early, off the critical path), substitutes against L_{j-1,j-1} itself and updates: one hand-over
+        if (i == j && k == j - 1) {
+          // the diagonal owner does not wait for tile (j, j-1) to come back from its owner; it takes that tile as it was BEFORE the
+          // substitution (published early, off the critical path), substitutes against L_{j-1,j-1} itself and updates: one hand-over
           // per column instead of two.  The owner of (j, j-1) does the same substitution for everybody else.
-          alive = tile_fetch(p.Cs + (size_t)(j - 1) * kT * kT, kT, lane, sA, p.sleep_urgent, p.sleep_urgent);
-          alive = tile_fetch(L + (size_t)((j - 1) * kT) * ld + (j - 1) * kT, ld, lane, sB, p.sleep_urgent, p.sleep_urgent) && alive;
+          alive = tile_fetch(p.Cs + (size_t)(j - 1) * kT * kT, kT, lane, sA, kSleepUrgent, kSleepUrgent);
+          alive = tile_fetch(L + (size_t)((j - 1) * kT) * ld + (j - 1) * kT, ld, lane, sB, kSleepUrgent, kSleepUrgent) && alive;
           double rdl;
-          alive = vec_fetch(p.rdiag + (j - 1) * kT, lane, rdl, p.sleep_urgent) && alive;
+          alive = vec_fetch(p.rdiag + (j - 1) * kT, lane, rdl, kSleepUrgent) && alive;
           s_rd[warp][lane] = rdl;
           __syncwarp();
-          RES_STAMP(j, 9);
           double x[kT];
 #pragma unroll
           for (int c = 0; c < kT; c++) x[c] = sA[lane][c];
@@ -742,20 +710,17 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
           for (int c = 0; c < kT; c++) sA[lane][c] = x[c];
           __syncwarp();
           slab_mac(acc, sA, sA, lane);
-          RES_STAMP(j, 10);
           __syncwarp();
           continue;
         }
         const bool urgent = (i <= j + 1) && (k >= j - 2);     // the tile is (about to be) on the critical path
-        const unsigned slp = urgent ? p.sleep_urgent : p.sleep_idle;
-        alive = tile_fetch(L + (size_t)(i * kT) * ld + k * kT, ld, lane, sA, slp, p.sleep_urgent);
+        const unsigned slp = urgent ? kSleepUrgent : kSleepIdle;
+        alive = tile_fetch(L + (size_t)(i * kT) * ld + k * kT, ld, lane, sA, slp, kSleepUrgent);
         if (i != j) {
-          alive = tile_fetch(L + (size_t)(j * kT) * ld + k * kT, ld, lane, sB, slp, p.sleep_urgent) && alive;
+          alive = tile_fetch(L + (size_t)(j * kT) * ld + k * kT, ld, lane, sB, slp, kSleepUrgent) && alive;
           slab_mac(acc, sA, sB, lane);
         } else {
-          if (last) RES_STAMP(j, 9);
           slab_mac(acc, sA, sA, lane);
-          if (last) RES_STAMP(j, 10);
         }
         __syncwarp();
       }
@@ -771,18 +736,13 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
       for (int c = 0; c < kT; c++) a[c] = sA[lane][c];                 // lane = row
       __syncwarp();
       if (i == j) {
-        RES_STAMP(j, 0);
-        const long long ck0 = clock64();
         double rd;
         if (!warp_potrf_compact(a, lane, s_colb[warp], sA, rd) && lane == 0) *p.fail = 1;
         s_rd[warp][lane] = rd;
         __syncwarp();
-        RES_STAMP(j, 7);
-        if (p.timing && lane == 0) p.timing[8 + 16 * j + 13] = (unsigned long long)(clock64() - ck0);
         stcg(p.rdiag + j * kT + lane, rd);
 #pragma unroll 8
         for (int r = 0; r < kT; r++) stcg(tile + (size_t)r * ld + lane, sA[r][lane]);
-        RES_STAMP(j, 1);
         // inverse of L_jj for the backward pass (off the critical path), rolled: lane c owns column c of X = L^-1, kept in the warp's
         // second slab;  X[r][c] = (delta_rc - sum_{m<r} L[r][m] X[m][c]) / L[r][r]  (entries above the diagonal come out as zeros)
 #pragma unroll 1
@@ -798,18 +758,16 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
         for (int r = 0; r < kT; r++) stcg(p.Linv + ((size_t)j * kT + r) * kT + lane, sB[r][lane]);
       } else {
         const bool sub = (i == j + 1);
-        if (sub && (p.warm & 2)) {
+        if (sub) {
 #pragma unroll 8
           for (int r = 0; r < kT; r++) stcg(p.Cs + ((size_t)j * kT + r) * kT + lane, sA[r][lane]);
         }
-        if (sub) RES_STAMP(j, 2);
         double rdl;
-        const unsigned slp = sub ? p.sleep_urgent : p.sleep_idle;
-        alive = tile_fetch(L + (size_t)(j * kT) * ld + j * kT, ld, lane, sB, slp, p.sleep_urgent) && alive;
-        alive = vec_fetch(p.rdiag + j * kT, lane, rdl, p.sleep_urgent) && alive;
+        const unsigned slp = sub ? kSleepUrgent : kSleepIdle;
+        alive = tile_fetch(L + (size_t)(j * kT) * ld + j * kT, ld, lane, sB, slp, kSleepUrgent) && alive;
+        alive = vec_fetch(p.rdiag + j * kT, lane, rdl, kSleepUrgent) && alive;
         s_rd[warp][lane] = rdl;
         __syncwarp();
-        if (sub) RES_STAMP(j, 4);
 #pragma unroll
         for (int c = 0; c < kT; c++) {
           const double xv = a[c] * s_rd[warp][c];
@@ -818,20 +776,18 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
           for (int jj = c + 1; jj < kT; jj++) a[jj] -= xv * sB[jj][c];
           asm volatile("" ::: "memory");
         }
-        if (sub) RES_STAMP(j, 5);
 #pragma unroll
         for (int c = 0; c < kT; c++) sA[lane][c] = a[c];
         __syncwarp();
 #pragma unroll 8
         for (int r = 0; r < kT; r++) stcg(tile + (size_t)r * ld + lane, sA[r][lane]);
-        if (sub) RES_STAMP(j, 3);
       }
     } else {
       // ---------------- right-hand side piece j: lane c holds entry 32 j + c;  y_j = L_jj^-1 (b_j - sum_k L_jk y_k)
       for (int k = 0; k < j && alive; k++) {
         double yk;
-        alive = vec_fetch(yrow + k * kT, lane, yk, p.sleep_idle);
-        alive = tile_fetch(L + (size_t)(j * kT) * ld + k * kT, ld, lane, sA, p.sleep_idle, p.sleep_urgent) && alive;
+        alive = vec_fetch(yrow + k * kT, lane, yk, kSleepIdle);
+        alive = tile_fetch(L + (size_t)(j * kT) * ld + k * kT, ld, lane, sA, kSleepIdle, kSleepUrgent) && alive;
         double s0 = 0.0, s1 = 0.0;
 #pragma unroll
         for (int c = 0; c < kT; c += 2) {
@@ -842,8 +798,8 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
         __syncwarp();
       }
       double rdl;
-      alive = tile_fetch(L + (size_t)(j * kT) * ld + j * kT, ld, lane, sB, j == nt - 1 ? p.sleep_urgent : p.sleep_idle, p.sleep_urgent) && alive;
-      alive = vec_fetch(p.rdiag + j * kT, lane, rdl, p.sleep_urgent) && alive;
+      alive = tile_fetch(L + (size_t)(j * kT) * ld + j * kT, ld, lane, sB, j == nt - 1 ? kSleepUrgent : kSleepIdle, kSleepUrgent) && alive;
+      alive = vec_fetch(p.rdiag + j * kT, lane, rdl, kSleepUrgent) && alive;
 #pragma unroll
       for (int c = 0; c < kT; c++) {
         const double yc = __shfl_sync(0xffffffffu, y, c) * __shfl_sync(0xffffffffu, rdl, c);
@@ -851,7 +807,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
         else if (lane > c) y -= sB[lane][c] * yc;
       }
       stcg(yrow + j * kT + lane, y);
-      RES_STAMP(j, 11);
     }
     if (!alive && lane == 0) *p.fail = 4;                    // a producer never arrived: give up loudly, never hang
   }
@@ -882,7 +837,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
 #pragma unroll
     for (int r = 0; r < kT; r++) inv_c[r] = __ldcg(p.Linv + ((size_t)(nt - 1) * kT + r) * kT + lane);
     __syncthreads();
-    if (p.timing && tid == 0) p.timing[4] = gtimer();
     for (int k = nt - 1; k >= 0; k--) {
       const double* invp = p.Linv + (size_t)k * kT * kT + lane;
       if (k > 0) {
@@ -916,7 +870,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
       s_y[k * kT + lane] = xk;
       asm volatile("bar.sync 1, %0;" ::"n"(kCholThreads) : "memory");
       asm volatile("bar.sync 2, %0;" ::"n"(kCholThreads) : "memory");
-      RES_STAMP(k, 12);
 #pragma unroll
       for (int r = 0; r < kT; r++) inv_c[r] = inv_n[r];
     }
@@ -962,7 +915,6 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
     }
   }
   __syncthreads();
-  if (p.timing && tid == 0) p.timing[3] = gtimer();
   const bool failed = (*reinterpret_cast<volatile int*>(p.fail)) != 0;
   for (int q = tid; q < n; q += kCholThreads) {
     const double v = s_y[q];
@@ -970,9 +922,9 @@ __global__ void __launch_bounds__(kCholThreads, 1) chol_resident_kernel(CholPara
   }
 }
 
-// Placement of the resident kernel's tiles on the cluster's warp slots.  The fp64 pipe of an SM is narrow (64 lanes/clk, measured) and the
-// potrf of a diagonal tile is a chain of ~8 dependent fp64 operations per column: measured, it takes 5.3 us while other warps of the
-// SM stream the DFMAs of their trailing updates and 2.9 us alone.  A tile of column c works until column c is finished, and potrf(s)
+// Placement of the resident kernel's tiles on the cluster's warp slots.  The fp64 pipe of an SM is narrow and the potrf of a diagonal
+// tile is a chain of ~8 dependent fp64 operations per column (measured on B200, not re-measured on H100: 64 lanes/clk; the potrf takes
+// 5.3 us while other warps of the SM stream the DFMAs of their trailing updates and 2.9 us alone).  A tile of column c works until column c is finished, and potrf(s)
 // runs when column s-1 is finished, so diagonal tile s gets CTA s to itself *in time*: a column-c tile may only share that SM if c < s
 // (finished before), if the SM has no diagonal tile (s >= nt), or if s == 0 (potrf(0) runs before anything else has operands).
 // Tiles of one column substitute at the same time and are spread over different SMs where possible.  Returns false if ncta is too small.
@@ -1007,11 +959,23 @@ static bool resident_tile_map(int nt, int ncta, unsigned char* map_i, unsigned c
   return true;
 }
 
+// Cluster size of the resident kernel for nt tile rows (every tile and right-hand-side piece needs its own warp, every diagonal tile its
+// own CTA) with the tile placement in map_i / map_j; 0 if the system is too large for it or needs more than max_cluster CTAs.
+static int resident_cluster_size(int nt, int max_cluster, unsigned char* map_i, unsigned char* map_j) {
+  if (nt > kResMaxNt) return 0;
+  const int tiles = nt * (nt + 1) / 2 + nt;
+  int rcs = 1;
+  while (rcs * kCholWarps < tiles || rcs < nt) rcs *= 2;
+  if (rcs > max_cluster || !resident_tile_map(nt, rcs, map_i, map_j)) return 0;
+  return rcs;
+}
+
+// L, Linv, rdiag, first (nt + 2 ints), then Cs at the next 256-byte boundary
 size_t chol_workspace_bytes(int n) {
   const size_t nt = (size_t)(n + kT - 1) / kT;
   const size_t ld = nt * kT;
   return ((nt + 1) * kT * ld + nt * kT * kT + nt * kT) * sizeof(double) + (nt + 2) * sizeof(int) + 256 +
-         (size_t)(kResMaxNt + 1) * kResMaxNt * sizeof(int) + (size_t)kResMaxNt * kT * kT * sizeof(double) + 256;
+         (size_t)kResMaxNt * kT * kT * sizeof(double);
 }
 
 // H [n][n] fp64, b [n] fp64 -> x [n] fp32; fail flag is a device int
@@ -1026,8 +990,7 @@ int chol_solve_launch(const double* H, const double* b, int n, double lm, double
   p.Linv = p.L + (size_t)(p.nt + 1) * kT * ld;
   p.rdiag = p.Linv + (size_t)p.nt * kT * kT;
   p.first = reinterpret_cast<int*>(p.rdiag + (size_t)p.nt * kT);
-  p.flags = p.first + (p.nt + 2);
-  p.Cs = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(p.flags + (kResMaxNt + 1) * kResMaxNt) + 255) & ~(uintptr_t)255);
+  p.Cs = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(p.first + (p.nt + 2)) + 255) & ~(uintptr_t)255);
 
   const size_t dyn_smem = ((size_t)2 * kCholWarps + 2) * kT * kTP * sizeof(double);
   static int cluster_size = 0;
@@ -1060,58 +1023,16 @@ int chol_solve_launch(const double* H, const double* b, int n, double lm, double
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
-  static unsigned long long* tbuf = nullptr;
-  static const bool want_timing = getenv("DBA_CHOL_TIMING") != nullptr;
-  p.timing = nullptr;
-  if (want_timing) {
-    if (!tbuf) cudaMallocHost(&tbuf, 4096 * sizeof(unsigned long long));
-    memset(tbuf, 0, 4096 * sizeof(unsigned long long));
-    if (8 + 16 * p.nt < 4096) p.timing = tbuf;
-  }
-  // resident-tile dataflow kernel: every tile needs its own warp
-  static const bool allow_resident = !(getenv("DBA_CHOL_RESIDENT") && atoi(getenv("DBA_CHOL_RESIDENT")) == 0);
-  const int res_tiles = p.nt * (p.nt + 1) / 2 + p.nt;
-  int rcs = 1;
-  while (rcs * kCholWarps < res_tiles || rcs < p.nt) rcs *= 2;
-  if (allow_resident && p.nt <= kResMaxNt && rcs <= cluster_size && resident_tile_map(p.nt, rcs, p.map_i, p.map_j)) {
+  // resident-tile dataflow kernel whenever it fits the cluster
+  const int rcs = resident_cluster_size(p.nt, cluster_size, p.map_i, p.map_j);
+  if (rcs > 0) {
     cfg.gridDim = dim3(rcs);
     at[0].val.clusterDim.x = rcs;
-    static const unsigned sl_u = getenv("DBA_CHOL_SLEEP_URGENT") ? (unsigned)atoi(getenv("DBA_CHOL_SLEEP_URGENT")) : 300u;
-    static const unsigned sl_i = getenv("DBA_CHOL_SLEEP_IDLE") ? (unsigned)atoi(getenv("DBA_CHOL_SLEEP_IDLE")) : 4000u;
-    p.sleep_urgent = sl_u; p.sleep_idle = sl_i;
-    static const int warm = getenv("DBA_CHOL_FUSED_SUBST") ? (atoi(getenv("DBA_CHOL_FUSED_SUBST")) ? 2 : 0) : 2;
-    p.warm = warm;
     if (p.peers.world > 1) DBA_CHECK_CUDA(cudaLaunchKernelEx(&cfg, chol_resident_kernel<true>, p), "chol_resident_kernel launch");
     else DBA_CHECK_CUDA(cudaLaunchKernelEx(&cfg, chol_resident_kernel<false>, p), "chol_resident_kernel launch");
-    if (p.timing) {
-      cudaStreamSynchronize(st);
-      const unsigned long long t0 = tbuf[0];
-      fprintf(stderr, "[chol resident timing] n=%d nt=%d cluster=%d  factor+forward %.1f us, backsub %.1f us\n", n, p.nt, rcs, (tbuf[4] - t0) / 1e3,
-              (tbuf[3] - tbuf[4]) / 1e3);
-      for (int k = 0; k < p.nt; k++) {
-        const unsigned long long* q = tbuf + 8 + 16 * k;
-        auto d = [&](int a, int b) { return (q[a] && q[b]) ? (double)((long long)q[a] - (long long)q[b]) / 1e3 : 0.0; };
-        fprintf(stderr, "  column %2d: diag: last update starts@%.1f wait+load %.1f mac %.1f transpose %.1f potrf %.1f store %.1f | (k+1,k): ready %+.1f after that, wait+load L_kk %.1f subst %.1f store %.1f\n",
-                k, q[8] ? (q[8] - t0) / 1e3 : 0.0, d(9, 8), d(10, 9), d(0, 10), d(7, 0), d(1, 7), d(2, 1), d(4, 2), d(5, 4), d(3, 5));
-        fprintf(stderr, "             y piece stored@%.1f   backward step done@%.1f   potrf: %llu SM cycles in %.2f us = %.0f MHz\n", q[11] ? (q[11] - t0) / 1e3 : 0.0,
-                q[12] ? (q[12] - t0) / 1e3 : 0.0, q[13], d(7, 0), d(7, 0) > 0 ? (double)q[13] / d(7, 0) : 0.0);
-      }
-    }
     return DBA_OK;
   }
   DBA_CHECK_CUDA(cudaLaunchKernelEx(&cfg, chol_cluster_kernel, p), "chol_cluster_kernel launch");
-  if (p.timing) {
-    cudaStreamSynchronize(st);
-    const unsigned long long t0 = tbuf[0];
-    fprintf(stderr, "[chol timing] n=%d nt=%d cluster=%d  load %.1f us, potrf0 %.1f us, total-to-backsub-end %.1f us\n", n, p.nt, cs, (tbuf[1] - t0) / 1e3,
-            (tbuf[2] - tbuf[1]) / 1e3, (tbuf[3] - t0) / 1e3);
-    for (int k = 0; k < p.nt; k++) {
-      const unsigned long long* q = tbuf + 8 + 8 * k;
-      fprintf(stderr, "  panel %2d: Lkk-load@%.1f trsm(cta0) %.1f  barrier %.1f  update(cta0 thread0) %.1f  inv+barrier %.1f | diag tile: coop-update %.1f potrf %.1f\n", k,
-              (q[0] - t0) / 1e3, (q[1] - q[0]) / 1e3, (q[2] - q[1]) / 1e3, (q[3] - q[2]) / 1e3, (q[4] - q[3]) / 1e3,
-              q[5] ? (q[5] - q[2]) / 1e3 : 0.0, q[6] ? (q[6] - q[5]) / 1e3 : 0.0);
-    }
-  }
   return DBA_OK;
 }
 
@@ -1121,13 +1042,7 @@ int chol_solve_launch(const double* H, const double* b, int n, double lm, double
 // map_i / map_j [128] receive the tile of every warp slot (0xFF = none); returns the cluster size, 0 if n is served by the barrier kernel
 extern "C" int dba_solve_tile_placement(int n, unsigned char* map_i, unsigned char* map_j) {
   if (n <= 0 || !map_i || !map_j) return 0;
-  const int nt = (n + dba::kT - 1) / dba::kT;
-  if (nt > dba::kResMaxNt) return 0;
-  const int tiles = nt * (nt + 1) / 2 + nt;
-  int rcs = 1;
-  while (rcs * dba::kCholWarps < tiles || rcs < nt) rcs *= 2;
-  if (rcs > 16 || !dba::resident_tile_map(nt, rcs, map_i, map_j)) return 0;
-  return rcs;
+  return dba::resident_cluster_size((n + dba::kT - 1) / dba::kT, 16, map_i, map_j);
 }
 
 // standalone entry (used by the solver tests and by callers that already hold a reduced system)

@@ -24,7 +24,6 @@
 #include "wgmma.cuh"
 #include <cuda.h>
 #include <string.h>
-#include <stdlib.h>
 
 namespace dba {
 
@@ -545,10 +544,6 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   // L2 -> SM traffic per MAC; bounded by the register accumulators (MT * N <= 256 columns) and by the image height
   p.MT = (p.HT >= 2 * p.RM) ? 2 : 1;
   if (p.N <= 64 && p.HT >= 4 * p.RM && (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0) >= 4 && p.KS == 3) p.MT = 4;
-  static const int ov_mt = getenv("DBA_CONV_MT") ? atoi(getenv("DBA_CONV_MT")) : 0;          // experiment switches (tools/conv_bench.py)
-  static const int ov_as = getenv("DBA_CONV_ASTAGES") ? atoi(getenv("DBA_CONV_ASTAGES")) : 0;
-  static const int ov_bs = getenv("DBA_CONV_BSTAGES") ? atoi(getenv("DBA_CONV_BSTAGES")) : 0;
-  if (ov_mt > 0) p.MT = ov_mt;
   if (p.MT > conv_max_mt(p.N)) p.MT = conv_max_mt(p.N);
   p.tiles_x = (p.WD + p.TW - 1) / p.TW;
   p.tiles_y = (p.HT + p.MT * p.RM - 1) / (p.MT * p.RM);
@@ -563,10 +558,8 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   const int budget = 227 * 1024 - 2048;
   p.a_stages = 2;
   while (p.a_stages < 4 && (p.a_stages + 1) * p.a_bytes + 4 * p.b_bytes <= budget) p.a_stages++;
-  if (ov_as > 0 && ov_as <= 4) p.a_stages = ov_as;
   p.b_stages = (budget - p.a_stages * p.a_bytes) / p.b_bytes;
   if (p.b_stages > 8) p.b_stages = 8;
-  if (ov_bs > 0 && ov_bs <= 8 && p.a_stages * p.a_bytes + ov_bs * p.b_bytes <= budget) p.b_stages = ov_bs;
   if (p.b_stages < 2) { set_error("update operator: tile does not fit shared memory"); return DBA_ERR_INVALID; }
   p.slots = p.tiles_x * p.tiles_y * p.MT * kSlotsPerMTile;
   if (slots_out) *slots_out = p.slots;

@@ -123,7 +123,8 @@ def test_stress_shape_72x96_bf16_and_ba(backends):
 def _mixed_degree_graph(N=34):
     """frames with 3-5 rows (packed tensor-core tiles), 16 rows (one tile per 32 pixels) and 25 rows (CUDA-core tile pairs),
     plus a duplicated edge: every Schur kernel and the duplicate-pose rule (both (r,c) and (c,r) land on one diagonal block).
-    The extra edges stay within 12 frames so that the problem is as well conditioned as a covisibility graph."""
+    With HW % 4 != 0 the same graph runs the CUDA-core kernels instead: 3-5 and 16 rows on ba_schur_small_kernel, 25 rows on
+    ba_schur_gemm_kernel.  The extra edges stay within 12 frames so that the problem is as well conditioned as a covisibility graph."""
     e = []
     for i in range(N):
         for j in (i - 2, i - 1, i + 1, i + 2):
@@ -135,9 +136,9 @@ def _mixed_degree_graph(N=34):
     return [a for a, _ in e], [b for _, b in e]
 
 
-def test_ba_every_schur_kernel_matches_oracle(backends):
+def _mixed_degree_ba_matches_oracle(backends, ht, wd):
     ii, jj = _mixed_degree_graph()
-    s = synth.make_scene(dict(E=len(ii), N=34, ht=48, wd=64, stereo=False, itrs=2, lm=1e-4, ep=0.1, graph=(ii, jj)), seed=1)
+    s = synth.make_scene(dict(E=len(ii), N=34, ht=ht, wd=wd, stereo=False, itrs=2, lm=1e-4, ep=0.1, graph=(ii, jj)), seed=1)
     deg = torch.bincount(s["ii"], minlength=34)
     assert int(deg[17]) == 24 and int(deg[26]) == 15 and int(deg.min()) >= 2
     torch.set_num_threads(min(16, torch.get_num_threads()))
@@ -148,6 +149,16 @@ def test_ba_every_schur_kernel_matches_oracle(backends):
     oracle.ba(P64, D64, s["intrinsics"], s["disps_sens"], s["targets"], s["weights"], s["eta"], s["ii"], s["jj"], s["t0"], s["t1"], 2,
               s["lm"], s["ep"], False, dtype=torch.float64)
     assert rel_err(P, P64, floor=1.0) < 1e-4 and rel_err(D, D64, floor=1.0) < 1e-4
+
+
+def test_ba_every_schur_kernel_matches_oracle(backends):
+    _mixed_degree_ba_matches_oracle(backends, 48, 64)
+
+
+def test_ba_cuda_core_schur_kernels_match_oracle(backends):
+    """47x63: HW % 4 != 0, so the pixel rows are not 16-byte aligned and the same graph runs ba_schur_small_kernel and
+    ba_schur_gemm_kernel instead of the tensor-core kernels"""
+    _mixed_degree_ba_matches_oracle(backends, 47, 63)
 
 
 @pytest.mark.parametrize("N,res", [(40, (24, 32)), (30, (48, 64))])

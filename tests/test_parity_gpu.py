@@ -403,7 +403,7 @@ def test_fused_reproject_matches_projective_transform_restatement(backends):
     assert 0.05 < float(rv.mean()) < 1.0 and bool((s["ii"] == s["jj"]).any())
 
 
-def test_fused_p2p_reduction_two_virtual_ranks_on_one_gpu(backends):
+def _fused_p2p_two_virtual_ranks(backends, s):
     """The cross-GPU reduction fused into the Cholesky kernel (DESIGN.md section 6), exercised on ONE device: two edge shards
     ("ranks") build their partial pose systems into two buffers that play the role of peer memory, publish their epochs, and each
     rank's solve sums both copies itself.  Result must match the unsharded BA and be identical on both ranks."""
@@ -414,7 +414,6 @@ def test_fused_p2p_reduction_two_virtual_ranks_on_one_gpu(backends):
             self.nd, self.ptrs, self.world, self.rank, self.epoch = nd, ptrs, len(ptrs), rank, 0
             self.epoch_dev = torch.zeros(1, dtype=torch.int64, device=dev)
 
-    s = synth.make_scene("c2_frontend")
     N, ht, wd = s["disps"].shape
     n = 6 * (s["t1"] - s["t0"]); nd = n * n + n
     bufs = [torch.zeros(2 * nd + 8, dtype=torch.float64, device=dev) for _ in range(2)]
@@ -444,3 +443,15 @@ def test_fused_p2p_reduction_two_virtual_ranks_on_one_gpu(backends):
     args = [s[k].to(dev) for k in ("intrinsics", "disps_sens", "targets", "weights", "eta", "ii", "jj")]
     backends.ba(P1, D1, *args, s["t0"], s["t1"], 2, s["lm"], s["ep"], False)
     assert float((s0["P"] - P1).abs().max()) < 2e-5 and float((D - D1).abs().max()) < 5e-5
+
+
+def test_fused_p2p_reduction_two_virtual_ranks_on_one_gpu(backends):
+    """the fused reduction on a frontend window (n = 144): resident Cholesky kernel"""
+    _fused_p2p_two_virtual_ranks(backends, synth.make_scene("c2_frontend"))
+
+
+def test_fused_p2p_reduction_cluster_kernel_two_virtual_ranks(backends):
+    """the fused reduction on a 100-frame window at 24x32 (n = 594 > 448): the cluster Cholesky kernel's peer loader"""
+    s = synth.make_scene(dict(E=400, N=100, ht=24, wd=32, stereo=False, itrs=2, lm=1e-4, ep=0.1))
+    assert 448 < 6 * (s["t1"] - s["t0"]) <= 1024
+    _fused_p2p_two_virtual_ranks(backends, s)

@@ -1,5 +1,5 @@
 """Distribution of the elementwise deviation between this build's ba and the reference build's ba (oracle/_ref) on the same GPU,
-and of both against the fp64 CPU oracle where that is affordable.  Output -> profiles/r2_ba_vs_reference_stats.txt"""
+and of both against the fp64 CPU oracle where that is affordable; prints quantiles of each."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))

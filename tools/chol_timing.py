@@ -1,6 +1,6 @@
-"""Per-phase timing of the damped SPD solve (in-kernel %globaltimer stamps printed by the library when DBA_CHOL_TIMING=1) followed by a
-CUDA-event timing of 200 back-to-back solves without the stamps.  usage: python tools/chol_timing.py [n]   (DBA_CHOL_RESIDENT=0 selects
-the barrier kernel for n <= 448)."""
+"""CUDA-event timing of the damped SPD solve (`dba_solve_spd`): 20 warm-up solves, then 200 back-to-back solves of one seeded system,
+printed with the card's name and power limit.  usage: python tools/chol_timing.py [n ...]   (default 426; n <= 448 runs the resident
+kernel, larger n the cluster kernel)."""
 import ctypes
 import os
 import subprocess
@@ -8,46 +8,58 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-n = int(sys.argv[1]) if len(sys.argv) > 1 else 426
-if len(sys.argv) <= 2:       # first a child with the stamps on, then this process without them
-    env = dict(os.environ, DBA_CHOL_TIMING="1")
-    subprocess.run([sys.executable, os.path.abspath(__file__), str(n), "stamps"], env=env)
 import torch  # noqa: E402
 from droid_slam_b200 import c_api  # noqa: E402
 
-L = c_api.load()
-g = torch.Generator().manual_seed(0)
-A = torch.randn(n, n + 8, generator=g, dtype=torch.float64)
-Hc = A @ A.t() + 1e-3 * torch.eye(n, dtype=torch.float64)
-bc = torch.randn(n, generator=g, dtype=torch.float64)
-H, b = Hc.cuda(), bc.cuda()
-ws = torch.empty(L.dba_solve_workspace_bytes(n), dtype=torch.uint8, device="cuda")
-x = torch.zeros(n, device="cuda")
-fail = torch.zeros(1, dtype=torch.int32, device="cuda")
+
+def power_limit_w():
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return "%.0f W" % float(out)
+    except (OSError, ValueError, subprocess.SubprocessError):
+        return "unknown"
 
 
-def solve():
-    L.dba_solve_spd(ctypes.c_void_p(H.data_ptr()), ctypes.c_void_p(b.data_ptr()), n, ctypes.c_float(1e-4), ctypes.c_float(0.1), ctypes.c_void_p(x.data_ptr()),
-                    ctypes.c_void_p(fail.data_ptr()), ctypes.c_void_p(ws.data_ptr()), ws.numel(), None)
+def time_solve(L, n):
+    g = torch.Generator().manual_seed(0)
+    A = torch.randn(n, n + 8, generator=g, dtype=torch.float64)
+    Hc = A @ A.t() + 1e-3 * torch.eye(n, dtype=torch.float64)
+    bc = torch.randn(n, generator=g, dtype=torch.float64)
+    H, b = Hc.cuda(), bc.cuda()
+    ws = torch.empty(L.dba_solve_workspace_bytes(n), dtype=torch.uint8, device="cuda")
+    x = torch.zeros(n, device="cuda")
+    fail = torch.zeros(1, dtype=torch.int32, device="cuda")
 
+    def solve():
+        c_api.check(L.dba_solve_spd(ctypes.c_void_p(H.data_ptr()), ctypes.c_void_p(b.data_ptr()), n, ctypes.c_float(1e-4), ctypes.c_float(0.1),
+                                    ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(fail.data_ptr()), ctypes.c_void_p(ws.data_ptr()), ws.numel(), None),
+                    "dba_solve_spd")
 
-if len(sys.argv) > 2:
-    for it in range(3):
+    for _ in range(20):
         solve()
-        torch.cuda.synchronize()
-    sys.exit(0)
-for it in range(20):
-    solve()
-torch.cuda.synchronize()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-for it in range(200):
-    solve()
-e1.record()
-torch.cuda.synchronize()
-Hd = Hc.clone()
-Hd.diagonal().add_(0.1 + 1e-4 * Hc.diagonal())
-ref = torch.linalg.solve(Hd, bc)
-err = float((x.cpu().double() - ref).abs().max() / ref.abs().max())
-print("n=%d  %s kernel: %.1f us per solve (200 back-to-back), fail=%d, max rel err vs fp64 LAPACK %.2e"
-      % (n, "barrier" if os.environ.get("DBA_CHOL_RESIDENT") == "0" or n > 448 else "resident", 1e3 * e0.elapsed_time(e1) / 200, int(fail), err))
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(200):
+        solve()
+    e1.record()
+    torch.cuda.synchronize()
+    Hd = Hc.clone()
+    Hd.diagonal().add_(0.1 + 1e-4 * Hc.diagonal())
+    ref = torch.linalg.solve(Hd, bc)
+    err = float((x.cpu().double() - ref).abs().max() / ref.abs().max())
+    return 1e3 * e0.elapsed_time(e1) / 200, int(fail), err
+
+
+def main():
+    L = c_api.load()
+    card = "%s, power limit %s" % (torch.cuda.get_device_name(), power_limit_w())
+    for n in [int(a) for a in sys.argv[1:]] or [426]:
+        us, fail, err = time_solve(L, n)
+        print("n=%d  %s kernel: %.1f us per solve (200 back-to-back), fail=%d, max rel err vs fp64 LAPACK %.2e  [%s]"
+              % (n, "resident" if n <= 448 else "cluster", us, fail, err, card))
+
+
+if __name__ == "__main__":
+    main()

@@ -1,5 +1,5 @@
-"""Two calls of the tensor-core update operator at E edges (env UPD_E, default 256), 48x64 -- the command ncu wraps
-(profiles/r2_update_*): the first call is the warm-up, the second the profiled one."""
+"""Two calls of the tensor-core update operator at E edges (env UPD_E, default 256), 48x64, for a profiler to wrap: the first call is
+the warm-up, the second the profiled one."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
