@@ -35,9 +35,14 @@ struct Layout {
 
 __host__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Stride of the workspace's per-pixel rows (Eij [E][6][pitch], C and w [M][pitch], Ei [M][6][pitch]): HW rounded up to 4 floats,
+// so that every row starts on a 16-byte boundary for the tensor-core Schur kernel's cp.async / float4 loads.  Pixels [HW, pitch)
+// are zeroed by ba_prepare_kernel and never written again.  Caller tensors (disps, targets, weights, eta, dz_out) keep the stride HW.
+__host__ __device__ __forceinline__ int ba_pitch(int HW) { return (HW + 3) & ~3; }
+
 __host__ inline Layout make_layout(int N, int E, int ht, int wd, int t0, int t1) {
   Layout L;
-  const size_t HW = (size_t)ht * wd;
+  const size_t pitch = (size_t)ba_pitch(ht * wd);
   L.P = t1 - t0 > 0 ? t1 - t0 : 0;
   L.n = 6 * L.P;
   size_t o = 0;
@@ -50,11 +55,11 @@ __host__ inline Layout make_layout(int N, int E, int ht, int wd, int t0, int t1)
   L.off_sys = o;      o = align_up(o + ((size_t)L.n * L.n + L.n) * sizeof(double), 256);
   L.off_L = o;        o = align_up(o + chol_workspace_bytes(L.n), 256);
   L.off_dx = o;       o = align_up(o + (size_t)(L.n + 6) * sizeof(float), 256);
-  L.off_Eij = o;      o = align_up(o + (size_t)E * 6 * HW * sizeof(float), 256);
+  L.off_Eij = o;      o = align_up(o + (size_t)E * 6 * pitch * sizeof(float), 256);
   const size_t Mmax = (size_t)N;   // at most one depth frame per buffer frame
-  L.off_C = o;        o = align_up(o + Mmax * HW * sizeof(float), 256);
-  L.off_w = o;        o = align_up(o + Mmax * HW * sizeof(float), 256);
-  L.off_Ei = o;       o = align_up(o + Mmax * 6 * HW * sizeof(float), 256);
+  L.off_C = o;        o = align_up(o + Mmax * pitch * sizeof(float), 256);
+  L.off_w = o;        o = align_up(o + Mmax * pitch * sizeof(float), 256);
+  L.off_Ei = o;       o = align_up(o + Mmax * 6 * pitch * sizeof(float), 256);
   L.total = o;
   return L;
 }
@@ -68,11 +73,24 @@ enum { ST_BAD_INDEX = 1, ST_ETA_ROWS = 2, ST_CHOL_FAIL = 4, ST_DEGREE = 8 };
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restrict__ ii, const int64_t* __restrict__ jj, int E, int N,
                                                           int t0, int t1, int eta_rows, int* __restrict__ hdr,
-                                                          int* __restrict__ frame2k, int* __restrict__ kx, int* __restrict__ rowptr, int* __restrict__ big) {
+                                                          int* __restrict__ frame2k, int* __restrict__ kx, int* __restrict__ rowptr, int* __restrict__ big,
+                                                          int HW, float* __restrict__ Eij, float* __restrict__ C, float* __restrict__ w,
+                                                          float* __restrict__ Ei) {
   __shared__ int s_scan[1024];
   __shared__ int s_carry;
   const int tid = threadIdx.x;
   if (tid == 0) { hdr[HDR_STATUS] = 0; hdr[HDR_CHOL_FAIL] = 0; }
+  // pad pixels [HW, pitch) of the per-pixel rows Eij [6E], C [N], w [N], Ei [6N]: the tensor-core Schur kernel reads them with the
+  // last 16-byte piece of a row, so they must be finite, and nothing else writes them
+  const int pitch = ba_pitch(HW);
+  if (pitch != HW) {
+    for (int r = tid; r < 6 * E + 8 * N; r += blockDim.x) {
+      const int k = r - 6 * E;
+      float* row = k < 0 ? Eij + (size_t)r * pitch : k < N ? C + (size_t)k * pitch : k < 2 * N ? w + (size_t)(k - N) * pitch
+                 : Ei + (size_t)(k - 2 * N) * pitch;
+      for (int p = HW; p < pitch; p++) row[p] = 0.f;
+    }
+  }
   for (int f = tid; f < N; f += blockDim.x) { frame2k[f] = (f >= t0 && f < t1) ? 1 : 0; rowptr[f] = 0; }
   if (tid == 0) { rowptr[N] = 0; rowptr[N + 1] = 0; }
   __syncthreads();
@@ -238,6 +256,7 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
 
   const float fx = __ldg(intr), fy = __ldg(intr + 1), cx = __ldg(intr + 2), cy = __ldg(intr + 3);
   const int n = 6 * P;
+  const int pitch = ba_pitch(HW);
 
   // this thread's pixels
   int pix[kPPT];
@@ -350,7 +369,7 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
           for (int c = 0; c < 6; c++) Ej[c] = au * Ju[c] + av * Jv[c];
           if (!motion_only) {
 #pragma unroll
-            for (int c = 0; c < 6; c++) Eij[((size_t)e * 6 + c) * HW + p] = Ej[c];
+            for (int c = 0; c < 6; c++) Eij[((size_t)e * 6 + c) * pitch + p] = Ej[c];
             // Eii = -A Eij, accumulated over the out-edges of this frame
 #pragma unroll
             for (int r = 0; r < 6; r++) {
@@ -441,10 +460,10 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
         const float mk = (dsn > 0.f) ? 1.f : 0.f;
         const float C = Cacc[s] + mk * alpha + (1 - mk) * __ldg(eta + (size_t)erow * HW + p);
         const float w = wacc[s] - mk * alpha * (dsp[s] - dsn);
-        Cout[(size_t)m * HW + p] = C;
-        wout[(size_t)m * HW + p] = w;
+        Cout[(size_t)m * pitch + p] = C;
+        wout[(size_t)m * pitch + p] = w;
 #pragma unroll
-        for (int c = 0; c < 6; c++) Eiout[((size_t)m * 6 + c) * HW + p] = Eiacc[s][c];
+        for (int c = 0; c < 6; c++) Eiout[((size_t)m * 6 + c) * pitch + p] = Eiacc[s][c];
       }
     }
   }
@@ -454,10 +473,14 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
 // Schur complement:  Hsys -= sum_k E_k Q_k E_k^T ,  bsys -= sum_k E_k Q_k w_k       (reference K9/K10 + schur_block)
 // rows of frame k: (pose k, Ei_k) if k is in [t0,t1), then (pose jj[e], Eij[e]) for the out-edges e of k; rows whose pose
 // is outside [t0,t1) are dropped (they contribute nothing, reference :1155,:1257).
-// Two kernels share the work: ba_schur_small_kernel (frames with <= 16 rows, the usual case) and ba_schur_gemm_kernel (more rows:
-// dense graphs, edge-sharded ranks).  Both keep 6x6 block pairs in registers over a whole pixel chunk, accumulate in fp32 like the
-// reference and flush once with fp64 atomics into the LOWER triangle of the reduced system.
+// The rows of a frame decide the kernel, for every image size (the workspace rows are padded to ba_pitch, i.e. 16-byte aligned):
+//   <= kTcRowsMax rows (every frame of a sliding-window graph)   ba_schur_tc_kernel<false>: tensor cores, packed or single tile
+//   kTcRowsMax+1 .. kPairRowsMax rows (dense graphs, sharded)    ba_schur_tc_kernel<true>:  tensor cores, pairs of row tiles
+//   more rows                                                    ba_schur_gemm_kernel:      SIMT fp32 block pairs
+// Each flushes once with fp64 atomics into the LOWER triangle of the reduced system.
 // ---------------------------------------------------------------------------------------------------------
+constexpr int kTcRowsMax = 21;
+constexpr int kPairRowsMax = 100;
 // Q = 1/C of the eliminated depth block.  C <= 0 only for a pixel with eta = 0 and no weight on any edge; the reference divides
 // anyway (inf -> NaN system -> zero pose update and NaN depths at that pixel).  All Schur kernels and the back-substitution here
 // drop such a pixel instead (Q = 0, dz = 0): one rule on every path, documented in INTEGRATION.md.
@@ -470,7 +493,7 @@ constexpr int kSchurMaxRows = 255;   // rows per frame (out-degree + 1); larger 
 // ballot compaction keeps the reference's row order.  Ends with a __syncthreads().
 template <int kThreads>
 __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ edgeidx,
-                                               int e_begin, int deg, int ix, int m, int HW, int t0, int P, const float* __restrict__ Eij,
+                                               int e_begin, int deg, int ix, int m, int pitch, int t0, int P, const float* __restrict__ Eij,
                                                const float* __restrict__ Eiin, int* s_pose, const float** s_ptr, int* s_nrows, int* s_wcount) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool self = (ix >= t0 && ix < t0 + P);
@@ -484,10 +507,10 @@ __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, i
   for (int w = 0; w < warp; w++) base += s_wcount[w];
   if (keep) {
     const int pos = base + __popc(bal & ((1u << lane) - 1u));
-    s_pose[pos] = pj; s_ptr[pos] = Eij + (size_t)e * 6 * HW;
+    s_pose[pos] = pj; s_ptr[pos] = Eij + (size_t)e * 6 * pitch;
   }
   if (tid == 0) {
-    if (self) { s_pose[0] = ix - t0; s_ptr[0] = Eiin + (size_t)m * 6 * HW; }
+    if (self) { s_pose[0] = ix - t0; s_ptr[0] = Eiin + (size_t)m * 6 * pitch; }
     int tot = self ? 1 : 0;
     for (int w = 0; w < kThreads / 32; w++) tot += s_wcount[w];
     *s_nrows = tot;
@@ -497,7 +520,7 @@ __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, i
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Schur complement for frames with many rows (dense graphs / edge-sharded ranks: out-degree >> 12): SGEMM-style kernel.
+// Schur complement for frames with more than kPairRowsMax rows (dense graphs / edge-sharded ranks): SGEMM-style kernel.
 // C = A diag(Q) A^T with A = [6R x pixels].  A CTA computes one 16-row x 16-row tile pair (96 x 96 scalars) for a pixel
 // chunk: thread (ty,tx) owns the 6x6 block pair (row 16*ti+ty, row 16*tj+tx) in registers for the WHOLE chunk (no per-tile
 // reductions), the K loop walks 64-pixel shared-memory tiles stored pixel-major so that a thread reads its 6+6 operands as
@@ -510,7 +533,7 @@ constexpr int kSgThreads = 256;
 
 __global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
     const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
-    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta, int min_rows,
+    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta,
     const float* __restrict__ Eij, const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
     double* __restrict__ Hsys, double* __restrict__ bsys) {
   const int m = blockIdx.y;
@@ -521,6 +544,7 @@ __global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int ty = tid >> 4, tx = tid & 15;
   const int n = 6 * P;
+  const int pitch = ba_pitch(HW);
 
   __shared__ int s_pose[kSchurMaxRows + 1];
   __shared__ const float* s_ptr[kSchurMaxRows + 1];
@@ -532,10 +556,10 @@ __global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
   __shared__ float sQw[kSgK];
   __shared__ float sQ[kSgK];
 
-  if (deg + 1 <= min_rows) return;                     // at most deg + 1 rows: not this kernel's frame (skips the row-list build)
-  build_row_list<kSgThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, HW, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
+  if (deg + 1 <= kPairRowsMax) return;                 // at most deg + 1 rows: not this kernel's frame (skips the row-list build)
+  build_row_list<kSgThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
   const int nrows = s_nrows;
-  if (nrows <= min_rows) return;                       // smaller frames belong to ba_schur_tc_kernel / ba_schur_small_kernel
+  if (nrows <= kPairRowsMax) return;                   // smaller frames belong to ba_schur_tc_kernel
   const int nT = (nrows + kSgRows - 1) / kSgRows;
   const int npairs = nT * (nT + 1) / 2;
   const int px_begin = blockIdx.x * px_per_cta;
@@ -563,16 +587,16 @@ __global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
       // ---- stage: A tile scaled by Q, B tile raw; one warp per (row, component) line of 64 pixels, transposed into [px][row*6+c]
       for (int px = tid; px < kSgK; px += kSgThreads) {
         const bool okp = px < np;
-        const float q = okp ? safe_rcp(__ldg(Cin + (size_t)m * HW + p0 + px)) : 0.f;
+        const float q = okp ? safe_rcp(__ldg(Cin + (size_t)m * pitch + p0 + px)) : 0.f;
         sQ[px] = q;
-        sQw[px] = okp ? __ldg(win + (size_t)m * HW + p0 + px) : 0.f;
+        sQw[px] = okp ? __ldg(win + (size_t)m * pitch + p0 + px) : 0.f;
       }
       __syncthreads();
       for (int ln = warp; ln < (ra + (diag_tile ? 0 : rb)) * 6; ln += kSgThreads / 32) {
         const int rowl = ln / 6, c = ln - rowl * 6;
         const bool second = rowl >= ra;
         const int row = second ? (tj * kSgRows + rowl - ra) : (ti * kSgRows + rowl);
-        const float* src = s_ptr[row] + (size_t)c * HW + p0;
+        const float* src = s_ptr[row] + (size_t)c * pitch + p0;
         float* dst = (second ? sB : sA) + (second ? rowl - ra : rowl) * 6 + c;
 #pragma unroll
         for (int h = 0; h < kSgK / 32; h++) {
@@ -638,165 +662,7 @@ __global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Schur complement for frames with at most 16 rows (the usual case: out-degree + 1): the same register-resident 6x6 block pairs
-// as the SGEMM-style kernel, but the T = R(R+1)/2 pairs of a frame do not fill a CTA, so the 256 threads form G = 256/T groups
-// that split the pixels of every 64-pixel tile (a K split); the groups' partial blocks meet once in shared memory at the end and
-// the CTA flushes T x 42 values with fp64 atomics.  The next tile travels global -> registers while the current one is being
-// multiplied (36 FMA per 6 LDS.64 per pixel and thread).
-// ---------------------------------------------------------------------------------------------------------
-constexpr int kSsLines = (kSgRows * 6) / (kSgThreads / 32);     // (row, component) lines per warp: 12
-
-__global__ void __launch_bounds__(kSgThreads, 2) ba_schur_small_kernel(
-    const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
-    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta,
-    const float* __restrict__ Eij, const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
-    double* __restrict__ Hsys, double* __restrict__ bsys) {
-  const int m = blockIdx.y;
-  if (m >= hdr[HDR_M]) return;
-  const int ix = kx[m];
-  const int e_begin = rowptr[m];
-  const int deg = rowptr[m + 1] - e_begin;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = 6 * P;
-
-  __shared__ int s_pose[kSchurMaxRows + 1];
-  __shared__ const float* s_ptr[kSchurMaxRows + 1];
-  __shared__ int s_nrows;
-  __shared__ int s_wcount[kSgThreads / 32];
-  extern __shared__ float sg_dyn[];
-  float* sA = sg_dyn;                                  // [64 px][98]: rows scaled by Q = 1/C
-  float* sB = sg_dyn + kSgK * kSgStride;               // raw rows
-  __shared__ float sQw[kSgK];
-
-  build_row_list<kSgThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, HW, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
-  const int nrows = s_nrows;
-  if (nrows == 0 || nrows > kSgRows) return;           // larger frames belong to ba_schur_gemm_kernel
-  const int px_begin = blockIdx.x * px_per_cta;
-  const int px_end = min(HW, px_begin + px_per_cta);
-  if (px_begin >= px_end) return;
-
-  const int T = nrows * (nrows + 1) / 2;
-  const int G = kSgThreads / T;                        // T <= 136 -> G >= 1
-  const int g = tid / T;
-  const int pr = tid - g * T;
-  const bool active = g < G;
-  int ty = (int)((sqrtf(8.f * (float)pr + 1.f) - 1.f) * 0.5f);       // pr -> (ty >= tx)
-  while (ty * (ty + 1) / 2 > pr) ty--;
-  while ((ty + 1) * (ty + 2) / 2 <= pr) ty++;
-  const int tx = pr - ty * (ty + 1) / 2;
-  const bool diag_pair = (ty == tx);
-  const int nlines = nrows * 6;
-
-  float acc[36], bacc[6];
-#pragma unroll
-  for (int k = 0; k < 36; k++) acc[k] = 0.f;
-#pragma unroll
-  for (int k = 0; k < 6; k++) bacc[k] = 0.f;
-
-  float pre[kSsLines][2], q0, q1, w0, w1;
-  auto load_tile = [&](int p0) {
-    const int np = min(kSgK, px_end - p0);
-    const bool ok0 = lane < np, ok1 = lane + 32 < np;
-    const size_t base = (size_t)m * HW + p0;
-    q0 = ok0 ? safe_rcp(__ldg(Cin + base + lane)) : 0.f;
-    q1 = ok1 ? safe_rcp(__ldg(Cin + base + lane + 32)) : 0.f;
-    w0 = ok0 ? __ldg(win + base + lane) : 0.f;
-    w1 = ok1 ? __ldg(win + base + lane + 32) : 0.f;
-#pragma unroll
-    for (int i = 0; i < kSsLines; i++) {
-      const int ln = warp + (kSgThreads / 32) * i;
-      pre[i][0] = 0.f; pre[i][1] = 0.f;
-      if (ln < nlines) {
-        const int rowl = ln / 6, c = ln - rowl * 6;
-        const float* src = s_ptr[rowl] + (size_t)c * HW + p0;
-        if (ok0) pre[i][0] = __ldg(src + lane);
-        if (ok1) pre[i][1] = __ldg(src + lane + 32);
-      }
-    }
-  };
-
-  load_tile(px_begin);
-  for (int p0 = px_begin; p0 < px_end; p0 += kSgK) {
-    __syncthreads();                                   // the previous tile has been consumed
-#pragma unroll
-    for (int i = 0; i < kSsLines; i++) {
-      const int ln = warp + (kSgThreads / 32) * i;
-      if (ln < nlines) {
-        const int o = ln;                              // = row * 6 + component
-        sB[lane * kSgStride + o] = pre[i][0];
-        sB[(lane + 32) * kSgStride + o] = pre[i][1];
-        sA[lane * kSgStride + o] = pre[i][0] * q0;     // ei = E*q   (reference K9)
-        sA[(lane + 32) * kSgStride + o] = pre[i][1] * q1;
-      }
-    }
-    if (warp == 0) { sQw[lane] = w0; sQw[lane + 32] = w1; }
-    __syncthreads();
-    if (p0 + kSgK < px_end) load_tile(p0 + kSgK);      // in flight while this tile is multiplied
-    if (active) {
-      const float* pa = sA + ty * 6;
-      const float* pb = sB + tx * 6;
-#pragma unroll 2
-      for (int px = g; px < kSgK; px += G) {
-        const float2 a01 = *reinterpret_cast<const float2*>(pa + px * kSgStride);
-        const float2 a23 = *reinterpret_cast<const float2*>(pa + px * kSgStride + 2);
-        const float2 a45 = *reinterpret_cast<const float2*>(pa + px * kSgStride + 4);
-        const float2 b01 = *reinterpret_cast<const float2*>(pb + px * kSgStride);
-        const float2 b23 = *reinterpret_cast<const float2*>(pb + px * kSgStride + 2);
-        const float2 b45 = *reinterpret_cast<const float2*>(pb + px * kSgStride + 4);
-        const float ea[6] = {a01.x, a01.y, a23.x, a23.y, a45.x, a45.y};
-        const float eb[6] = {b01.x, b01.y, b23.x, b23.y, b45.x, b45.y};
-#pragma unroll
-        for (int a = 0; a < 6; a++)
-#pragma unroll
-          for (int c = 0; c < 6; c++) acc[a * 6 + c] += ea[a] * eb[c];
-        if (diag_pair) {
-          const float w = sQw[px];                     // (Q E) w = Q w E
-#pragma unroll
-          for (int c = 0; c < 6; c++) bacc[c] += w * ea[c];
-        }
-      }
-    }
-  }
-  // ---- the G pixel groups meet in shared memory (the staging area is free now), then one flush into the lower triangle
-  __syncthreads();
-  float* red = sg_dyn;                                 // [G][T][42]
-  if (active) {
-    float* dst = red + (size_t)(g * T + pr) * 42;
-#pragma unroll
-    for (int k = 0; k < 36; k++) dst[k] = acc[k];
-#pragma unroll
-    for (int k = 0; k < 6; k++) dst[36 + k] = bacc[k];
-  }
-  __syncthreads();
-  for (int k = tid; k < T * 42; k += kSgThreads) {
-    const int q = k / 42, o = k - q * 42;
-    int r2 = (int)((sqrtf(8.f * (float)q + 1.f) - 1.f) * 0.5f);
-    while (r2 * (r2 + 1) / 2 > q) r2--;
-    while ((r2 + 1) * (r2 + 2) / 2 <= q) r2++;
-    const int r = q - r2 * (r2 + 1) / 2;
-    const bool same_row = (r == r2);
-    if (o >= 36 && !same_row) continue;
-    float sum = 0.f;
-    for (int gg = 0; gg < G; gg++) sum += red[(size_t)(gg * T + q) * 42 + o];
-    const double v = -(double)sum;
-    const int pa_ = s_pose[r2], pb_ = s_pose[r];       // block S(pa_, pb_)[a][c]; its transpose sits at (pb_, pa_)[c][a]
-    if (o < 36) {
-      const int a = o / 6, c = o - a * 6;
-      const int gr = pa_ * 6 + a, gc = pb_ * 6 + c;
-      if (same_row) {
-        if (gr >= gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
-      } else {
-        if (gr >= gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
-        if (gc >= gr) atomicAdd(&Hsys[(size_t)gc * n + gr], v);
-      }
-    } else {
-      atomicAdd(&bsys[pa_ * 6 + (o - 36)], v);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Schur complement on the tensor cores (frames with at most 21 rows, i.e. every frame of a sliding-window graph):
+// Schur complement on the tensor cores (frames with at most kTcRowsMax rows; PAIR mode below: up to kPairRowsMax rows):
 //   S = X X^T  with  X = [ E_r / sqrt(C) ; w / sqrt(C) ]  (6R + 1 rows x pixels),  so that S[:6R,:6R] = sum E q E^T and
 //   S[:6R, 6R] = sum E q w  -- one symmetric rank-K update per frame, K = pixels.
 // fp32 accuracy on the tf32 pipe by operand splitting (3xTF32): x = hi + lo with hi = tf32(x), lo = x - hi (exact), and
@@ -813,11 +679,11 @@ __global__ void __launch_bounds__(kSgThreads, 2) ba_schur_small_kernel(
 // Frames with 6R + 2 <= 64 (R <= 10) run "packed": the two halves of a 64-pixel chunk sit in operand rows 0..63 and 64..127,
 // one M = N = 128 product then yields both halves' products on the diagonal blocks (the MMA cost is set by the 128 operand rows
 // it streams whether they are live or not).
+// The copies move whole 16-byte pieces, so the last piece of a row also carries the pad pixels [HW, pitch).  They are zero in E, w
+// and C, and rsqrt(C) is taken as 0 there, so they add nothing.
 // ---------------------------------------------------------------------------------------------------------
-constexpr int kTcRowsMax = 21;
 constexpr int kPairTileRows = 10;               // pair mode: row tiles of 10 frame rows (60 lines + the w line <= 64 operand rows)
-constexpr int kPairRowsMax = 100;               // pair mode handles 22..100 rows (up to 45 tile pairs over gridDim.z); more rows: SIMT kernel
-constexpr int kPairGridZ = 45;
+constexpr int kPairGridZ = 45;                  // tile pairs of a kPairRowsMax-row frame (10 tiles)
 constexpr int kTcThreads = 256;
 constexpr int kTcRawStages = 4;
 constexpr int kTcRawBytes = 128 * 128;          // up to 128 lines (6R rows, w, C; two halves when packed) x 128 bytes
@@ -856,6 +722,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   const int deg = rowptr[m + 1] - e_begin;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int n = 6 * P;
+  const int pitch = ba_pitch(HW);
 
   __shared__ int s_pose[kSchurMaxRows + 1];
   __shared__ const float* s_ptr[kSchurMaxRows + 1];
@@ -870,7 +737,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
     const int tmax = (min(deg + 1, kPairRowsMax) + kPairTileRows - 1) / kPairTileRows;
     if ((int)blockIdx.z >= tmax * (tmax - 1) / 2) return;
   }
-  build_row_list<kTcThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, HW, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
+  build_row_list<kTcThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
   const int nrows = s_nrows;
   if (!PAIR && (nrows == 0 || nrows > kTcRowsMax)) return;            // larger frames belong to the pair-mode launch / ba_schur_gemm_kernel
   if (PAIR && (nrows <= kTcRowsMax || nrows > kPairRowsMax)) return;
@@ -933,12 +800,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
     src[i] = Cin; pxo[i] = 1 << 30;
     dst[i] = raw_base + warp * 2048 + li * 128 + piece * 16;
     if (line <= R6x) {
-      const float* base = (line < R6x) ? s_ptr[row0 + line / 6] + (size_t)(line % 6) * HW : win + (size_t)m * HW;
+      const float* base = (line < R6x) ? s_ptr[row0 + line / 6] + (size_t)(line % 6) * pitch : win + (size_t)m * pitch;
       pxo[i] = (packed ? hf * 32 : 0) + piece * 4;
       src[i] = base + pxo[i];
     }
   }
-  const float* Cm = Cin + (size_t)m * HW;
+  const float* Cm = Cin + (size_t)m * pitch;
   auto issue = [&](int c) {
     if (c < nchunks) {
       const int p0 = px_begin + c * cpx;
@@ -1143,6 +1010,7 @@ __global__ void __launch_bounds__(256) ba_backsub_kernel(
   const int e_begin = rowptr[m], e_end = rowptr[m + 1];
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= HW) return;
+  const int pitch = ba_pitch(HW);
   // dw = sum over rows of frame m of  E[row,:,p] . dx[pose]   with the Q9 guard 0 < pose < P   (reference :1114)
   float dw = 0.f;
   {
@@ -1150,7 +1018,7 @@ __global__ void __launch_bounds__(256) ba_backsub_kernel(
     if (ps > 0 && ps < P) {
       float s = 0.f;
 #pragma unroll
-      for (int c = 0; c < 6; c++) s += __ldg(Eiin + ((size_t)m * 6 + c) * HW + p) * __ldg(dx + ps * 6 + c);
+      for (int c = 0; c < 6; c++) s += __ldg(Eiin + ((size_t)m * 6 + c) * pitch + p) * __ldg(dx + ps * 6 + c);
       dw += s;
     }
   }
@@ -1160,12 +1028,12 @@ __global__ void __launch_bounds__(256) ba_backsub_kernel(
     if (pj > 0 && pj < P) {
       float s = 0.f;
 #pragma unroll
-      for (int c = 0; c < 6; c++) s += __ldg(Eij + ((size_t)e * 6 + c) * HW + p) * __ldg(dx + pj * 6 + c);
+      for (int c = 0; c < 6; c++) s += __ldg(Eij + ((size_t)e * 6 + c) * pitch + p) * __ldg(dx + pj * 6 + c);
       dw += s;
     }
   }
-  const float q = safe_rcp(__ldg(Cin + (size_t)m * HW + p));
-  const float dz = q * (__ldg(win + (size_t)m * HW + p) - dw);
+  const float q = safe_rcp(__ldg(Cin + (size_t)m * pitch + p));
+  const float dz = q * (__ldg(win + (size_t)m * pitch + p) - dw);
   dz_out[(size_t)m * HW + p] = owned ? dz : 0.f;
   if (owned) disps[(size_t)ix * HW + p] += dz;       // K8 (:942-955)
 }
@@ -1238,7 +1106,8 @@ extern "C" int dba_ba_prepare(const dba_ba_args* a) {
   Layout L; int rc = check_ba_args(a, L); if (rc) return rc;
   cudaStream_t st = (cudaStream_t)a->stream;
   ba_prepare_kernel<<<1, 1024, 0, st>>>(a->ii, a->jj, a->n_edges, a->n_frames, a->t0, a->t1, (a->motion_only || a->eta_by_frame) ? 1 : a->eta_rows,
-                                        WS(int, L.off_hdr), WS(int, L.off_frame2k), WS(int, L.off_kx), WS(int, L.off_rowptr), WS(int, L.off_big));
+                                        WS(int, L.off_hdr), WS(int, L.off_frame2k), WS(int, L.off_kx), WS(int, L.off_rowptr), WS(int, L.off_big),
+                                        a->ht * a->wd, WS(float, L.off_Eij), WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei));
   DBA_CHECK_LAUNCH("ba_prepare");
   if (a->n_edges > 0) {
     ba_fill_csr_kernel<<<(a->n_edges + 7) / 8, 256, 0, st>>>(a->ii, a->jj, a->n_edges, a->n_frames, WS(int, L.off_frame2k),
@@ -1273,11 +1142,6 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
   DBA_CHECK_LAUNCH("ba_build");
   if (!a->motion_only) {
     const size_t smem2 = (size_t)2 * kSgK * kSgStride * sizeof(float);
-    // small frames: about 2.5 CTAs per SM worth of (frame, chunk) work items of whole 64-pixel tiles
-    const int tiles1 = (HW + kSgK - 1) / kSgK;
-    const int chunks1 = std::max(1, std::min(tiles1, (5 * sms / 2 + eff_frames - 1) / eff_frames));
-    const int px_per_cta1 = ((tiles1 + chunks1 - 1) / chunks1) * kSgK;
-    const int gx1 = (HW + px_per_cta1 - 1) / px_per_cta1;
     // the SGEMM-style kernel keeps its accumulators in registers over the whole pixel chunk: few long chunks, tile pairs over z
     const int px_per_cta2 = ((HW + 2) / 3 + kSgK - 1) / kSgK * kSgK;
     const int gx2 = (HW + px_per_cta2 - 1) / px_per_cta2;
@@ -1285,38 +1149,29 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
     static bool attr_set = false;
     if (!attr_set) {
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2), "schur gemm smem attr");
-      DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2), "schur smem attr");
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc smem attr");
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc pair smem attr");
       attr_set = true;
     }
-    // the tensor-core kernels need 16-byte aligned pixel rows: frames with at most 21 rows go to the packed / single kernel, 22..100 rows
-    // to the pair kernel, more to ba_schur_gemm_kernel.  Otherwise ba_schur_small_kernel takes frames with at most 16 rows and
-    // ba_schur_gemm_kernel the rest.
-    const bool use_tc = (HW % 4 == 0);
-    if (use_tc) {
-      const int tiles64 = (HW + 63) / 64;
-      const int chunks_tc = std::max(1, std::min(tiles64, (sms + eff_frames / 2) / eff_frames));     // one CTA per SM
-      const int px_per_cta_tc = ((tiles64 + chunks_tc - 1) / chunks_tc) * 64;
-      const int gx_tc = (HW + px_per_cta_tc - 1) / px_per_cta_tc;
-      ba_schur_tc_kernel<false><<<dim3(gx_tc, a->n_frames, 1), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                           WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta_tc, WS(float, L.off_Eij),
-                                                           WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
-      // frames with 22..100 rows (dense graphs, edge-sharded ranks): tile pairs over gridDim.z, whole pixel range per CTA; CTAs of
-      // frames outside that range (and pair indices beyond a frame's count) exit after the row-list build.
-      const int max_big = std::min(a->n_frames, a->n_edges / kTcRowsMax);     // a frame with 22+ rows has 21+ out-edges
-      if (max_big > 0)
-        ba_schur_tc_kernel<true><<<dim3(1, max_big, kPairGridZ), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                           WS(int, L.off_edgeidx), HW, a->t0, L.P, ((HW + 31) / 32) * 32, WS(float, L.off_Eij),
-                                                           WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
-    } else {
-      ba_schur_small_kernel<<<dim3(gx1, a->n_frames, 1), kSgThreads, smem2, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                           WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta1, WS(float, L.off_Eij),
-                                                           WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys);
-    }
+    // one launch per routing-table entry (see the Schur section): frames with at most kTcRowsMax rows on the packed / single
+    // tensor-core kernel, up to kPairRowsMax rows on the pair kernel, more on ba_schur_gemm_kernel.  Each kernel exits on other frames.
+    const int tiles64 = (HW + 63) / 64;
+    const int chunks_tc = std::max(1, std::min(tiles64, (sms + eff_frames / 2) / eff_frames));     // one CTA per SM
+    const int px_per_cta_tc = ((tiles64 + chunks_tc - 1) / chunks_tc) * 64;
+    const int gx_tc = (HW + px_per_cta_tc - 1) / px_per_cta_tc;
+    ba_schur_tc_kernel<false><<<dim3(gx_tc, a->n_frames, 1), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
+                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta_tc, WS(float, L.off_Eij),
+                                                         WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
+    // pair mode: tile pairs over gridDim.z, whole pixel range per CTA; CTAs of frames outside its row range (and pair indices beyond
+    // a frame's count) exit after the row-list build.
+    const int max_big = std::min(a->n_frames, a->n_edges / kTcRowsMax);     // a frame with 22+ rows has 21+ out-edges
+    if (max_big > 0)
+      ba_schur_tc_kernel<true><<<dim3(1, max_big, kPairGridZ), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
+                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, ((HW + 31) / 32) * 32, WS(float, L.off_Eij),
+                                                         WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
     DBA_CHECK_LAUNCH("ba_schur<single>");
     ba_schur_gemm_kernel<<<dim3(gx2, a->n_frames, zsplit2), kSgThreads, smem2, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta2, use_tc ? kPairRowsMax : kSgRows, WS(float, L.off_Eij),
+                                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta2, WS(float, L.off_Eij),
                                                                          WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys);
     DBA_CHECK_LAUNCH("ba_schur<multi>");
   }

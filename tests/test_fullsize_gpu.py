@@ -6,7 +6,7 @@ import torch
 
 import oracle
 from droid_slam_b200 import synth
-from util import rel_err
+from util import c_ba, rel_err
 
 pytestmark = pytest.mark.gpu
 dev = "cuda"
@@ -121,10 +121,10 @@ def test_stress_shape_72x96_bf16_and_ba(backends):
 
 
 def _mixed_degree_graph(N=34):
-    """frames with 3-5 rows (packed tensor-core tiles), 16 rows (one tile per 32 pixels) and 25 rows (CUDA-core tile pairs),
-    plus a duplicated edge: every Schur kernel and the duplicate-pose rule (both (r,c) and (c,r) land on one diagonal block).
-    With HW % 4 != 0 the same graph runs the CUDA-core kernels instead: 3-5 and 16 rows on ba_schur_small_kernel, 25 rows on
-    ba_schur_gemm_kernel.  The extra edges stay within 12 frames so that the problem is as well conditioned as a covisibility graph."""
+    """frames with 3-5 rows (packed tensor-core tiles), 16 rows (one tile per 32 pixels) and 25 rows (tensor-core tile pairs),
+    plus a duplicated edge: every tensor-core Schur mode and the duplicate-pose rule (both (r,c) and (c,r) land on one diagonal
+    block), at every image size.  The extra edges stay within 12 frames so that the problem is as well conditioned as a covisibility
+    graph."""
     e = []
     for i in range(N):
         for j in (i - 2, i - 1, i + 1, i + 2):
@@ -155,10 +155,38 @@ def test_ba_every_schur_kernel_matches_oracle(backends):
     _mixed_degree_ba_matches_oracle(backends, 48, 64)
 
 
-def test_ba_cuda_core_schur_kernels_match_oracle(backends):
-    """47x63: HW % 4 != 0, so the pixel rows are not 16-byte aligned and the same graph runs ba_schur_small_kernel and
-    ba_schur_gemm_kernel instead of the tensor-core kernels"""
+def test_ba_every_schur_kernel_on_padded_rows_matches_oracle(backends):
+    """47x63: HW % 4 != 0, so the workspace pixel rows end in pad pixels, and the tensor-core kernels read them with the last 16-byte
+    piece of each row"""
     _mixed_degree_ba_matches_oracle(backends, 47, 63)
+
+
+def _high_degree_graph():
+    """_mixed_degree_graph plus frame 12 with its 24 targets within 12 frames repeated 5 times: 124 out-edges -> 125 rows (120 after
+    dropping the 5 rows of frame 0, which is outside the window).  That frame takes ba_schur_gemm_kernel (more than 100 rows), where
+    repeated targets put rows with one pose into different tiles (the duplicate-pose rule)."""
+    ii, jj = _mixed_degree_graph()
+    extra = [j for _ in range(5) for j in range(0, 25) if j != 12]
+    return ii + [12] * len(extra), jj + extra
+
+
+@pytest.mark.parametrize("ht,wd", [(48, 64), (47, 63)])
+def test_ba_schur_gemm_frame_over_100_rows_matches_oracle(capi, ht, wd):
+    """every Schur kernel in one graph, with a workspace that starts as NaN: a pad pixel that the Schur kernels read but nothing
+    zeroed would turn the result into NaN"""
+    ii, jj = _high_degree_graph()
+    s = synth.make_scene(dict(E=len(ii), N=34, ht=ht, wd=wd, stereo=False, itrs=2, lm=1e-4, ep=0.1, graph=(ii, jj)), seed=7)
+    deg = torch.bincount(s["ii"], minlength=34)
+    assert int(deg[12]) == 124 and int(deg[17]) == 24 and int(deg[26]) == 15
+    torch.set_num_threads(min(16, torch.get_num_threads()))
+    P, D = s["poses"].to(dev), s["disps"].to(dev)
+    args = [s[k].to(dev) for k in ("intrinsics", "disps_sens", "targets", "weights", "eta", "ii", "jj")]
+    _, _, M, st, _ = c_ba(capi, P, D, *args, s["t0"], s["t1"], 2, s["lm"], s["ep"], False, s["M"], ws_fill=255)
+    assert M == s["M"] and st == 0
+    P64, D64 = s["poses"].double(), s["disps"].double()
+    oracle.ba(P64, D64, s["intrinsics"], s["disps_sens"], s["targets"], s["weights"], s["eta"], s["ii"], s["jj"], s["t0"], s["t1"], 2,
+              s["lm"], s["ep"], False, dtype=torch.float64)
+    assert rel_err(P, P64, floor=1.0) < 1e-4 and rel_err(D, D64, floor=1.0) < 1e-4, (rel_err(P, P64, floor=1.0), rel_err(D, D64, floor=1.0))
 
 
 @pytest.mark.parametrize("N,res", [(40, (24, 32)), (30, (48, 64))])

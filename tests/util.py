@@ -30,11 +30,14 @@ def c_corr_index_backward(L, volume, coords, grad, r):
     return out
 
 
-def c_ba(L, poses, disps, intr, disps_sens, targets, weights, eta, ii, jj, t0, t1, itrs, lm, ep, motion_only, M):
+def c_ba(L, poses, disps, intr, disps_sens, targets, weights, eta, ii, jj, t0, t1, itrs, lm, ep, motion_only, M, ws_fill=None):
+    """dba_ba through ctypes; ws_fill: byte value the workspace starts with (255 makes every float in it NaN) instead of torch.empty's"""
     N, ht, wd = disps.shape
     E = ii.shape[0]
     ws_bytes = L.dba_ba_workspace_bytes(N, E, ht, wd, t0, t1)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=poses.device)
+    if ws_fill is not None:
+        ws.fill_(ws_fill)
     dx = torch.full((t1 - t0, 6), float("nan"), device=poses.device)
     dz = torch.full((M, ht * wd), float("nan"), device=poses.device)
     a = c_api.BAArgs()
