@@ -280,6 +280,59 @@ torch::Tensor corr_lookup_pyramid(std::vector<torch::Tensor> pyramid, torch::Ten
   return out;
 }
 
+// extension: AltCorrBlock.__init__ (reference modules/corr.py:90-101) as one launch.  fmaps [B,N,C,H,W] f16/f32 -> num_levels tensors
+// [B,N,H>>l,W>>l,C] in the private channels-last, pre-quartered layout of include/droid_b200.h (dba_altcorr_pyramid).
+std::vector<torch::Tensor> altcorr_pyramid(torch::Tensor fmaps, int num_levels) {
+  CHECK_INPUT(fmaps);
+  TORCH_CHECK(fmaps.dim() == 5, "altcorr_pyramid: fmaps must be [B,N,C,H,W]");
+  TORCH_CHECK(fmaps.scalar_type() == torch::kFloat16 || fmaps.scalar_type() == torch::kFloat32, "altcorr_pyramid: float16 or float32 feature maps expected, got ",
+              fmaps.scalar_type());
+  TORCH_CHECK(num_levels >= 1 && num_levels <= 4, "altcorr_pyramid: 1..4 levels expected");
+  c10::cuda::CUDAGuard guard(fmaps.device());
+  const int B = (int)fmaps.size(0), N = (int)fmaps.size(1), C = (int)fmaps.size(2), H = (int)fmaps.size(3), W = (int)fmaps.size(4);
+  std::vector<torch::Tensor> out;
+  void* p[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (int l = 0; l < num_levels; l++) {
+    out.push_back(torch::empty({B, N, H >> l, W >> l, C}, fmaps.options()));
+    p[l] = out.back().data_ptr();
+  }
+  check_status(dba_altcorr_pyramid(fmaps.data_ptr(), p[0], p[1], p[2], p[3], B, N, C, H, W, num_levels, dtype_code(fmaps, "altcorr_pyramid"), cur_stream()),
+               "altcorr_pyramid");
+  return out;
+}
+
+// extension: AltCorrBlock.__call__ (reference modules/corr.py:104-117) in one launch.  pyramid from altcorr_pyramid, coords [B,M,2,H,W] f32
+// at level-0 scale, ii/jj [M] -> [B,M,L*49,H,W] = stack over levels of altcorr_forward(level 0, level l, coords / 2^l, ii, jj, radius)
+torch::Tensor altcorr_lookup_pyramid(std::vector<torch::Tensor> pyramid, torch::Tensor coords, torch::Tensor ii, torch::Tensor jj, int radius) {
+  const int L = (int)pyramid.size();
+  TORCH_CHECK(L >= 1 && L <= 4, "altcorr_lookup_pyramid: 1..4 pyramid levels expected");
+  CHECK_INPUT(coords); CHECK_F32(coords);
+  CHECK_CUDA(ii); CHECK_CUDA(jj); CHECK_I64(ii); CHECK_I64(jj);
+  for (auto& v : pyramid) {
+    CHECK_INPUT(v);
+    TORCH_CHECK(v.dim() == 5 && v.scalar_type() == pyramid[0].scalar_type() && v.device() == coords.device(),
+                "altcorr_lookup_pyramid: pyramid levels must be [B,N,H>>l,W>>l,C] tensors of one dtype on the device of coords");
+  }
+  const auto& p0 = pyramid[0];
+  const int B = (int)p0.size(0), N = (int)p0.size(1), H = (int)p0.size(2), W = (int)p0.size(3), C = (int)p0.size(4);
+  TORCH_CHECK(coords.dim() == 5 && coords.size(0) == B && coords.size(2) == 2 && coords.size(3) == H && coords.size(4) == W,
+              "altcorr_lookup_pyramid: coords must be [B,M,2,H,W] with B, H, W of pyramid level 0");
+  for (int l = 1; l < L; l++)
+    TORCH_CHECK(pyramid[l].size(0) == B && pyramid[l].size(1) == N && pyramid[l].size(2) == (H >> l) && pyramid[l].size(3) == (W >> l) &&
+                    pyramid[l].size(4) == C, "altcorr_lookup_pyramid: pyramid level ", l, " has the wrong shape");
+  const int M = (int)coords.size(1);
+  auto iic = ii.contiguous(), jjc = jj.contiguous();
+  TORCH_CHECK(iic.dim() == 1 && jjc.dim() == 1 && iic.size(0) == M && jjc.size(0) == M, "altcorr_lookup_pyramid: ii/jj must have one entry per edge");
+  c10::cuda::CUDAGuard guard(coords.device());
+  auto out = torch::empty({B, M, L * (2 * radius + 1) * (2 * radius + 1), H, W}, p0.options());
+  const void* p[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (int l = 0; l < L; l++) p[l] = pyramid[l].data_ptr();
+  check_status(dba_altcorr_lookup_pyramid(p[0], p[1], p[2], p[3], coords.data_ptr<float>(), iic.data_ptr<int64_t>(), jjc.data_ptr<int64_t>(),
+                                          out.data_ptr(), B, N, C, H, W, M, L, radius, dtype_code(p0, "altcorr_lookup_pyramid"), cur_stream()),
+               "altcorr_lookup_pyramid");
+  return out;
+}
+
 // extension: fused DepthVideo.reproject (reference depth_video.py:171-179 -> geom/projective_ops.py:165-198, jacobian=False)
 std::vector<torch::Tensor> reproject(torch::Tensor poses, torch::Tensor disps, torch::Tensor intrinsics, torch::Tensor ii, torch::Tensor jj) {
   CHECK_INPUT(poses); CHECK_INPUT(disps); CHECK_INPUT(intrinsics); CHECK_INPUT(ii); CHECK_INPUT(jj);
@@ -429,6 +482,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("tiled") = false);
   m.def("corr_lookup_pyramid", &corr_lookup_pyramid, "4-level radius-3 lookup in one launch -> [E,196,H,W], native extension", pybind11::arg("pyramid"), pybind11::arg("coords"),
         pybind11::arg("tiled") = false);
+  m.def("altcorr_pyramid", &altcorr_pyramid, "AltCorrBlock pyramid in one launch -> levels [B,N,H>>l,W>>l,C] (private channels-last layout), native extension",
+        pybind11::arg("fmaps"), pybind11::arg("num_levels") = 4);
+  m.def("altcorr_lookup_pyramid", &altcorr_lookup_pyramid, "AltCorrBlock lookup over all levels in one launch -> [B,M,L*49,H,W], native extension",
+        pybind11::arg("pyramid"), pybind11::arg("coords"), pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("radius") = 3);
   m.def("corr_volume_supported", [](int dim, int ht, int wd) { return dba_corr_volume_supported(dim, ht, wd, DBA_F16) != 0; }, "does corr_volume_pyramid have a kernel for f16 [.,dim,ht,wd] feature maps");
   m.def("reproject", &reproject, "fused pops.projective_transform(jacobian=False), native extension");
   m.def("update_forward", &update_forward, "update operator (ConvGRU + heads + GraphAgg) on wgmma, native extension");

@@ -7,6 +7,11 @@ kernel for is offered as a hook:
   * `install_corr_volume_hook(corr_module)`: `CorrBlock.__init__` (modules/corr.py:24-38, 63-71: torch.matmul + 3x avg_pool2d) builds
     its four pyramid levels with the one-pass wgmma kernel `droid_backends.corr_volume_pyramid` instead.  Only the constructor is
     replaced; lookups, `cat` and `__getitem__` stay the reference's code.
+  * `install_alt_corr_hook(corr_module)`: `AltCorrBlock` (modules/corr.py:89-117, the on-the-fly path of `FactorGraph.update_lowmem`
+    and of the global-BA backends) on a private channels-last pyramid: `__init__` builds all levels in one launch
+    (`droid_backends.altcorr_pyramid`, instead of 3x avg_pool2d) and `__call__` does every level's lookup in one launch
+    (`droid_backends.altcorr_lookup_pyramid`, instead of 4x altcorr_forward + stack).  Bit-identical to the reference's call sequence;
+    forward only.  The private level 0 is a copy: the block holds about 1.33x the feature maps (the reference: 0.33x extra).
   * `reproject(...)`: `DepthVideo.reproject` (depth_video.py:171-179 -> geom/projective_ops.py:165-198) as one kernel.
   * `add_proximity_factors(graph, ...)` / `install_proximity_hook(FactorGraph)`: the edge selection of
     `FactorGraph.add_proximity_factors` (factor_graph.py:346-412) on the device (row F1).
@@ -15,7 +20,7 @@ import torch
 
 from . import install
 
-__all__ = ["install_corr_volume_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook"]
+__all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook"]
 
 
 def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
@@ -48,6 +53,69 @@ def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
     corr_module.CorrBlock.__init__ = __init__
     if fused_lookup:
         corr_module.CorrBlock.__call__ = __call__
+    return corr_module
+
+
+def _alt_unsupported(fmaps, num_levels, radius):
+    """why altcorr_pyramid / altcorr_lookup_pyramid have no kernel for these AltCorrBlock arguments (None: they have one)"""
+    if fmaps.dim() != 5:
+        return "fmaps must be [B,N,C,H,W]"
+    if not fmaps.is_cuda:
+        return "fmaps are not on a CUDA device"
+    if fmaps.dtype not in (torch.float16, torch.float32):
+        return "dtype %s (float16 and float32 have kernels)" % fmaps.dtype
+    B, N, C, H, W = fmaps.shape
+    if radius != 3:
+        return "radius %d (3 has a kernel)" % radius
+    if not 1 <= num_levels <= 4:
+        return "%d levels (1..4 have kernels)" % num_levels
+    if C % 8:
+        return "%d channels (a multiple of 8 is needed)" % C
+    if min(H, W) < 2 ** (num_levels - 1):
+        return "%dx%d feature maps are too small for %d levels" % (H, W, num_levels)
+    return None
+
+
+def install_alt_corr_hook(corr_module, strict=True):
+    """corr_module = the imported reference module `modules.corr`.  Replaces `AltCorrBlock.__init__(fmaps, num_levels=4, radius=3)` and
+    `__call__(coords [B,M,H,W,2], ii, jj)` in place on the class (so `from modules.corr import AltCorrBlock` elsewhere picks it up) by
+    the one-launch pyramid build and the one-launch all-level lookup on a private channels-last pyramid; the output equals the reference's
+    bit for bit.  strict: fmaps / radii without a kernel (not f16/f32 on CUDA, C % 8 != 0, radius != 3, more than 4 levels) raise; with
+    strict=False the reference's own methods run for them.  Forward only: inputs that require grad under grad mode raise (the hook would
+    otherwise drop their gradients)."""
+    be = install()
+    cls = corr_module.AltCorrBlock
+    ref_init, ref_call = cls.__init__, cls.__call__
+
+    def _no_grad_inputs(*ts):
+        if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts):
+            raise RuntimeError("the native AltCorrBlock is forward only: an input requires grad")
+
+    def __init__(self, fmaps, num_levels=4, radius=3):
+        _no_grad_inputs(fmaps)
+        why = _alt_unsupported(fmaps, num_levels, radius)
+        if why is not None:
+            if strict:
+                raise RuntimeError("altcorr_pyramid has no kernel for AltCorrBlock(%s %s, num_levels=%d, radius=%d): %s"
+                                   % (tuple(fmaps.shape), fmaps.dtype, num_levels, radius, why))
+            self._b200_pyramid = None
+            return ref_init(self, fmaps, num_levels, radius)
+        self.num_levels, self.radius = num_levels, radius
+        self._b200_pyramid = be.altcorr_pyramid(fmaps.contiguous(), num_levels)
+
+    def __call__(self, coords, ii, jj):
+        pyramid = getattr(self, "_b200_pyramid", None)
+        if pyramid is None:
+            return ref_call(self, coords, ii, jj)
+        _no_grad_inputs(coords)
+        if not (coords.is_cuda and coords.dtype == torch.float32 and coords.dim() == 5 and coords.shape[-1] == 2):
+            raise RuntimeError("AltCorrBlock: coords must be a float32 CUDA tensor [B,M,H,W,2], got %s %s on %s"
+                               % (tuple(coords.shape), coords.dtype, coords.device))
+        c = coords.permute(0, 1, 4, 2, 3).contiguous()
+        return be.altcorr_lookup_pyramid(pyramid, c, ii, jj, self.radius)
+
+    cls.__init__ = __init__
+    cls.__call__ = __call__
     return corr_module
 
 

@@ -91,6 +91,25 @@ int dba_altcorr_backward(const void* fmap1, const void* fmap2, const float* coor
                          int B, int N1, int N2, int C, int H, int W, int H2, int W2, int M,
                          int radius, int dtype, dba_stream_t stream);
 
+/* ---- AltCorrBlock on a private channels-last pyramid ----------------------------------------------------------
+ * replaces AltCorrBlock.__init__ / __call__ (reference droid_slam/modules/corr.py:89-117: 3x avg_pool2d, then per level
+ * altcorr_forward + flatten + stack).  Shapes: f16 or f32, C % 8 == 0, 1 <= levels <= 4, H, W >= 2^(levels-1), radius 3;
+ * extents as for dba_altcorr_forward.  An empty batch (B, N or M zero) returns 0 without a launch; no host synchronisation.
+ *
+ * dba_altcorr_pyramid: fmaps [B,N,C,H,W] -> out_l [B,N,H>>l,W>>l,C] (channels last) for l < levels; out_l for l >= levels may be NULL.
+ *   PRIVATE LAYOUT: element (b,n,y,x,c) of out_l holds (reference level l)[b,n,c,y,x] / 4 rounded to the dtype, reference level l+1
+ *   being F.avg_pool2d(level l, 2, stride=2) of the rounded level l (fp32 sum of the 2x2 window, / 4, rounded; floor sizes).  The /4
+ *   is the scaling the reference applies to both operands of every product (src/altcorr_kernel.cu:67-68).  NOT readable by
+ *   dba_altcorr_forward / the reference's CorrLayer; level 0 is a copy, so the pyramid takes about 1.33x the feature maps.
+ * dba_altcorr_lookup_pyramid: p_l = the pyramid above; coords [B,M,2,H,W] f32 at level-0 scale; ii,jj [M] int64 frame indices
+ *   (source, target); out [B,M,levels*49,H,W], channel l*49 + xo*7 + yo = the reference's
+ *   stack([altcorr_forward(level 0, level l, coords / 2^l, ii, jj, 3).flatten(2,3) for l], 2).flatten(2,3), bit for bit. */
+int dba_altcorr_pyramid(const void* fmaps, void* out0, void* out1, void* out2, void* out3,
+                        int B, int N, int C, int H, int W, int levels, int dtype, dba_stream_t stream);
+int dba_altcorr_lookup_pyramid(const void* p0, const void* p1, const void* p2, const void* p3, const float* coords,
+                               const int64_t* ii, const int64_t* jj, void* out,
+                               int B, int N, int C, int H, int W, int M, int levels, int radius, int dtype, dba_stream_t stream);
+
 /* ---- streaming geometry -------------------------------------------------------------------------
  * poses [n_poses,7] (tx,ty,tz,qx,qy,qz,qw) f32, disps [n_disps,ht,wd] f32, intrinsics [4] f32 (fx,fy,cx,cy).
  * replace projmap_cuda / frame_distance_cuda / depth_filter_cuda / iproj_cuda
