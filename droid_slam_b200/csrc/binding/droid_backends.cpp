@@ -409,6 +409,48 @@ std::vector<torch::Tensor> update_forward(torch::Tensor net, torch::Tensor inp, 
   return {net_out, delta, weight};
 }
 
+// extension: BasicEncoder.forward (reference droid_slam/modules/extractor.py:183-198) for DroidNet's fnet (norm 1 = instance, output_dim
+// 128) and cnet (norm 0 = none, output_dim 256).  images [n,3,H,W] f32/f16, H and W multiples of 8; packed = the 28 tensors of
+// droid_slam_b200.encoder.pack_encoder_weights (w[0..13] f16, then b[0..13] f32, include/droid_b200.h).  Returns [n,output_dim,H/8,W/8] f16.
+torch::Tensor encoder_forward(torch::Tensor images, std::vector<torch::Tensor> packed, int64_t norm, int64_t output_dim) {
+  CHECK_INPUT(images);
+  TORCH_CHECK(images.dim() == 4 && images.size(1) == 3, "encoder_forward: images must be [n,3,H,W]");
+  TORCH_CHECK(images.scalar_type() == torch::kFloat32 || images.scalar_type() == torch::kFloat16, "encoder_forward: float32 or float16 images expected");
+  TORCH_CHECK(norm == 0 || norm == 1, "encoder_forward: norm must be 0 (none) or 1 (instance)");
+  TORCH_CHECK(output_dim == 128 || output_dim == 256, "encoder_forward: output_dim must be 128 or 256");
+  TORCH_CHECK(packed.size() == 2 * DBA_ENCODER_CONVS, "encoder_forward: 28 packed tensors expected");
+  const int n = (int)images.size(0), H = (int)images.size(2), W = (int)images.size(3);
+  TORCH_CHECK(n > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, "encoder_forward: H and W must be positive multiples of 8, got ", H, "x", W);
+  c10::cuda::CUDAGuard guard(images.device());
+  // [taps, N, Kpad] of each packed weight
+  const int64_t shapes[DBA_ENCODER_CONVS][3] = {{1, 32, 192}, {9, 32, 64}, {9, 32, 64}, {9, 32, 64}, {9, 32, 64}, {1, 128, 320}, {9, 64, 64},
+                                                {9, 64, 64}, {9, 64, 64}, {1, 256, 576}, {9, 128, 128}, {9, 128, 128}, {9, 128, 128}, {1, output_dim, 128}};
+  dba_encoder_weights Wt;
+  for (int k = 0; k < DBA_ENCODER_CONVS; k++) {
+    const torch::Tensor& w = packed[k];
+    const torch::Tensor& b = packed[DBA_ENCODER_CONVS + k];
+    CHECK_INPUT(w); CHECK_INPUT(b);
+    TORCH_CHECK(w.device() == images.device() && b.device() == images.device(), "encoder_forward: packed weights must be on the images' device");
+    TORCH_CHECK(w.scalar_type() == torch::kFloat16 && w.dim() == 3 && w.size(0) == shapes[k][0] && w.size(1) == shapes[k][1] && w.size(2) == shapes[k][2],
+                "encoder_forward: packed weight ", k, " must be f16 [", shapes[k][0], ",", shapes[k][1], ",", shapes[k][2], "], got ", w.sizes());
+    TORCH_CHECK(b.scalar_type() == torch::kFloat32 && b.numel() == shapes[k][1], "encoder_forward: packed bias ", k, " must be f32 [", shapes[k][1], "]");
+    Wt.w[k] = w.data_ptr();
+    Wt.b[k] = b.data_ptr<float>();
+  }
+  auto out = torch::empty({n, output_dim, H / 8, W / 8}, images.options().dtype(torch::kFloat16));
+  const size_t ws_bytes = dba_encoder_workspace_bytes(n, H, W, (int)output_dim);
+  auto ws = torch::empty({(int64_t)ws_bytes + 256}, images.options().dtype(torch::kUInt8));
+  dba_encoder_args a;
+  memset(&a, 0, sizeof(a));
+  a.images = images.data_ptr(); a.images_dtype = dtype_code(images, "encoder_forward");
+  a.n_images = n; a.H = H; a.W = W;
+  a.weights = &Wt; a.norm = (int)norm; a.output_dim = (int)output_dim;
+  a.out = out.data_ptr();
+  a.workspace = (void*)(((uintptr_t)ws.data_ptr() + 255) & ~(uintptr_t)255); a.workspace_bytes = ws_bytes; a.stream = cur_stream();
+  check_status(dba_encoder_forward(&a), "encoder_forward");
+  return out;
+}
+
 // extension: channels-last tensor-core convolution (building block of update_forward).  src0 [E,ht,wd,C0] f16 (+ src1 [E,ht,wd,C1]),
 // wpk f16 [k*k][N][Kpad], bias f32 [N] -> [E,ht,wd,N] f16
 torch::Tensor conv_nhwc(torch::Tensor src0, c10::optional<torch::Tensor> src1, torch::Tensor wpk, torch::Tensor bias, int64_t ksize, bool relu) {
@@ -489,7 +531,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("corr_volume_supported", [](int dim, int ht, int wd) { return dba_corr_volume_supported(dim, ht, wd, DBA_F16) != 0; }, "does corr_volume_pyramid have a kernel for f16 [.,dim,ht,wd] feature maps");
   m.def("reproject", &reproject, "fused pops.projective_transform(jacobian=False), native extension");
   m.def("update_forward", &update_forward, "update operator (ConvGRU + heads + GraphAgg) on wgmma, native extension");
-  m.def("conv_nhwc", &conv_nhwc, "channels-last 1x1/3x3 convolution on wgmma, native extension");
+  m.def("encoder_forward", &encoder_forward, "feature / context encoder (BasicEncoder: fnet norm=1, cnet norm=0) on wgmma -> [n,output_dim,H/8,W/8] f16, native extension",
+        pybind11::arg("images"), pybind11::arg("packed_weights"), pybind11::arg("norm"), pybind11::arg("output_dim"));
+  m.def("conv_nhwc", &conv_nhwc,"channels-last 1x1/3x3 convolution on wgmma, native extension");
   m.def("cvx_upsample", &cvx_upsample, "convex upsampling of inverse depth maps (droid_net.cvx_upsample, dim = 1), native extension");
   m.def("proximity_edges", &proximity_edges, "edge selection of FactorGraph.add_proximity_factors (factor_graph.py:357-411), native extension");
   m.def("_b200_native", []() { return true; });

@@ -20,257 +20,9 @@
 //     context sum, sigmoid / softplus of the heads and the NCHW layout of the upsampling mask.
 // Segment mean (GraphAgg's scatter_mean), the 7x7 flow encoder's im2col (4 input channels: 49 taps x 4 = one 196-wide K),
 // the global-context mat-vec and the NCHW -> channels-last transposes are small SIMT kernels around it.
-#include "common.cuh"
-#include "wgmma.cuh"
-#include <cuda.h>
-#include <string.h>
+#include "conv_engine.cuh"
 
 namespace dba {
-
-enum { EPI_STORE = 0, EPI_GATE = 1, EPI_ZR = 2, EPI_Q = 3, EPI_F32 = 4, EPI_NCHW = 5 };
-
-constexpr int kUpThreads = 288;   // warps 0..7 two consumer warpgroups, warp 8 TMA
-constexpr int kSlotsPerMTile = 8;  // EPI_GATE partial-sum slots per 128-pixel M tile (one per consumer warp)
-
-struct ConvParams {
-  int E, HT, WD;                    // images (edges or frames), image height / width
-  int TW, RM, MT;                   // tile width in pixels, image rows per 128-pixel M tile (RM * TW = 128), M tiles per CTA tile
-  int tiles_x, tiles_y, n_ntiles;   // CTA tiles per image, N tiles (output-channel blocks)
-  int KS;                           // kernel size 1 or 3
-  int nk0, nk1;                     // 64-channel K blocks taken from source 0 / source 1
-  int N;                            // output channels per N tile (<= 256)
-  int w_rows;                       // rows per tap of the packed weight tensor (0: n_ntiles * N); larger when only the first N rows are used
-  int boxn;                         // weight rows per TMA box
-  int a_stages, b_stages, a_bytes, b_bytes;
-  const float* bias;                // [n_ntiles * N]
-  int relu;
-  __half* out; int out_stride;      // EPI_STORE / EPI_Q: channels-last f16, out[pix * out_stride + n]
-  const __half* h; int h_stride;    // hidden state, channels-last (EPI_GATE, EPI_ZR, EPI_Q)
-  const float* glo;                 // [E][384] global-context terms: z | r | q
-  __half* z; __half* rh;            // EPI_ZR outputs [pix][128]; EPI_Q reads z
-  float* partial; int slots;        // EPI_GATE: [E][slots][128] column sums of sigmoid(.) * h over 16-pixel groups
-  float* f32a; int f32_cols, f32_stride;      // EPI_F32: f32 out[pix * f32_stride + n] for n < f32_cols (per-tap partial sums of the narrow heads)
-  __half* nchw; int nchw_C;         // EPI_NCHW: out[(img * nchw_C + n) * HT*WD + pixel]
-};
-
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_w(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  const __half2 t = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&t);
-}
-__device__ __forceinline__ float2 unpack2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
-
-__device__ __forceinline__ float2 ldh2(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
-
-// M tiles per CTA tile a consumer warpgroup can hold in registers: MT * N / 2 <= 128 fp32 accumulators per thread
-constexpr int conv_max_mt(int nw) { return 256 / nw < 4 ? 256 / nw : 4; }
-
-// epilogue of one 64-pixel x N fragment (M tile t of the CTA tile) of consumer warpgroup wg: this thread holds pixels r, r + 8
-// (r = 16 (warp % 4) + lane / 4) and columns 8 j + 2 (lane % 4) + {0, 1}
-template <int EPI, int NW>
-__device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (&acc)[NW / 2], int t, int wg, int warp, int lane, int nt, int e, int ty,
-                                              int tx) {
-  const int qd = lane & 3;
-  const float* bias = p.bias + nt * p.N;
-  float csum[NW / 4];                                                  // EPI_GATE: per-column sums over this thread's two pixels
-#pragma unroll
-  for (int i = 0; i < 2; i++) {
-    const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
-    const int my = m / p.TW, mx = m - my * p.TW;
-    const int y = ty * (p.MT * p.RM) + t * p.RM + my, x = tx * p.TW + mx;
-    const bool valid = y < p.HT && x < p.WD;
-    const size_t pix = ((size_t)e * p.HT + (valid ? y : 0)) * p.WD + (valid ? x : 0);
-#pragma unroll
-    for (int j = 0; j < NW / 8; j++) {
-      const int c = 8 * j + 2 * qd;
-      float v0 = acc[4 * j + 2 * i] + __ldg(bias + c), v1 = acc[4 * j + 2 * i + 1] + __ldg(bias + c + 1);
-      if (EPI == EPI_STORE) {
-        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + nt * p.N + c) = pack2(v0, v1);
-      } else if (EPI == EPI_GATE) {
-        float g0 = 0.f, g1 = 0.f;
-        if (valid) { const float2 hh = ldh2(p.h + pix * p.h_stride + c); g0 = sigmoid_fast(v0) * hh.x; g1 = sigmoid_fast(v1) * hh.y; }
-        if (i == 0) { csum[2 * j] = g0; csum[2 * j + 1] = g1; }
-        else { csum[2 * j] += g0; csum[2 * j + 1] += g1; }
-      } else if (EPI == EPI_ZR) {
-        const float* g = p.glo + (size_t)e * 384 + c;
-        v0 = sigmoid_fast(v0 + __ldg(g)); v1 = sigmoid_fast(v1 + __ldg(g + 1));
-        if (valid) {
-          if (c < 128) {
-            *reinterpret_cast<uint32_t*>(p.z + pix * 128 + c) = pack2(v0, v1);
-          } else {
-            const float2 hh = ldh2(p.h + pix * p.h_stride + (c - 128));
-            *reinterpret_cast<uint32_t*>(p.rh + pix * 128 + (c - 128)) = pack2(v0 * hh.x, v1 * hh.y);
-          }
-        }
-      } else if (EPI == EPI_Q) {
-        const float* g = p.glo + (size_t)e * 384 + 256 + c;
-        if (valid) {
-          const float2 hh = ldh2(p.h + pix * p.h_stride + c), zz = ldh2(p.z + pix * 128 + c);
-          const float q0 = tanh_fast(v0 + __ldg(g)), q1 = tanh_fast(v1 + __ldg(g + 1));
-          *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack2((1.f - zz.x) * hh.x + zz.x * q0, (1.f - zz.y) * hh.y + zz.y * q1);
-        }
-      } else if (EPI == EPI_F32) {
-        if (valid && c < p.f32_cols) *reinterpret_cast<float2*>(p.f32a + pix * p.f32_stride + c) = make_float2(v0, v1);   // f32_cols even
-      } else if (EPI == EPI_NCHW) {
-        if (valid) {
-          const size_t HW = (size_t)p.HT * p.WD;
-          __half* o = p.nchw + ((size_t)e * p.nchw_C + nt * p.N + c) * HW + (size_t)y * p.WD + x;
-          o[0] = __float2half_rn(v0);
-          o[HW] = __float2half_rn(v1);
-        }
-      }
-    }
-  }
-  if (EPI == EPI_GATE) {
-    // column sums over the warp's 16 pixels (lanes with equal lane % 4 hold the same columns), one slot per warp and M tile
-#pragma unroll
-    for (int k = 0; k < NW / 4; k++) {
-      csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 4);
-      csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 8);
-      csum[k] += __shfl_xor_sync(0xffffffffu, csum[k], 16);
-    }
-    if (lane < 4) {
-      const int slot = ((ty * p.tiles_x + tx) * p.MT + t) * kSlotsPerMTile + wg * 4 + (warp & 3);
-      float* dst = p.partial + ((size_t)e * p.slots + slot) * 128;
-#pragma unroll
-      for (int j = 0; j < NW / 8; j++) *reinterpret_cast<float2*>(dst + 8 * j + 2 * qd) = make_float2(csum[2 * j], csum[2 * j + 1]);
-    }
-  }
-}
-
-template <int EPI, int NW>
-__global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                                                               const __grid_constant__ CUtensorMap tmW, const ConvParams p) {
-  constexpr int kMT = conv_max_mt(NW);
-  extern __shared__ uint8_t up_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(up_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + p.a_stages * p.a_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sB + p.b_stages * p.b_bytes);
-  uint64_t* a_full = bars;              // [4]
-  uint64_t* a_empty = bars + 4;         // [4]
-  uint64_t* b_full = bars + 8;          // [8]
-  uint64_t* b_empty = bars + 16;        // [8]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
-  const int total_tiles = p.n_ntiles * p.E * tiles_per_img;
-  const int nk = p.nk0 + p.nk1;
-  const int pad = p.KS >> 1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.a_stages; s++) { mbar_init(a_full + s, 1); mbar_init(a_empty + s, 8); }
-    for (int s = 0; s < p.b_stages; s++) { mbar_init(b_full + s, 1); mbar_init(b_empty + s, 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (warp == 8) {
-    // ================= TMA producer (one thread) =================
-    if (lane == 0) {
-      uint32_t ac = 0, bc = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int nt = tile / (p.E * tiles_per_img);
-        const int r0 = tile - nt * (p.E * tiles_per_img);
-        const int e = r0 / tiles_per_img;
-        const int r1 = r0 - e * tiles_per_img;
-        const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
-        const int y0 = ty * (p.MT * p.RM), x0 = tx * p.TW;
-        for (int kb = 0; kb < nk; kb++) {
-          const CUtensorMap* am = kb < p.nk0 ? &tmA0 : &tmA1;
-          const int ch = (kb < p.nk0 ? kb : kb - p.nk0) * 64;
-          for (int dx = 0; dx < p.KS; dx++) {
-            const int as = ac % p.a_stages;
-            mbar_wait(a_empty + as, ((ac / p.a_stages) & 1) ^ 1);
-            mbar_expect_tx(a_full + as, p.a_bytes);
-            tma_load_4d(sA + as * p.a_bytes, am, a_full + as, ch, x0 + dx - pad, y0 - pad, e);
-            ac++;
-            for (int dy = 0; dy < p.KS; dy++) {
-              const int bs = bc % p.b_stages;
-              mbar_wait(b_empty + bs, ((bc / p.b_stages) & 1) ^ 1);
-              mbar_expect_tx(b_full + bs, p.b_bytes);
-              for (int n = 0; n < p.N; n += p.boxn)
-                tma_load_3d_w(sB + bs * p.b_bytes + n * 128, &tmW, b_full + bs, kb * 64, nt * p.N + n, dy * p.KS + dx);
-              bc++;
-            }
-          }
-        }
-      }
-    }
-    return;
-  }
-  // ================= consumers: warpgroup wg = pixels 64 wg .. 64 wg + 63 of every M tile =================
-  // A stage is released (one arrival per warp) when the wgmma batch after the last one reading it has been issued and the
-  // batch reading it has completed (wgmma.wait_group 1), so one batch is always in flight.
-  const int wg = warp >> 2;
-  const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-  float acc[kMT][NW / 2];
-  uint32_t ac = 0, bc = 0;
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int nt = tile / (p.E * tiles_per_img);
-    const int r0 = tile - nt * (p.E * tiles_per_img);
-    const int e = r0 / tiles_per_img;
-    const int r1 = r0 - e * tiles_per_img;
-    const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
-    bool first = true;
-    int pend_a = -1, pend_b = -1;
-    for (int kb = 0; kb < nk; kb++) {
-      for (int dx = 0; dx < p.KS; dx++) {
-        const int as = ac % p.a_stages;
-        mbar_wait(a_full + as, (ac / p.a_stages) & 1);
-        for (int dy = 0; dy < p.KS; dy++) {
-          const int bs = bc % p.b_stages;
-          mbar_wait(b_full + bs, (bc / p.b_stages) & 1);
-          const uint32_t b_base = sB_u + bs * p.b_bytes;
-          wgmma_fence();
-#pragma unroll
-          for (int t = 0; t < kMT; t++) {
-            if (t < p.MT) {
-              const uint32_t a_base = sA_u + as * p.a_bytes + (uint32_t)((t * p.RM + dy) * p.TW + wg * 64) * 128u;
-#pragma unroll
-              for (int k = 0; k < 4; k++)
-                wgmma_f16<NW>(acc[t], gmma_desc_sw128(a_base + k * 32, 16, 1024), gmma_desc_sw128(b_base + k * 32, 16, 1024), (first && k == 0) ? 0 : 1, 0);
-            }
-          }
-          wgmma_commit();
-          wgmma_wait<1>();
-          __syncwarp();
-          if (lane == 0) {
-            if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
-            if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
-          }
-          pend_a = -1;
-          pend_b = bs;
-          first = false;
-          bc++;
-        }
-        pend_a = as;
-        ac++;
-      }
-    }
-    wgmma_wait<0>();
-    __syncwarp();
-    if (lane == 0) {
-      if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
-      if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
-    }
-#pragma unroll
-    for (int t = 0; t < kMT; t++) {
-      wgmma_fence_regs(acc[t]);
-      if (t < p.MT) conv_epilogue<EPI, NW>(p, acc[t], t, wg, warp, lane, nt, e, ty, tx);
-    }
-  }
-}
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // small SIMT kernels around the tensor-core convolutions
@@ -453,136 +205,6 @@ __global__ void __launch_bounds__(256) segment_mean_kernel(const __half* __restr
       make_uint4(pack2(acc[0] * inv, acc[1] * inv), pack2(acc[2] * inv, acc[3] * inv), pack2(acc[4] * inv, acc[5] * inv), pack2(acc[6] * inv, acc[7] * inv));
 }
 
-// ---------------------------------------------------------------------------------------------------------------------------
-// host side
-// ---------------------------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFnU)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFnU get_encode_fn_u() {
-  static EncodeTiledFnU fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess) return nullptr;
-    fn = reinterpret_cast<EncodeTiledFnU>(ptr);
-  }
-  return fn;
-}
-
-// activation map: channels-last f16 [E][HT][WD][stride], channels [0, C) of the slice starting at `base`
-static int make_act_map(CUtensorMap* map, const void* base, int C, int stride, int WD, int HT, int E, int TW, int box_rows) {
-  EncodeTiledFnU enc = get_encode_fn_u();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return DBA_ERR_CUDA; }
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)WD, (cuuint64_t)HT, (cuuint64_t)E};
-  cuuint64_t strides[3] = {(cuuint64_t)stride * 2, (cuuint64_t)WD * stride * 2, (cuuint64_t)HT * WD * stride * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (activation, C=%d stride=%d %dx%d E=%d box %dx%d) failed with CUresult %d", C, stride, HT, WD, E, TW, box_rows, (int)r); return DBA_ERR_CUDA; }
-  return DBA_OK;
-}
-// weight map: [taps][Ntot][Kpad] f16
-static int make_weight_map(CUtensorMap* map, const void* base, int Kpad, int Ntot, int taps, int boxn) {
-  EncodeTiledFnU enc = get_encode_fn_u();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return DBA_ERR_CUDA; }
-  cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Ntot, (cuuint64_t)taps};
-  cuuint64_t strides[2] = {(cuuint64_t)Kpad * 2, (cuuint64_t)Ntot * Kpad * 2};
-  cuuint32_t box[3] = {64, (cuuint32_t)boxn, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (weights K=%d N=%d taps=%d) failed with CUresult %d", Kpad, Ntot, taps, (int)r); return DBA_ERR_CUDA; }
-  return DBA_OK;
-}
-
-struct ConvSrc { const void* base; int C; int stride; };
-
-static int g_num_sms = 0;
-
-template <int EPI>
-constexpr bool conv_width_used(int nw) {
-  return EPI == EPI_STORE || (EPI == EPI_GATE && nw == 128) || (EPI == EPI_ZR && nw == 256) || (EPI == EPI_Q && nw == 128) ||
-         (EPI == EPI_F32 && (nw == 32 || nw == 64)) || (EPI == EPI_NCHW && nw == 192);
-}
-
-template <int EPI, int NW>
-static int launch_conv_nw(const ConvParams& p, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tW, int grid, int smem, cudaStream_t st) {
-  if constexpr (!conv_width_used<EPI>(NW)) {
-    set_error("update operator: no convolution kernel for this epilogue with %d output channels", NW);
-    return DBA_ERR_INVALID;
-  } else {
-    static bool attr_set = false;
-    if (!attr_set) {
-      DBA_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<EPI, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), "conv_tc smem attr");
-      attr_set = true;
-    }
-    conv_tc_kernel<EPI, NW><<<grid, kUpThreads, smem, st>>>(tA0, tA1, tW, p);
-    DBA_CHECK_LAUNCH("conv_tc_kernel");
-    return DBA_OK;
-  }
-}
-
-// one convolution launch.  src0 (+ optional src1) = channels-last sources concatenated along K; wpk = packed weights
-// [KS*KS][n_ntiles*N][Kpad] with Kpad = 64 * (kblocks(src0) + kblocks(src1)).
-template <int EPI>
-static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cudaStream_t st, int* slots_out = nullptr) {
-  if (!g_num_sms) {
-    int dev = 0; cudaGetDevice(&dev);
-    cudaDeviceProp prop; DBA_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties");
-    g_num_sms = prop.multiProcessorCount;
-  }
-  if (p.N > 256) {                // 384 outputs: two 192-wide N tiles (the register accumulator holds at most 256 columns)
-    if (p.w_rows == 0) p.w_rows = p.n_ntiles * p.N;
-    p.n_ntiles *= p.N / 192;
-    p.N = 192;
-  }
-  if (p.N % 32 != 0 || p.N < 32) { set_error("update operator: %d output channels per tile", p.N); return DBA_ERR_INVALID; }
-  p.TW = (p.WD % 64 == 0) ? 64 : 32;
-  p.RM = 128 / p.TW;
-  // M tiles per CTA tile: every weight stage is shared by MT tiles (and every halo row by 3 taps), so larger is better for the
-  // L2 -> SM traffic per MAC; bounded by the register accumulators (MT * N <= 256 columns) and by the image height
-  p.MT = (p.HT >= 2 * p.RM) ? 2 : 1;
-  if (p.N <= 64 && p.HT >= 4 * p.RM && (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0) >= 4 && p.KS == 3) p.MT = 4;
-  if (p.MT > conv_max_mt(p.N)) p.MT = conv_max_mt(p.N);
-  p.tiles_x = (p.WD + p.TW - 1) / p.TW;
-  p.tiles_y = (p.HT + p.MT * p.RM - 1) / (p.MT * p.RM);
-  p.nk0 = (s0.C + 63) / 64;
-  p.nk1 = s1.base ? (s1.C + 63) / 64 : 0;
-  p.boxn = p.N;
-  const int box_rows = p.MT * p.RM + p.KS - 1;
-  p.a_bytes = box_rows * p.TW * 128;
-  p.b_bytes = p.N * 128;
-  // shared memory: at least 2 halo stages and 3 weight stages; what is left goes to more halo stages (up to 4: with narrow N the
-  // MMAs of a stage are short and the TMA latency of the next halo tile is what the pipeline has to cover), then weight stages
-  const int budget = 227 * 1024 - 2048;
-  p.a_stages = 2;
-  while (p.a_stages < 4 && (p.a_stages + 1) * p.a_bytes + 4 * p.b_bytes <= budget) p.a_stages++;
-  p.b_stages = (budget - p.a_stages * p.a_bytes) / p.b_bytes;
-  if (p.b_stages > 8) p.b_stages = 8;
-  if (p.b_stages < 2) { set_error("update operator: tile does not fit shared memory"); return DBA_ERR_INVALID; }
-  p.slots = p.tiles_x * p.tiles_y * p.MT * kSlotsPerMTile;
-  if (slots_out) *slots_out = p.slots;
-  const int smem = p.a_stages * p.a_bytes + p.b_stages * p.b_bytes + 1024 + 256;
-  CUtensorMap tA0, tA1, tW;
-  int rc = make_act_map(&tA0, s0.base, s0.C, s0.stride, p.WD, p.HT, p.E, p.TW, box_rows); if (rc) return rc;
-  if (s1.base) { rc = make_act_map(&tA1, s1.base, s1.C, s1.stride, p.WD, p.HT, p.E, p.TW, box_rows); if (rc) return rc; }
-  else tA1 = tA0;
-  rc = make_weight_map(&tW, wpk, 64 * (p.nk0 + p.nk1), p.w_rows > 0 ? p.w_rows : p.n_ntiles * p.N, p.KS * p.KS, p.boxn); if (rc) return rc;
-  const long long total = (long long)p.n_ntiles * p.E * p.tiles_x * p.tiles_y;
-  if (total <= 0) return DBA_OK;
-  const int grid = (int)(total < g_num_sms ? total : g_num_sms);
-  switch (p.N) {
-    case 32: return launch_conv_nw<EPI, 32>(p, tA0, tA1, tW, grid, smem, st);
-    case 64: return launch_conv_nw<EPI, 64>(p, tA0, tA1, tW, grid, smem, st);
-    case 96: return launch_conv_nw<EPI, 96>(p, tA0, tA1, tW, grid, smem, st);
-    case 128: return launch_conv_nw<EPI, 128>(p, tA0, tA1, tW, grid, smem, st);
-    case 160: return launch_conv_nw<EPI, 160>(p, tA0, tA1, tW, grid, smem, st);
-    case 192: return launch_conv_nw<EPI, 192>(p, tA0, tA1, tW, grid, smem, st);
-    case 224: return launch_conv_nw<EPI, 224>(p, tA0, tA1, tW, grid, smem, st);
-    default: return launch_conv_nw<EPI, 256>(p, tA0, tA1, tW, grid, smem, st);
-  }
-}
 
 static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 

@@ -12,6 +12,8 @@ kernel for is offered as a hook:
     (`droid_backends.altcorr_pyramid`, instead of 3x avg_pool2d) and `__call__` does every level's lookup in one launch
     (`droid_backends.altcorr_lookup_pyramid`, instead of 4x altcorr_forward + stack).  Bit-identical to the reference's call sequence;
     forward only.  The private level 0 is a copy: the block holds about 1.33x the feature maps (the reference: 0.33x extra).
+  * `install_encoder_hook(extractor_module)`: `BasicEncoder.forward` (modules/extractor.py:183-198) of DroidNet's fnet (instance norm)
+    and cnet (no norm) on the kernels of csrc/encoder.cu (`droid_backends.encoder_forward`) instead of cuDNN convolutions and ATen norms.
   * `reproject(...)`: `DepthVideo.reproject` (depth_video.py:171-179 -> geom/projective_ops.py:165-198) as one kernel.
   * `add_proximity_factors(graph, ...)` / `install_proximity_hook(FactorGraph)`: the edge selection of
     `FactorGraph.add_proximity_factors` (factor_graph.py:346-412) on the device (row F1).
@@ -20,7 +22,7 @@ import torch
 
 from . import install
 
-__all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook"]
+__all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook"]
 
 
 def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
@@ -117,6 +119,66 @@ def install_alt_corr_hook(corr_module, strict=True):
     cls.__init__ = __init__
     cls.__call__ = __call__
     return corr_module
+
+
+def _encoder_unsupported(enc, x):
+    """why encoder_forward has no kernel for this BasicEncoder and input (None: it has one)"""
+    if enc.norm_fn not in ("instance", "none"):
+        return "norm_fn %r (instance and none have kernels)" % (enc.norm_fn,)
+    if enc.multidim:
+        return "multidim"
+    if getattr(enc, "dropout", None) is not None:
+        return "dropout"
+    if enc.conv2.out_channels not in (128, 256):
+        return "output_dim %d (128 and 256 have kernels)" % enc.conv2.out_channels
+    if x.dim() != 5 or x.shape[2] != 3:
+        return "input must be [b,n,3,H,W]"
+    if not x.is_cuda:
+        return "input is not on a CUDA device"
+    if x.dtype not in (torch.float16, torch.float32):
+        return "dtype %s (float16 and float32 have kernels)" % x.dtype
+    if x.shape[3] % 8 or x.shape[4] % 8:
+        return "%dx%d images (H and W must be multiples of 8)" % (x.shape[3], x.shape[4])
+    return None
+
+
+def install_encoder_hook(extractor_module, strict=True):
+    """extractor_module = the imported reference module `modules.extractor`.  Replaces `BasicEncoder.forward(x [b,n,3,H,W])` in place on
+    the class (so droid_net.py, motion_filter.py and trajectory_filler.py pick it up unchanged) by one `encoder_forward` call: the
+    module keeps the reference's parameters (a DROID checkpoint loads as before); they are packed once and re-packed when a parameter's
+    storage or version changes.  Output [b,n,output_dim,H/8,W/8]: f16 under CUDA autocast (as the reference's last convolution gives),
+    otherwise the input's dtype.  strict: encoders and inputs without a kernel (norm_fn other than instance / none, multidim, dropout,
+    output_dim other than 128 / 256, inputs not f16/f32 on CUDA, H or W not a multiple of 8) raise; with strict=False the reference's own
+    forward runs for them.  Forward only: an input that requires grad under grad mode raises, and the parameters get no gradient."""
+    be = install()
+    from .encoder import pack_encoder_weights
+    cls = extractor_module.BasicEncoder
+    ref_forward = cls.forward
+
+    def packed(self, device):
+        key = (str(device),) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        if getattr(self, "_b200_packed_key", None) != key:
+            self._b200_packed = pack_encoder_weights(self.state_dict(), self.norm_fn, self.conv2.out_channels, device)
+            self._b200_packed_key = key
+        return self._b200_packed
+
+    def forward(self, x):
+        why = _encoder_unsupported(self, x)
+        if why is not None:
+            if strict:
+                raise RuntimeError("encoder_forward has no kernel for BasicEncoder(norm_fn=%r) on %s %s: %s" % (self.norm_fn, tuple(x.shape), x.dtype, why))
+            return ref_forward(self, x)
+        if torch.is_grad_enabled() and x.requires_grad:
+            raise RuntimeError("the native BasicEncoder is forward only: the input requires grad")
+        b, n, c, h, w = x.shape
+        out = be.encoder_forward(x.reshape(b * n, c, h, w).contiguous(), packed(self, x.device), 1 if self.norm_fn == "instance" else 0,
+                                 self.conv2.out_channels)
+        if not torch.is_autocast_enabled("cuda"):
+            out = out.to(x.dtype)
+        return out.view(b, n, -1, h // 8, w // 8)
+
+    cls.forward = forward
+    return extractor_module
 
 
 def reproject(poses, disps, intrinsics, ii, jj):

@@ -270,6 +270,24 @@ def make_update_weights(seed=0, dtype=torch.float32):
     return w
 
 
+def make_encoder_weights(seed=0, output_dim=128):
+    """He-scaled random weights (fan_out, like the reference's init, extractor.py:166-168) + nonzero biases for every conv of a
+    BasicEncoder (extractor.py:118-181), keyed like its state_dict()."""
+    g = torch.Generator().manual_seed(8765 + seed)
+    shapes = {"conv1": (32, 3, 7), "conv2": (output_dim, 128, 1)}
+    for layer, cin, p in ((1, 32, 32), (2, 32, 64), (3, 64, 128)):
+        shapes["layer%d.0.conv1" % layer] = (p, cin, 3)
+        for name in ("layer%d.0.conv2" % layer, "layer%d.1.conv1" % layer, "layer%d.1.conv2" % layer):
+            shapes[name] = (p, p, 3)
+        if layer > 1:
+            shapes["layer%d.0.downsample.0" % layer] = (p, cin, 1)
+    w = {}
+    for name, (co, ci, k) in shapes.items():
+        w[name + ".weight"] = torch.randn(co, ci, k, k, generator=g) * math.sqrt(2.0 / (co * k * k))
+        w[name + ".bias"] = 0.1 * torch.randn(co, generator=g)
+    return w
+
+
 def make_update_inputs(E=5, ht=6, wd=8, seed=0, n_src=3):
     """net/inp/corr/flow of E edges at ht x wd and source-frame indices ii with n_src distinct (unsorted) values."""
     g = torch.Generator().manual_seed(99 + seed)

@@ -259,6 +259,44 @@ int dba_update_forward(const dba_update_args* a);
 int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* src1, int c1, int stride1, const void* wpk, const float* bias,
                   void* out, int out_stride, int n_images, int ht, int wd, int ksize, int n_out, int relu, dba_stream_t stream);
 
+/* ---- feature / context encoders (BasicEncoder) on the tensor cores ---------------------------------------------------
+ * replaces BasicEncoder.forward (reference droid_slam/modules/extractor.py:183-198) for the two encoders DroidNet builds
+ * (droid_net.py:149-150): fnet = BasicEncoder(output_dim=128, norm_fn='instance') and cnet = BasicEncoder(output_dim=256,
+ * norm_fn='none'), dropout 0, multidim False.  images [n_images,3,H,W] DBA_F32 or DBA_F16 (rounded to f16 on load, the cast autocast
+ * applies), H and W positive multiples of 8; out [n_images,output_dim,H/8,W/8] f16, fully overwritten.  Instance norm: per image and
+ * channel, biased variance, eps 1e-5, no affine parameters.  Never synchronises the host; can be captured in a CUDA graph.
+ *
+ * Packed weights (device memory, made once per checkpoint by droid_slam_b200/encoder.py:pack_encoder_weights), w[k] f16 [taps][N][Kpad]
+ * (tap = dy*k + dx, K contiguous and zero padded to a multiple of 64), b[k] f32 [N]:
+ *   k = 0       conv1 7x7/2 3->32           [1][32][192]    K = (dy*7 + dx)*3 + c (the 147 taps of the stride-2 window)
+ *   k = 1..4    layer1.{0,1}.{conv1,conv2}  [9][32][64]
+ *   k = 5       layer2.0.conv1 | downsample [1][128][320]   K = (dy*3 + dx)*32 + c (the 3x3/2 taps gathered at output resolution);
+ *                                                           rows 0..63 conv1, rows 64..127 downsample.0 in the centre-tap rows K 128..159
+ *   k = 6..8    layer2.0.conv2, layer2.1.{conv1,conv2}       [9][64][64]
+ *   k = 9       layer3.0.conv1 | downsample [1][256][576]   K = (dy*3 + dx)*64 + c; rows 128..255 downsample.0 in K 256..319
+ *   k = 10..12  layer3.0.conv2, layer3.1.{conv1,conv2}       [9][128][128]
+ *   k = 13      conv2 1x1 128->output_dim   [1][output_dim][128] */
+#define DBA_ENCODER_CONVS 14
+typedef struct {
+  const void* w[DBA_ENCODER_CONVS];
+  const float* b[DBA_ENCODER_CONVS];
+} dba_encoder_weights;
+
+typedef struct {
+  const void* images; int images_dtype;                /* [n_images,3,H,W], DBA_F32 or DBA_F16 */
+  int n_images, H, W;
+  const dba_encoder_weights* weights;                  /* HOST struct of DEVICE pointers */
+  int norm;                                            /* 0 = none (cnet), 1 = instance (fnet) */
+  int output_dim;                                      /* 128 or 256 */
+  void* out;                                           /* [n_images,output_dim,H/8,W/8] f16 */
+  void* workspace; size_t workspace_bytes;             /* dba_encoder_workspace_bytes(), 256-byte aligned */
+  dba_stream_t stream;
+} dba_encoder_args;
+
+/* 0 for extents without a kernel (n_images < 1, H or W not a positive multiple of 8, output_dim not 128 or 256) */
+size_t dba_encoder_workspace_bytes(int n_images, int H, int W, int output_dim);
+int dba_encoder_forward(const dba_encoder_args* a);
+
 /* ---- standalone damped SPD solve (the solver inside dba_ba_solve) ---------------------------------------
  * (H + diag(ep + lm*diag(H))) x = b with H [n,n] fp64 (full symmetric), b [n] fp64 -> x [n] fp32, on the device in
  * fp64; replaces SparseBlock::solve (reference src/droid_kernels.cu:1201-1222).  *fail_flag_device is set to 1 and x to 0
