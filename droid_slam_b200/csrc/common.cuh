@@ -22,6 +22,9 @@ struct CholPeers {            // fused peer-to-peer reduction (world > 1): H/b a
 int chol_solve_launch(const double* H, const double* b, int n, double lm, double ep, void* workspace, int* fail, float* x, cudaStream_t st,
                       const CholPeers* peers = nullptr);
 int cuda_fail(cudaError_t e, const char* what);
+// corr_lookup_rows.cu: dba_corr_lookup_pyramid for level rows that are not whole 16-byte chunks (arguments checked by the caller)
+int corr_lookup_pyramid_rows_launch(const __half* v0, const __half* v1, const __half* v2, const __half* v3, const float* coords, __half* out,
+                                    long long total, int h1, int w1, cudaStream_t st);
 
 #define DBA_CHECK_ARG(cond, msg)                                   \
   do { if (!(cond)) { dba::set_error("invalid argument: %s", msg); return DBA_ERR_INVALID; } } while (0)

@@ -25,32 +25,58 @@ from . import install
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook"]
 
 
+def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
+    """why corr_volume_pyramid has no kernel for these CorrBlock arguments (None: it has one)"""
+    if fmap1.dim() != 5 or fmap2.shape != fmap1.shape:
+        return "fmap1 and fmap2 must be [B,N,C,H,W] of one shape"
+    if not (fmap1.is_cuda and fmap2.is_cuda):
+        return "fmaps are not on a CUDA device"
+    if fmap1.dtype != torch.float16 or fmap2.dtype != torch.float16:
+        return "dtype %s / %s (float16 has a kernel)" % (fmap1.dtype, fmap2.dtype)
+    if num_levels != 4:
+        return "%d levels (4 has a kernel)" % num_levels
+    batch, num, dim, ht, wd = fmap1.shape
+    if dim != 128:
+        return "%d channels (128 has a kernel)" % dim
+    if ht < 8 or wd < 8:
+        return "%dx%d feature maps (ht and wd must be at least 8)" % (ht, wd)
+    if not be.corr_volume_supported(dim, ht, wd):
+        return "no kernel for %dx%d" % (ht, wd)
+    return None
+
+
 def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
-    """corr_module = the imported reference module `modules.corr`.  strict: shapes without a kernel (anything but f16, 128 channels,
-    wd = 64 handled by corr_volume_pyramid) raise instead of silently taking the reference's library path.
-    fused_lookup: additionally replace `CorrBlock.__call__` by the one-launch 4-level lookup `corr_lookup_pyramid`; the volumes of
-    levels 0 and 1 are then kept in the tiled private layout (64-byte DRAM atoms, about a third less HBM traffic per lookup) -- same
-    tensor shapes, `cat` / `__getitem__` over edges keep working, results bit-identical to the reference-layout path."""
+    """corr_module = the imported reference module `modules.corr`.  `CorrBlock.__init__` builds its pyramid with corr_volume_pyramid for
+    f16 feature maps with 128 channels, 4 levels and ht, wd >= 8.  strict: anything else raises (naming the reason) instead of silently
+    taking the reference's library path; with strict=False the reference's own methods run for it.
+    fused_lookup: additionally replace `CorrBlock.__call__` by the one-launch 4-level lookup `corr_lookup_pyramid`.  Where
+    corr_volume_pyramid has a tiled builder (wd = 64, ht % 8 == 0) the volumes of levels 0 and 1 are kept in the tiled private layout
+    (64-byte DRAM atoms, about a third less HBM traffic per lookup); elsewhere the reference layout.  Same tensor shapes, `cat` /
+    `__getitem__` over edges keep working, results bit-identical to the reference-layout path."""
     be = install()
-    ref_init = corr_module.CorrBlock.__init__
-    tiled = bool(fused_lookup)
+    ref_init, ref_call = corr_module.CorrBlock.__init__, corr_module.CorrBlock.__call__
 
     def __init__(self, fmap1, fmap2, num_levels=4, radius=3):
-        batch, num, dim, ht, wd = fmap1.shape
-        ok = fmap1.is_cuda and fmap1.dtype == torch.float16 and fmap2.dtype == torch.float16 and num_levels == 4 and be.corr_volume_supported(dim, ht, wd)
-        if not ok:
+        why = _corr_volume_unsupported(be, fmap1, fmap2, num_levels)
+        self._b200_native = why is None
+        if why is not None:
             if strict:
-                raise RuntimeError("corr_volume_pyramid has no kernel for fmaps %s %s, levels=%d" % (tuple(fmap1.shape), fmap1.dtype, num_levels))
+                raise RuntimeError("corr_volume_pyramid has no kernel for CorrBlock(%s %s, num_levels=%d): %s"
+                                   % (tuple(fmap1.shape), fmap1.dtype, num_levels, why))
             return ref_init(self, fmap1, fmap2, num_levels, radius)
+        batch, num, dim, ht, wd = fmap1.shape
+        tiled = bool(fused_lookup) and be.corr_volume_supported(dim, ht, wd, tiled=True)
         self.num_levels, self.radius = num_levels, radius
         idx = torch.arange(batch * num, device=fmap1.device)
         self.corr_pyramid = be.corr_volume_pyramid(fmap1.reshape(batch * num, dim, ht, wd).contiguous(), fmap2.reshape(batch * num, dim, ht, wd).contiguous(), idx, idx, tiled)
         self._b200_tiled = tiled
 
     def __call__(self, coords):
+        if not getattr(self, "_b200_native", False):
+            return ref_call(self, coords)
         batch, num, ht, wd, _ = coords.shape
         c = coords.permute(0, 1, 4, 2, 3).contiguous().view(batch * num, 2, ht, wd)
-        return be.corr_lookup_pyramid([v.contiguous() for v in self.corr_pyramid], c, getattr(self, "_b200_tiled", False)).view(batch, num, -1, ht, wd)
+        return be.corr_lookup_pyramid([v.contiguous() for v in self.corr_pyramid], c, self._b200_tiled).view(batch, num, -1, ht, wd)
 
     corr_module.CorrBlock.__init__ = __init__
     if fused_lookup:

@@ -55,22 +55,38 @@ int dba_corr_index_backward(const float* coords, const void* corr_grad, void* vo
  * /4-scaled feature maps + 3x avg_pool2d).  fmap1 [n_frames1,C,ht,wd], fmap2 [n_frames2,C,ht,wd] (f16, C = 128),
  * ii,jj [E] int64 frame indices into fmap1 / fmap2;  out_l [E,ht,wd,ht/2^l,wd/2^l] f16 for l = 0..3, fully overwritten.
  * One wgmma/TMA kernel writes all four levels in a single pass over the accumulator.
- * Implemented for wd = 64, ht % 8 == 0 (DBA_ERR_INVALID otherwise). */
-/* 1 when dba_corr_volume_pyramid has a kernel for this shape / dtype (f16, 128 channels, wd = 64, ht % 8 == 0), else 0 */
+ * Any ht, wd >= 8 (DBA_ERR_INVALID below: the reference's avg_pool2d fails on a 1-pixel level).  Level l keeps only the complete
+ * 2^l x 2^l blocks (avg_pool2d's floor rule): a trailing odd row or column is dropped at every level.  Level 0 is
+ * fp16(sum_c f1 f2 / 16) from fp32 accumulators; levels 1-3 are the fp32 cascade of 2x2 means, each rounded once.
+ * Checked before any launch: more than 65535 edges, null pointers, pointers not 16-byte aligned, a missing or small workspace. */
+/* 1 when dba_corr_volume_pyramid has a kernel for this shape / dtype (f16, 128 channels, ht >= 8, wd >= 8), else 0 */
 int dba_corr_volume_supported(int channels, int ht, int wd, int dtype);
+/* 1 when dba_corr_volume_pyramid_tiled has a kernel (f16, 128 channels, wd = 64, ht % 8 == 0), else 0 */
+int dba_corr_volume_tiled_supported(int channels, int ht, int wd, int dtype);
+/* device workspace of dba_corr_volume_pyramid_ws: 0 when wd % 8 == 0, else a copy of both feature-map tensors with rows padded to a
+ * multiple of 8 pixels (TMA global strides are multiples of 16 bytes), about 2 * 2 * C * ht * wd bytes per frame.  Read and written once
+ * per call: with one frame pair per edge about 1024 * ht * wd bytes per edge, against 2.66 * (ht * wd)^2 bytes of volume written. */
+size_t dba_corr_volume_workspace_bytes(int n_frames1, int n_frames2, int channels, int ht, int wd);
+/* every supported shape; workspace (16-byte aligned) of at least dba_corr_volume_workspace_bytes, may be NULL when that is 0 */
+int dba_corr_volume_pyramid_ws(const void* fmap1, const void* fmap2, const int64_t* ii, const int64_t* jj,
+                               void* out0, void* out1, void* out2, void* out3,
+                               int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype,
+                               void* workspace, size_t workspace_bytes, dba_stream_t stream);
+/* the same without a workspace: shapes with wd % 8 != 0 return DBA_ERR_INVALID */
 int dba_corr_volume_pyramid(const void* fmap1, const void* fmap2, const int64_t* ii, const int64_t* jj,
                             void* out0, void* out1, void* out2, void* out3,
                             int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype, dba_stream_t stream);
 
 /* private-layout variant: levels 0 and 1 of every plane stored as 4x8-element tiles ([h2/4][w2/8][4][8] f16 = one 64-byte DRAM atom per
  * tile) for dba_corr_lookup_pyramid(tiled_mask = 3); levels 2, 3 and all tensor shapes are unchanged.  NOT readable by
- * dba_corr_index_forward / the reference's CorrBlock.__call__. */
+ * dba_corr_index_forward / the reference's CorrBlock.__call__.  Only where dba_corr_volume_tiled_supported (DBA_ERR_INVALID elsewhere). */
 int dba_corr_volume_pyramid_tiled(const void* fmap1, const void* fmap2, const int64_t* ii, const int64_t* jj,
                                   void* out0, void* out1, void* out2, void* out3,
                                   int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype, dba_stream_t stream);
 /* CorrBlock.__call__ (reference droid_slam/modules/corr.py:40-50) in one launch: out [n,196,h1,w1] = concatenation over the four levels
  * of corr_index_forward(volume_l, coords / 2^l, 3) -- bit-identical values; coords [n,2,h1,w1] f32 at level-0 scale are read once.
- * f16 volumes, h1 % 8 == 0, w1 % 64 == 0.  tiled_mask: 0 = reference layout, 3 = levels 0 and 1 in the tiled layout above. */
+ * f16 volumes, h1, w1 >= 8, planes of level l [h1 >> l, w1 >> l], each level tensor 16-byte aligned; no load leaves a level tensor.
+ * tiled_mask: 0 = reference layout, 3 = levels 0 and 1 in the tiled layout above (h1 % 8 == 0 and w1 % 64 == 0 only). */
 int dba_corr_lookup_pyramid(const void* v0, const void* v1, const void* v2, const void* v3, const float* coords, void* out,
                             int n, int h1, int w1, int tiled_mask, int dtype, dba_stream_t stream);
 
