@@ -17,7 +17,8 @@ constexpr int kSlotsPerMTile = 8;  // EPI_GATE / EPI_STATS partial-sum slots per
 struct ConvParams {
   int E, HT, WD;                    // images (edges or frames), image height / width
   int TW, RM, MT;                   // tile width in pixels, image rows per 128-pixel M tile (RM * TW = 128), M tiles per CTA tile
-  int tiles_x, tiles_y, n_ntiles;   // CTA tiles per image, N tiles (output-channel blocks)
+                                    // (row-flattened tiles: TW = row pitch TWp, RM unused)
+  int tiles_x, tiles_y, n_ntiles;   // CTA tiles per image (row-flattened: tiles_x linear tiles, tiles_y = 1), N tiles (output-channel blocks)
   int KS;                           // kernel size 1 or 3
   int nk0, nk1;                     // 64-channel K blocks taken from source 0 / source 1
   int N;                            // output channels per N tile (<= 256)
@@ -62,8 +63,9 @@ __device__ __forceinline__ float2 ldh2(const __half* p) { return __half22float2(
 constexpr int conv_max_mt(int nw) { return 256 / nw < 4 ? 256 / nw : 4; }
 
 // epilogue of one 64-pixel x N fragment (M tile t of the CTA tile) of consumer warpgroup wg: this thread holds pixels r, r + 8
-// (r = 16 (warp % 4) + lane / 4) and columns 8 j + 2 (lane % 4) + {0, 1}
-template <int EPI, int NW>
+// (r = 16 (warp % 4) + lane / 4) and columns 8 j + 2 (lane % 4) + {0, 1}.  Row-flattened tiles (FLAT): ty = 0, tx = linear tile,
+// pixel m is flat index q = tx * 128 MT + 128 t + m on the padded row pitch TW, i.e. y = q / TW, x = q mod TW.
+template <int EPI, int NW, bool FLAT>
 __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (&acc)[NW / 2], int t, int wg, int warp, int lane, int nt, int e, int ty,
                                               int tx) {
   const int qd = lane & 3;
@@ -72,8 +74,14 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
 #pragma unroll
   for (int i = 0; i < 2; i++) {
     const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
-    const int my = m / p.TW, mx = m - my * p.TW;
-    const int y = ty * (p.MT * p.RM) + t * p.RM + my, x = tx * p.TW + mx;
+    int y, x;
+    if constexpr (FLAT) {
+      const int q = (tx * p.MT + t) * 128 + m;
+      y = q / p.TW; x = q - y * p.TW;
+    } else {
+      const int my = m / p.TW, mx = m - my * p.TW;
+      y = ty * (p.MT * p.RM) + t * p.RM + my; x = tx * p.TW + mx;
+    }
     const bool valid = y < p.HT && x < p.WD;
     const size_t pix = ((size_t)e * p.HT + (valid ? y : 0)) * p.WD + (valid ? x : 0);
 #pragma unroll
@@ -178,7 +186,16 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
   }
 }
 
-template <int EPI, int NW>
+// Two tilings, chosen at compile time:
+//  * FLAT = false: a CTA tile is MT M tiles of RM image rows x TW columns (TW = 64 or 32); per (K block, dx) one TMA box of
+//    TW x (MT RM + KS - 1) pixels, the A operand of tap dy at box pixel (t RM + dy) TW + 64 wg.
+//  * FLAT = true (row-flattened): pixels are numbered row-major on the row pitch TW = TWp = wd rounded up to a multiple of 8, and a
+//    CTA tile is the 128 MT consecutive pixels from p0 = tx * 128 MT (it may start mid-row).  Per (K block, dx) one TMA box of TWp
+//    columns x box_rows rows anchored at row y0 - pad (y0 = p0 / TWp), column dx - pad; columns >= wd and rows outside [0, ht) are
+//    TMA zero fill, so no buffer needs padded columns.  The A operand of tap dy is box pixel c0 + 128 t + dy TWp + 64 wg with
+//    c0 = p0 mod TWp.  TWp and c0 are multiples of 8, so every such offset is a multiple of the 1024-byte 128B-swizzle atom (8 rows
+//    of 128 bytes) and the gmma_desc_sw128 descriptors hold unchanged: this is why TWp is wd rounded up to 8 and not wd itself.
+template <int EPI, int NW, bool FLAT = false>
 __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                                                                const __grid_constant__ CUtensorMap tmW, const ConvParams p) {
   constexpr int kMT = conv_max_mt(NW);
@@ -215,7 +232,12 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
         const int e = r0 / tiles_per_img;
         const int r1 = r0 - e * tiles_per_img;
         const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
-        const int y0 = ty * (p.MT * p.RM), x0 = tx * p.TW;
+        int y0, x0;
+        if constexpr (FLAT) {
+          y0 = (tx * p.MT * 128) / p.TW; x0 = 0;
+        } else {
+          y0 = ty * (p.MT * p.RM); x0 = tx * p.TW;
+        }
         for (int kb = 0; kb < nk; kb++) {
           const CUtensorMap* am = kb < p.nk0 ? &tmA0 : &tmA1;
           const int ch = (kb < p.nk0 ? kb : kb - p.nk0) * 64;
@@ -252,6 +274,7 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
     const int e = r0 / tiles_per_img;
     const int r1 = r0 - e * tiles_per_img;
     const int ty = r1 / p.tiles_x, tx = r1 - ty * p.tiles_x;
+    const int c0 = FLAT ? (tx * p.MT * 128) % p.TW : 0;               // row-flattened: column of the tile's first pixel in box row 0
     bool first = true;
     int pend_a = -1, pend_b = -1;
     for (int kb = 0; kb < nk; kb++) {
@@ -266,7 +289,8 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
           for (int t = 0; t < kMT; t++) {
             if (t < p.MT) {
-              const uint32_t a_base = sA_u + as * p.a_bytes + (uint32_t)((t * p.RM + dy) * p.TW + wg * 64) * 128u;
+              const uint32_t a_base = sA_u + as * p.a_bytes +
+                                      (uint32_t)(FLAT ? c0 + t * 128 + dy * p.TW + wg * 64 : (t * p.RM + dy) * p.TW + wg * 64) * 128u;
 #pragma unroll
               for (int k = 0; k < 4; k++)
                 wgmma_f16<NW>(acc[t], gmma_desc_sw128(a_base + k * 32, 16, 1024), gmma_desc_sw128(b_base + k * 32, 16, 1024), (first && k == 0) ? 0 : 1, 0);
@@ -297,7 +321,7 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
     for (int t = 0; t < kMT; t++) {
       wgmma_fence_regs(acc[t]);
-      if (t < p.MT) conv_epilogue<EPI, NW>(p, acc[t], t, wg, warp, lane, nt, e, ty, tx);
+      if (t < p.MT) conv_epilogue<EPI, NW, FLAT>(p, acc[t], t, wg, warp, lane, nt, e, ty, tx);
     }
   }
 }
@@ -356,26 +380,42 @@ constexpr bool conv_width_used(int nw) {
          ((EPI == EPI_STATS || EPI == EPI_RELU_RES) && (nw == 32 || nw == 64 || nw == 128 || nw == 256));
 }
 
-template <int EPI, int NW>
+template <int EPI, int NW, bool FLAT>
 static int launch_conv_nw(const ConvParams& p, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tW, int grid, int smem, cudaStream_t st) {
-  if constexpr (!conv_width_used<EPI>(NW)) {
+  if constexpr (!conv_width_used<EPI>(NW) || (FLAT && (EPI == EPI_STATS || EPI == EPI_RELU_RES))) {
     set_error("update operator: no convolution kernel for this epilogue with %d output channels", NW);
     return DBA_ERR_INVALID;
   } else {
     static bool attr_set = false;
     if (!attr_set) {
-      DBA_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<EPI, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), "conv_tc smem attr");
+      DBA_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<EPI, NW, FLAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024), "conv_tc smem attr");
       attr_set = true;
     }
-    conv_tc_kernel<EPI, NW><<<grid, kUpThreads, smem, st>>>(tA0, tA1, tW, p);
+    conv_tc_kernel<EPI, NW, FLAT><<<grid, kUpThreads, smem, st>>>(tA0, tA1, tW, p);
     DBA_CHECK_LAUNCH("conv_tc_kernel");
     return DBA_OK;
   }
 }
 
+template <int EPI, bool FLAT>
+static int launch_conv_n(const ConvParams& p, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tW, int grid, int smem, cudaStream_t st) {
+  switch (p.N) {
+    case 32: return launch_conv_nw<EPI, 32, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    case 64: return launch_conv_nw<EPI, 64, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    case 96: return launch_conv_nw<EPI, 96, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    case 128: return launch_conv_nw<EPI, 128, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    case 160: return launch_conv_nw<EPI, 160, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    case 192: return launch_conv_nw<EPI, 192, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    case 224: return launch_conv_nw<EPI, 224, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+    default: return launch_conv_nw<EPI, 256, FLAT>(p, tA0, tA1, tW, grid, smem, st);
+  }
+}
+
 // one convolution launch.  src0 (+ optional src1) = channels-last sources concatenated along K; wpk = packed weights
 // [KS*KS][n_ntiles*N][Kpad] with Kpad = 64 * (kblocks(src0) + kblocks(src1)).
-template <int EPI>
+// ROW_FLAT (the update operator): widths that are not a multiple of 8 take the row-flattened tiles of conv_tc_kernel where 2 halo
+// and 2 weight stages of them fit in shared memory; the rectangular tiles, correct at every width, run everywhere else.
+template <int EPI, bool ROW_FLAT = false>
 static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cudaStream_t st, int* slots_out = nullptr) {
   if (!g_num_sms) {
     int dev = 0; cudaGetDevice(&dev);
@@ -388,24 +428,47 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
     p.N = 192;
   }
   if (p.N % 32 != 0 || p.N < 32) { set_error("update operator: %d output channels per tile", p.N); return DBA_ERR_INVALID; }
-  p.TW = (p.WD % 64 == 0) ? 64 : 32;
-  p.RM = 128 / p.TW;
-  // M tiles per CTA tile: every weight stage is shared by MT tiles (and every halo row by 3 taps), so larger is better for the
-  // L2 -> SM traffic per MAC; bounded by the register accumulators (MT * N <= 256 columns) and by the image height
-  p.MT = (p.HT >= 2 * p.RM) ? 2 : 1;
-  if (p.N <= 64 && p.HT >= 4 * p.RM && (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0) >= 4 && p.KS == 3) p.MT = 4;
-  if (p.MT > conv_max_mt(p.N)) p.MT = conv_max_mt(p.N);
-  p.tiles_x = (p.WD + p.TW - 1) / p.TW;
-  p.tiles_y = (p.HT + p.MT * p.RM - 1) / (p.MT * p.RM);
+  const int budget = 227 * 1024 - 2048;
+  const int nk = (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0);
+  int box_rows = 0;
+  bool flat = false;
+  if constexpr (ROW_FLAT) {
+    if (p.WD % 8 != 0) {
+      // row-flattened tiles (conv_tc_kernel): 128 MT consecutive pixels on the row pitch twp; the halo box spans the rows those
+      // pixels touch from any start column c0 <= twp - 8, plus KS - 1 halo rows.  MT as for the rectangular tiles below.
+      const int twp = (p.WD + 7) & ~7, px = p.HT * twp;
+      int mt = px >= 2 * 128 ? 2 : 1;
+      if (p.N <= 64 && px >= 4 * 128 && nk >= 4 && p.KS == 3) mt = 4;
+      if (mt > conv_max_mt(p.N)) mt = conv_max_mt(p.N);
+      const int rows = (twp - 8 + 128 * mt + twp - 1) / twp + p.KS - 1;
+      if (twp <= 256 && 2 * rows * twp * 128 + 2 * p.N * 128 <= budget) {   // TMA box extents <= 256; 2 halo + 2 weight stages
+        flat = true;
+        p.TW = twp; p.RM = 0; p.MT = mt;
+        p.tiles_x = (px + 128 * mt - 1) / (128 * mt);
+        p.tiles_y = 1;
+        box_rows = rows;
+      }
+    }
+  }
+  if (!flat) {
+    p.TW = (p.WD % 64 == 0) ? 64 : 32;
+    p.RM = 128 / p.TW;
+    // M tiles per CTA tile: every weight stage is shared by MT tiles (and every halo row by 3 taps), so larger is better for the
+    // L2 -> SM traffic per MAC; bounded by the register accumulators (MT * N <= 256 columns) and by the image height
+    p.MT = (p.HT >= 2 * p.RM) ? 2 : 1;
+    if (p.N <= 64 && p.HT >= 4 * p.RM && nk >= 4 && p.KS == 3) p.MT = 4;
+    if (p.MT > conv_max_mt(p.N)) p.MT = conv_max_mt(p.N);
+    p.tiles_x = (p.WD + p.TW - 1) / p.TW;
+    p.tiles_y = (p.HT + p.MT * p.RM - 1) / (p.MT * p.RM);
+    box_rows = p.MT * p.RM + p.KS - 1;
+  }
   p.nk0 = (s0.C + 63) / 64;
   p.nk1 = s1.base ? (s1.C + 63) / 64 : 0;
   p.boxn = p.N;
-  const int box_rows = p.MT * p.RM + p.KS - 1;
   p.a_bytes = box_rows * p.TW * 128;
   p.b_bytes = p.N * 128;
   // shared memory: at least 2 halo stages and 3 weight stages; what is left goes to more halo stages (up to 4: with narrow N the
   // MMAs of a stage are short and the TMA latency of the next halo tile is what the pipeline has to cover), then weight stages
-  const int budget = 227 * 1024 - 2048;
   p.a_stages = 2;
   while (p.a_stages < 4 && (p.a_stages + 1) * p.a_bytes + 4 * p.b_bytes <= budget) p.a_stages++;
   p.b_stages = (budget - p.a_stages * p.a_bytes) / p.b_bytes;
@@ -422,16 +485,10 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   const long long total = (long long)p.n_ntiles * p.E * p.tiles_x * p.tiles_y;
   if (total <= 0) return DBA_OK;
   const int grid = (int)(total < g_num_sms ? total : g_num_sms);
-  switch (p.N) {
-    case 32: return launch_conv_nw<EPI, 32>(p, tA0, tA1, tW, grid, smem, st);
-    case 64: return launch_conv_nw<EPI, 64>(p, tA0, tA1, tW, grid, smem, st);
-    case 96: return launch_conv_nw<EPI, 96>(p, tA0, tA1, tW, grid, smem, st);
-    case 128: return launch_conv_nw<EPI, 128>(p, tA0, tA1, tW, grid, smem, st);
-    case 160: return launch_conv_nw<EPI, 160>(p, tA0, tA1, tW, grid, smem, st);
-    case 192: return launch_conv_nw<EPI, 192>(p, tA0, tA1, tW, grid, smem, st);
-    case 224: return launch_conv_nw<EPI, 224>(p, tA0, tA1, tW, grid, smem, st);
-    default: return launch_conv_nw<EPI, 256>(p, tA0, tA1, tW, grid, smem, st);
+  if constexpr (ROW_FLAT) {
+    if (flat) return launch_conv_n<EPI, true>(p, tA0, tA1, tW, grid, smem, st);
   }
+  return launch_conv_n<EPI, false>(p, tA0, tA1, tW, grid, smem, st);
 }
 
 }  // namespace dba

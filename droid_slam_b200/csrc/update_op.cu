@@ -9,7 +9,8 @@
 //     for free (cp.async.bulk.tensor.4d with out-of-bounds fill at negative / beyond-the-edge coordinates);
 //   * per (64-channel block, dx) ONE halo tile of (rows + 2) image rows is loaded and the three dy taps are the same
 //     shared-memory buffer at +dy*TW*128 bytes (a multiple of the 1024-byte swizzle atom), so a 3x3 convolution reads its
-//     input 3x (not 9x) from L2;
+//     input 3x (not 9x) from L2; widths that are not a multiple of 8 take row-flattened tiles instead (128 consecutive pixels of
+//     the image on a row pitch rounded up to 8, conv_engine.cuh), so odd widths cost ~1.1x, not ~1.5x, the tensor work they need;
 //   * weights are pre-packed [tap][N][K] f16 (K contiguous) and stream through a second TMA ring;
 //   * wgmma.m64nNk16 (f16 operands from shared memory, fp32 accumulators in registers), N = the output channels of the tile
 //     (up to 256; 384 outputs run as two 192-wide N tiles), M = 128 pixels per tile (x MT tiles sharing every weight stage);
@@ -215,7 +216,13 @@ static UpWs up_layout(int E, int n_src, int ht, int wd) {
   UpWs w;
   const size_t px = (size_t)E * ht * wd, spx = (size_t)(n_src > 0 ? n_src : 1) * ht * wd;
   const int tw = (wd % 64 == 0) ? 64 : 32, rm = 128 / tw;
-  const size_t slots = (size_t)((wd + tw - 1) / tw) * ((ht + rm - 1) / rm) * kSlotsPerMTile * 2;   // upper bound over MT
+  size_t slots = (size_t)((wd + tw - 1) / tw) * ((ht + rm - 1) / rm) * kSlotsPerMTile * 2;   // upper bound over MT
+  if (wd % 8 != 0) {
+    // row-flattened tiles (launch_conv): ceil(P / (128 MT)) CTA tiles of MT M tiles, P = ht * (wd rounded up to 8), so at most
+    // ceil(P / 128) + MT - 1 <= ceil(P / 128) + 3 M tiles
+    const size_t flat = ((size_t)ht * ((wd + 7) & ~7) + 127) / 128 + 3;
+    if (flat * kSlotsPerMTile > slots) slots = flat * kSlotsPerMTile;
+  }
   size_t o = 0;
   w.hin = o; o += al256(px * 128 * 2);
   w.x320 = o; o += al256(px * 320 * 2);
@@ -251,7 +258,6 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
   if (E == 0) return DBA_OK;
   DBA_CHECK_ARG(a->net && a->inp && a->corr && a->net_out && a->delta && a->weight && a->weights && a->workspace, "null pointer");
   DBA_CHECK_ARG(n_src == 0 || (a->seg && a->eta && a->upmask), "aggregation outputs / segment ids missing");
-  DBA_CHECK_ARG(wd % 8 == 0, "update operator: image width must be a multiple of 8");
   const UpWs L = up_layout(E, n_src, ht, wd);
   DBA_CHECK_ARG(a->workspace_bytes >= L.total, "workspace too small (dba_update_workspace_bytes)");
   DBA_CHECK_ARG(((uintptr_t)a->workspace & 255) == 0 && ((uintptr_t)a->net_out & 15) == 0 && ((uintptr_t)a->net & 15) == 0, "pointers must be 16-byte aligned (workspace 256)");
@@ -305,36 +311,36 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
   int rc;
   // ---- corr_encoder: 1x1 196->128 + ReLU, 3x3 128->128 + ReLU -> X[:, 128:256]   (droid_net.py:83-87)
   { ConvParams p = base; p.KS = 1; p.N = 128; p.bias = W->b_corr0; p.relu = 1; p.out = C1; p.out_stride = 128;
-    rc = launch_conv<EPI_STORE>(p, ConvSrc{Cc, 196, 200}, none, W->w_corr0, st); if (rc) return rc; }
+    rc = launch_conv<EPI_STORE, true>(p, ConvSrc{Cc, 196, 200}, none, W->w_corr0, st); if (rc) return rc; }
   { ConvParams p = base; p.KS = 3; p.N = 128; p.bias = W->b_corr2; p.relu = 1; p.out = X + 128; p.out_stride = 320;
-    rc = launch_conv<EPI_STORE>(p, ConvSrc{C1, 128, 128}, none, W->w_corr2, st); if (rc) return rc; }
+    rc = launch_conv<EPI_STORE, true>(p, ConvSrc{C1, 128, 128}, none, W->w_corr2, st); if (rc) return rc; }
   // ---- flow_encoder: 7x7 4->128 + ReLU (as a 196-wide 1x1 over the im2col rows), 3x3 128->64 + ReLU -> X[:, 256:320]   (:89-93)
   { ConvParams p = base; p.KS = 1; p.N = 128; p.bias = W->b_flow0; p.relu = 1; p.out = F1; p.out_stride = 128;
-    rc = launch_conv<EPI_STORE>(p, ConvSrc{F0, 196, 200}, none, W->w_flow0, st); if (rc) return rc; }
+    rc = launch_conv<EPI_STORE, true>(p, ConvSrc{F0, 196, 200}, none, W->w_flow0, st); if (rc) return rc; }
   { ConvParams p = base; p.KS = 3; p.N = 64; p.bias = W->b_flow2; p.relu = 1; p.out = X + 256; p.out_stride = 320;
-    rc = launch_conv<EPI_STORE>(p, ConvSrc{F1, 128, 128}, none, W->w_flow2, st); if (rc) return rc; }
+    rc = launch_conv<EPI_STORE, true>(p, ConvSrc{F1, 128, 128}, none, W->w_flow2, st); if (rc) return rc; }
   // ---- ConvGRU (gru.py:19-32): global context
   int slots = 0;
   { ConvParams p = base; p.KS = 1; p.N = 128; p.bias = W->b_gate; p.h = H; p.h_stride = 128; p.partial = partial;
-    rc = launch_conv<EPI_GATE>(p, ConvSrc{H, 128, 128}, none, W->w_gate, st, &slots); if (rc) return rc; }
+    rc = launch_conv<EPI_GATE, true>(p, ConvSrc{H, 128, 128}, none, W->w_gate, st, &slots); if (rc) return rc; }
   glo_kernel<<<E, 384, 0, st>>>(partial, slots, 1.f / (float)HW, W->w_glo, W->b_glo, glo);
   DBA_CHECK_LAUNCH("glo_kernel");
   // z, r = sigmoid(conv3x3(h | x) + glo): one 256-output convolution; epilogue writes z and r*h
   { ConvParams p = base; p.KS = 3; p.N = 256; p.bias = W->b_zr; p.h = H; p.h_stride = 128; p.glo = glo; p.z = Z; p.rh = RH;
-    rc = launch_conv<EPI_ZR>(p, ConvSrc{H, 128, 128}, ConvSrc{X, 320, 320}, W->w_zr, st); if (rc) return rc; }
+    rc = launch_conv<EPI_ZR, true>(p, ConvSrc{H, 128, 128}, ConvSrc{X, 320, 320}, W->w_zr, st); if (rc) return rc; }
   // q = tanh(conv3x3(r*h | x) + glo); h' = (1-z) h + z q
   { ConvParams p = base; p.KS = 3; p.N = 128; p.bias = W->b_q; p.h = H; p.h_stride = 128; p.glo = glo; p.z = Z;
     p.out = (__half*)a->net_out; p.out_stride = 128;
-    rc = launch_conv<EPI_Q>(p, ConvSrc{RH, 128, 128}, ConvSrc{X, 320, 320}, W->w_q, st); if (rc) return rc; }
+    rc = launch_conv<EPI_Q, true>(p, ConvSrc{RH, 128, 128}, ConvSrc{X, 320, 320}, W->w_q, st); if (rc) return rc; }
   // ---- heads: stems delta.0 | weight.0 | agg.conv1 as one 384-output convolution + ReLU (droid_net.py:95-106, :60)
   const int stemN = n_src > 0 ? 384 : 256;
   { ConvParams p = base; p.KS = 3; p.N = stemN; p.w_rows = 384; p.bias = W->b_stem; p.relu = 1; p.out = S; p.out_stride = 384;
-    rc = launch_conv<EPI_STORE>(p, ConvSrc{a->net_out, 128, 128}, none, W->w_stem, st); if (rc) return rc; }
+    rc = launch_conv<EPI_STORE, true>(p, ConvSrc{a->net_out, 128, 128}, none, W->w_stem, st); if (rc) return rc; }
   // delta.2 and weight.2 (3x3 128->2 each): per-tap partial sums by one 1x1 convolution 256 -> 36 (block-diagonal weights), then the
   // 9-tap gather with bias / sigmoid
   float* Yh = (float*)(ws + L.cc);                        // [E,HW,36] f32 on the (dead) corr staging buffer
   { ConvParams p = base; p.KS = 1; p.N = 64; p.bias = W->b_zero; p.f32a = Yh; p.f32_cols = 36; p.f32_stride = 36;
-    rc = launch_conv<EPI_F32>(p, ConvSrc{S, 256, 384}, none, W->w_heads, st); if (rc) return rc; }
+    rc = launch_conv<EPI_F32, true>(p, ConvSrc{S, 256, 384}, none, W->w_heads, st); if (rc) return rc; }
   head_gather_kernel<<<(unsigned)(((size_t)E * HW + 255) / 256), 256, 0, st>>>(Yh, 36, 4, W->b_heads, 0, a->delta, a->weight, E, ht, wd);
   DBA_CHECK_LAUNCH("head_gather_kernel");
   if (n_src > 0) {
@@ -344,20 +350,21 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
     DBA_CHECK_LAUNCH("segment mean");
     ConvParams fb = base; fb.E = n_src;
     { ConvParams p = fb; p.KS = 3; p.N = 128; p.bias = W->b_agg2; p.relu = 1; p.out = B2; p.out_stride = 128;
-      rc = launch_conv<EPI_STORE>(p, ConvSrc{Am, 128, 128}, none, W->w_agg2, st); if (rc) return rc; }
+      rc = launch_conv<EPI_STORE, true>(p, ConvSrc{Am, 128, 128}, none, W->w_agg2, st); if (rc) return rc; }
     float* Ye = (float*)(ws + L.f0);                      // [n_src,HW,12] f32 (9 used) on the (dead) flow im2col buffer
     { ConvParams p = fb; p.KS = 1; p.N = 32; p.bias = W->b_zero; p.f32a = Ye; p.f32_cols = 12; p.f32_stride = 12;
-      rc = launch_conv<EPI_F32>(p, ConvSrc{B2, 128, 128}, none, W->w_eta, st); if (rc) return rc; }
+      rc = launch_conv<EPI_F32, true>(p, ConvSrc{B2, 128, 128}, none, W->w_eta, st); if (rc) return rc; }
     head_gather_kernel<<<(unsigned)(((size_t)n_src * HW + 255) / 256), 256, 0, st>>>(Ye, 12, 1, W->b_eta, 1, a->eta, nullptr, n_src, ht, wd);
     DBA_CHECK_LAUNCH("head_gather_kernel(eta)");
     { ConvParams p = fb; p.KS = 1; p.N = 192; p.n_ntiles = 3; p.bias = W->b_upmask; p.nchw = (__half*)a->upmask; p.nchw_C = 576;
-      rc = launch_conv<EPI_NCHW>(p, ConvSrc{B2, 128, 128}, none, W->w_upmask, st); if (rc) return rc; }
+      rc = launch_conv<EPI_NCHW, true>(p, ConvSrc{B2, 128, 128}, none, W->w_upmask, st); if (rc) return rc; }
   }
   return DBA_OK;
 }
 
 // channels-last tensor-core convolution building block (the kernel behind every layer of dba_update_forward), exported for
-// tests and for callers that keep activations channels-last: out[e,y,x,n] = act(bias[n] + sum_{tap,k} src[e,y+dy,x+dx,k] w[tap][n][k])
+// tests and for callers that keep activations channels-last: out[e,y,x,n] = act(bias[n] + sum_{tap,k} src[e,y+dy,x+dx,k] w[tap][n][k]).
+// Any ht, wd > 0, tiled by the same rule as dba_update_forward.
 extern "C" int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* src1, int c1, int stride1, const void* wpk, const float* bias,
                              void* out, int out_stride, int n_images, int ht, int wd, int ksize, int n_out, int relu, dba_stream_t stream) {
   DBA_CHECK_ARG(src0 && wpk && bias && out, "null pointer");
@@ -372,5 +379,5 @@ extern "C" int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* 
   memset(&p, 0, sizeof(p));
   p.E = n_images; p.HT = ht; p.WD = wd; p.n_ntiles = 1; p.KS = ksize; p.N = n_out; p.bias = bias; p.relu = relu;
   p.out = (__half*)out; p.out_stride = out_stride;
-  return launch_conv<EPI_STORE>(p, ConvSrc{src0, c0, stride0}, ConvSrc{src1, c1, stride1}, wpk, (cudaStream_t)stream);
+  return launch_conv<EPI_STORE, true>(p, ConvSrc{src0, c0, stride0}, ConvSrc{src1, c1, stride1}, wpk, (cudaStream_t)stream);
 }

@@ -229,7 +229,8 @@ int dba_ba_read_info(const dba_ba_args* a, int* n_depth_frames, int* device_stat
  * replaces UpdateModule.forward (reference droid_slam/droid_net.py:111-143), ConvGRU.forward (droid_slam/modules/gru.py:19-32) and
  * GraphAgg.forward (droid_net.py:59-75) -- in the reference a chain of 19 cuDNN convolutions + ~25 elementwise launches.
  * Every convolution runs as an implicit GEMM (wgmma / TMA, f16 operands, fp32 accumulation) on channels-last
- * activations; gates, activations, the global-context sum and output layouts are fused into the epilogues.
+ * activations; gates, activations, the global-context sum and output layouts are fused into the epilogues.  Any ht, wd > 0: widths
+ * that are not a multiple of 8 (e.g. 69, 70, 73 at 1/8 of the reference's demo / ETH3D image sizes) run row-flattened tiles.
  *
  * Packed weights (device memory, made once per checkpoint by the host side, droid_slam_b200/update.py:pack_update_weights):
  *   w_* : f16 [taps][N][Kpad]  (tap = dy*k + dx, K = input channels in the reference's concatenation order, zero padded to a
@@ -271,7 +272,8 @@ int dba_update_forward(const dba_update_args* a);
 /* the building block of dba_update_forward, exported: 1x1 / 3x3 'same' convolution of channels-last f16 activations on the tensor
  * cores.  src0 (+ optional src1, concatenated along channels after src0) [n_images,ht,wd,stride] using channels [0,c); wpk f16
  * [ksize*ksize][n_out][Kpad] with Kpad = 64*ceil(c0/64) + 64*ceil(c1/64), K contiguous; bias f32 [n_out]; out f16
- * [n_images,ht,wd,out_stride] channels [0,n_out) written.  n_out in {32,64,...,256,384}. */
+ * [n_images,ht,wd,out_stride] channels [0,n_out) written.  n_out in {32,64,...,256,384}; any ht, wd > 0, tiled as in
+ * dba_update_forward. */
 int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* src1, int c1, int stride1, const void* wpk, const float* bias,
                   void* out, int out_stride, int n_images, int ht, int wd, int ksize, int n_out, int relu, dba_stream_t stream);
 
