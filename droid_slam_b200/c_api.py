@@ -9,7 +9,7 @@ SYMBOLS = [
     "dba_corr_index_forward", "dba_corr_index_backward", "dba_corr_volume_pyramid", "dba_corr_volume_pyramid_tiled", "dba_corr_lookup_pyramid", "dba_corr_volume_supported",
     "dba_corr_volume_tiled_supported", "dba_corr_volume_workspace_bytes", "dba_corr_volume_pyramid_ws", "dba_altcorr_forward", "dba_altcorr_backward",
     "dba_altcorr_pyramid", "dba_altcorr_lookup_pyramid",
-    "dba_projmap", "dba_reproject", "dba_cvx_upsample", "dba_frame_distance", "dba_depth_filter", "dba_iproj",
+    "dba_projmap", "dba_reproject", "dba_motion_features", "dba_graph_writeback", "dba_cvx_upsample", "dba_frame_distance", "dba_depth_filter", "dba_iproj",
     "dba_ba_workspace_bytes", "dba_ba_system_offset", "dba_ba_system_bytes",
     "dba_ba_prepare", "dba_ba_build", "dba_ba_solve", "dba_ba", "dba_ba_read_info", "dba_ba_p2p_signal",
     "dba_solve_workspace_bytes", "dba_solve_spd", "dba_solve_tile_placement",
@@ -71,6 +71,10 @@ def load():
     L.dba_altcorr_lookup_pyramid.argtypes = [vp] * 8 + [ci] * 9 + [vp]
     L.dba_projmap.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, vp]
     L.dba_reproject.argtypes = [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, vp]
+    L.dba_motion_features.argtypes = [vp] * 10 + [ci] * 3 + [vp]
+    L.dba_graph_writeback.argtypes = [vp] * 4 + [ci] + [vp] * 4 + [ci] + [vp, vp, ci, vp, vp, ci, vp, cf, ci, ci, vp]
+    L.dba_update_workspace_bytes.restype = ctypes.c_size_t
+    L.dba_update_workspace_bytes.argtypes = [ci] * 4
     L.dba_frame_distance.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
     L.dba_depth_filter.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]
     L.dba_iproj.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp]

@@ -360,6 +360,94 @@ std::vector<torch::Tensor> reproject(torch::Tensor poses, torch::Tensor disps, t
   return {coords, valid};
 }
 
+static void check_rows(const torch::Tensor& t, const char* name, const torch::Device& dev, int64_t per_row, const char* shape) {
+  CHECK_CONTIGUOUS(t); CHECK_F32(t);
+  TORCH_CHECK(t.device() == dev, name, " must be on ", dev);
+  TORCH_CHECK(t.dim() >= 1 && t.numel() % per_row == 0, name, " must be ", shape);
+}
+
+static const int64_t* opt_index(const c10::optional<torch::Tensor>& t, const torch::Device& dev, int64_t n, const char* name) {
+  if (!t.has_value() || !t->defined()) return nullptr;
+  CHECK_CONTIGUOUS((*t)); CHECK_I64((*t));
+  TORCH_CHECK(t->device() == dev && t->numel() == n, name, " must be an int64 tensor of ", n, " entries on ", dev);
+  return t->data_ptr<int64_t>();
+}
+
+// extension: FactorGraph.update / update_lowmem motion features (reference factor_graph.py:220-222, :280-282) fused with the reprojection.
+// poses [N,7], disps [N,ht,wd], intrinsics [N,4], ii / jj [E] int64, target [(1,)E,ht,wd,2] f32; call row r reads edge edge_index[r]
+// (all E edges in order when edge_index is None).  Returns [coords [n,ht,wd,2], coords_t [n,2,ht,wd], motn [n,4,ht,wd]].
+std::vector<torch::Tensor> motion_features(torch::Tensor poses, torch::Tensor disps, torch::Tensor intrinsics, torch::Tensor ii, torch::Tensor jj,
+                                           torch::Tensor target, c10::optional<torch::Tensor> edge_index) {
+  CHECK_INPUT(poses); CHECK_INPUT(disps); CHECK_INPUT(intrinsics); CHECK_INPUT(ii); CHECK_INPUT(jj);
+  CHECK_F32(poses); CHECK_F32(disps); CHECK_F32(intrinsics); CHECK_I64(ii); CHECK_I64(jj);
+  TORCH_CHECK(disps.dim() == 3 && intrinsics.dim() == 2 && intrinsics.size(1) == 4, "disps [N,ht,wd], intrinsics [N,4]");
+  const auto dev = poses.device();
+  TORCH_CHECK(disps.device() == dev && intrinsics.device() == dev && ii.device() == dev && jj.device() == dev, "motion_features: all tensors on one device");
+  c10::cuda::CUDAGuard guard(dev);
+  const int E = (int)ii.numel(), ht = (int)disps.size(1), wd = (int)disps.size(2);
+  TORCH_CHECK(jj.numel() == E, "ii and jj must have the same length");
+  check_rows(target, "target", dev, (int64_t)ht * wd * 2, "[E,ht,wd,2]");
+  TORCH_CHECK(target.numel() == (int64_t)E * ht * wd * 2, "target must be [E,ht,wd,2] with E = len(ii)");
+  const int n = (edge_index.has_value() && edge_index->defined()) ? (int)edge_index->numel() : E;
+  const int64_t* ei = opt_index(edge_index, dev, n, "edge_index");
+  auto coords = torch::empty({n, ht, wd, 2}, poses.options());
+  auto coords_t = torch::empty({n, 2, ht, wd}, poses.options());
+  auto motn = torch::empty({n, 4, ht, wd}, poses.options());
+  check_status(dba_motion_features(poses.data_ptr<float>(), disps.data_ptr<float>(), intrinsics.data_ptr<float>(), ii.data_ptr<int64_t>(),
+                                   jj.data_ptr<int64_t>(), ei, target.data_ptr<float>(), coords.data_ptr<float>(), coords_t.data_ptr<float>(),
+                                   motn.data_ptr<float>(), n, ht, wd, cur_stream()), "motion_features");
+  return {coords, coords_t, motn};
+}
+
+// extension: write-back of one update-operator call into the factor graph and BA's inputs (reference factor_graph.py:234-251, :304-320).
+// delta / weight / coords [n,ht,wd,2] f32 (call rows), edge_index [n] int64 or None (row r = edge r); target / weight_out [(1,)E,ht,wd,2] and
+// ba_target / ba_weight [E_ba,2,ht,wd] written in place (row n_inactive + e); eta [n_src,ht,wd] scattered to damping[src_frames];
+// then, when ba_frames is given, ba_damping[r] = .2 * damping[ba_frames[r]] + ep.
+void graph_writeback(torch::Tensor delta, torch::Tensor weight, torch::Tensor coords, c10::optional<torch::Tensor> edge_index,
+                     torch::Tensor target, torch::Tensor weight_out, torch::Tensor ba_target, torch::Tensor ba_weight, int64_t n_inactive,
+                     c10::optional<torch::Tensor> eta, c10::optional<torch::Tensor> src_frames, torch::Tensor damping,
+                     c10::optional<torch::Tensor> ba_frames, c10::optional<torch::Tensor> ba_damping, double ep) {
+  const auto dev = damping.device();
+  CHECK_CUDA(damping);
+  check_rows(damping, "damping", dev, 1, "[n_frames,ht,wd]");
+  TORCH_CHECK(damping.dim() == 3, "damping must be [n_frames,ht,wd]");
+  const int ht = (int)damping.size(1), wd = (int)damping.size(2);
+  const int64_t px2 = (int64_t)ht * wd * 2;
+  for (auto* t : {&delta, &weight, &coords, &target, &weight_out, &ba_target, &ba_weight}) check_rows(*t, "graph_writeback tensor", dev, px2, "[rows,ht,wd,2]");
+  const int n = (int)(delta.numel() / px2);
+  TORCH_CHECK(weight.numel() == delta.numel() && coords.numel() == delta.numel(), "delta, weight and coords must have the same shape");
+  const int64_t E = target.numel() / px2, E_ba = ba_target.numel() / px2;
+  TORCH_CHECK(weight_out.numel() == target.numel() && ba_weight.numel() == ba_target.numel(), "target / weight_out and ba_target / ba_weight shapes differ");
+  TORCH_CHECK(n_inactive >= 0 && n_inactive + E <= E_ba, "ba_target must hold n_inactive + E rows");
+  TORCH_CHECK(edge_index.has_value() && edge_index->defined() ? true : n <= E, "more call rows than graph edges");
+  c10::cuda::CUDAGuard guard(dev);
+  const int64_t* ei = opt_index(edge_index, dev, n, "edge_index");
+  int n_src = 0;
+  const float* eta_p = nullptr;
+  const int64_t* src_p = nullptr;
+  if (eta.has_value() && eta->defined()) {
+    check_rows(*eta, "eta", dev, (int64_t)ht * wd, "[n_src,ht,wd]");
+    n_src = (int)(eta->numel() / ((int64_t)ht * wd));
+    eta_p = eta->data_ptr<float>();
+    src_p = opt_index(src_frames, dev, n_src, "src_frames");
+    TORCH_CHECK(src_p, "src_frames is required with eta");
+  }
+  int n_ba = 0;
+  const int64_t* baf = nullptr;
+  float* bad = nullptr;
+  if (ba_frames.has_value() && ba_frames->defined()) {
+    n_ba = (int)ba_frames->numel();
+    baf = opt_index(ba_frames, dev, n_ba, "ba_frames");
+    TORCH_CHECK(ba_damping.has_value() && ba_damping->defined(), "ba_damping is required with ba_frames");
+    check_rows(*ba_damping, "ba_damping", dev, (int64_t)ht * wd, "[M,ht,wd]");
+    TORCH_CHECK(ba_damping->numel() == (int64_t)n_ba * ht * wd, "ba_damping must be [len(ba_frames),ht,wd]");
+    bad = ba_damping->data_ptr<float>();
+  }
+  check_status(dba_graph_writeback(delta.data_ptr<float>(), weight.data_ptr<float>(), coords.data_ptr<float>(), ei, n, target.data_ptr<float>(),
+                                   weight_out.data_ptr<float>(), ba_target.data_ptr<float>(), ba_weight.data_ptr<float>(), (int)n_inactive, eta_p, src_p,
+                                   n_src, damping.data_ptr<float>(), baf, n_ba, bad, (float)ep, ht, wd, cur_stream()), "graph_writeback");
+}
+
 // extension: the update operator (reference droid_slam/droid_net.py:111-143, modules/gru.py:19-32, droid_net.py:59-75) on the tensor
 // cores.  net [E,128,ht,wd] f16/f32 (or channels-last f16 [E,ht,wd,128] when net_channels_last), inp [E,128,ht,wd], corr [E,196,ht,wd],
 // flow [E,4,ht,wd] f32 or None, seg [E] int64 (torch.unique inverse of the source frames) or None, n_src distinct sources,
@@ -545,6 +633,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "does corr_volume_pyramid (tiled: with tiled=True) have a kernel for f16 [.,dim,ht,wd] feature maps", pybind11::arg("dim"), pybind11::arg("ht"),
         pybind11::arg("wd"), pybind11::arg("tiled") = false);
   m.def("reproject", &reproject, "fused pops.projective_transform(jacobian=False), native extension");
+  m.def("motion_features", &motion_features, "reprojection + FactorGraph motion features in one launch -> [coords, coords_t, motn], native extension",
+        pybind11::arg("poses"), pybind11::arg("disps"), pybind11::arg("intrinsics"), pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("target"),
+        pybind11::arg("edge_index") = pybind11::none());
+  m.def("graph_writeback", &graph_writeback, "update-operator outputs -> factor graph target / weight / damping and BA inputs (in place), native extension",
+        pybind11::arg("delta"), pybind11::arg("weight"), pybind11::arg("coords"), pybind11::arg("edge_index"), pybind11::arg("target"),
+        pybind11::arg("weight_out"), pybind11::arg("ba_target"), pybind11::arg("ba_weight"), pybind11::arg("n_inactive"), pybind11::arg("eta"),
+        pybind11::arg("src_frames"), pybind11::arg("damping"), pybind11::arg("ba_frames") = pybind11::none(),
+        pybind11::arg("ba_damping") = pybind11::none(), pybind11::arg("ep") = 1e-7);
+  m.def("update_workspace_bytes", [](int n_edges, int n_src, int ht, int wd) { return dba_update_workspace_bytes(n_edges, n_src, ht, wd); },
+        "device workspace of one update_forward call (dba_update_workspace_bytes)");
   m.def("update_forward", &update_forward, "update operator (ConvGRU + heads + GraphAgg) on wgmma, native extension");
   m.def("encoder_forward", &encoder_forward, "feature / context encoder (BasicEncoder: fnet norm=1, cnet norm=0) on wgmma -> [n,output_dim,H/8,W/8] f16, native extension",
         pybind11::arg("images"), pybind11::arg("packed_weights"), pybind11::arg("norm"), pybind11::arg("output_dim"));

@@ -151,6 +151,22 @@ __global__ void __launch_bounds__(256) iproj_kernel(const float* __restrict__ po
   p[0] = Xj[0] / Xj[3]; p[1] = Xj[1] / Xj[3]; p[2] = Xj[2] / Xj[3];
 }
 
+// One pixel of the reprojection below: k = pixel index in frame ix, T = the edge transform,
+// returns the coordinates in frame jx and the transformed point's depth z.
+__device__ __forceinline__ float2 reproject_pixel(const float* T, const Intr& Ki, const Intr& Kj, const float* __restrict__ disps, int ix,
+                                                  int k, int hw, int wd, float& z) {
+  const int i = k / wd, j = k - i * wd;
+  float Xi[4] = {((float)j - Ki.cx) / Ki.fx, ((float)i - Ki.cy) / Ki.fy, 1.f, __ldg(disps + (size_t)ix * hw + k)}, Xj[4];
+  act_se3(T, T + 3, Xi, Xj);
+  const float Z = (Xj[2] < 0.5f * 0.2f) ? 1.f : Xj[2];
+  const float d = 1.0f / Z;
+  float2 c;
+  c.x = Kj.fx * (Xj[0] * d) + Kj.cx;
+  c.y = Kj.fy * (Xj[1] * d) + Kj.cy;
+  z = Xj[2];
+  return c;
+}
+
 // Fused reprojection of the update operator's input (replaces the ~10 torch/lietorch launches of
 // pops.projective_transform(..., jacobian=False), reference droid_slam/geom/projective_ops.py:165-198, called through
 // DepthVideo.reproject, depth_video.py:171-179):  coords = proj(G_j G_i^-1 iproj(d_i)), valid = Z > 0.2.
@@ -170,16 +186,84 @@ __global__ void __launch_bounds__(256) reproject_kernel(const float* __restrict_
   const int hw = ht * wd;
   const int k = blockIdx.y * blockDim.x + threadIdx.x;
   if (k >= hw) return;
-  const int i = k / wd, j = k - i * wd;
-  float Xi[4] = {((float)j - Ki.cx) / Ki.fx, ((float)i - Ki.cy) / Ki.fy, 1.f, __ldg(disps + (size_t)ix * hw + k)}, Xj[4];
-  act_se3(T, T + 3, Xi, Xj);
-  const float Z = (Xj[2] < 0.5f * 0.2f) ? 1.f : Xj[2];
-  const float d = 1.0f / Z;
-  float2 c;
-  c.x = Kj.fx * (Xj[0] * d) + Kj.cx;
-  c.y = Kj.fy * (Xj[1] * d) + Kj.cy;
+  float z;
+  const float2 c = reproject_pixel(T, Ki, Kj, disps, ix, k, hw, wd, z);
   reinterpret_cast<float2*>(coords)[(size_t)e * hw + k] = c;
-  valid[(size_t)e * hw + k] = (Xj[2] > 0.2f) ? 1.f : 0.f;
+  valid[(size_t)e * hw + k] = (z > 0.2f) ? 1.f : 0.f;
+}
+
+// torch.clamp(v, -64, 64): NaN stays NaN (fminf / fmaxf would return the bound)
+__device__ __forceinline__ float clamp64(float v) { return v < -64.f ? -64.f : (v > 64.f ? 64.f : v); }
+
+// The motion features of FactorGraph.update / update_lowmem (reference factor_graph.py:220-222, :280-282) in one pass: the
+// reprojection above (same device code, so coords are bit-identical to reproject_kernel's), written in both layouts the corr
+// lookups take, and motn = clamp(cat([coords - grid, target - coords]), +-64) channel-major.  Call row r reads graph edge
+// e = edge_index[r] (identity when edge_index is null): ii[e], jj[e], target[e].
+__global__ void __launch_bounds__(256) motion_features_kernel(const float* __restrict__ poses, const float* __restrict__ disps,
+                                                              const float* __restrict__ intr, const int64_t* __restrict__ ii,
+                                                              const int64_t* __restrict__ jj, const int64_t* __restrict__ edge_index,
+                                                              const float* __restrict__ target, float* __restrict__ coords,
+                                                              float* __restrict__ coords_t, float* __restrict__ motn, int ht, int wd) {
+  const int r = blockIdx.x;
+  const size_t e = edge_index ? (size_t)edge_index[r] : (size_t)r;
+  __shared__ float T[7];
+  const int ix = (int)ii[e], jx = (int)jj[e];
+  if (threadIdx.x == 0) edge_transform(poses, ix, jx, /*stereo_quirk=*/true, T, T + 3);
+  __syncthreads();
+  const Intr Ki = load_intr(intr + 4 * (size_t)ix), Kj = load_intr(intr + 4 * (size_t)jx);
+  const int hw = ht * wd;
+  const int k = blockIdx.y * blockDim.x + threadIdx.x;
+  if (k >= hw) return;
+  float z;
+  const float2 c = reproject_pixel(T, Ki, Kj, disps, ix, k, hw, wd, z);
+  const int i = k / wd, j = k - i * wd;
+  const float2 t = reinterpret_cast<const float2*>(target)[e * hw + k];
+  reinterpret_cast<float2*>(coords)[(size_t)r * hw + k] = c;
+  coords_t[(size_t)r * 2 * hw + k] = c.x;
+  coords_t[((size_t)r * 2 + 1) * hw + k] = c.y;
+  float* m = motn + (size_t)r * 4 * hw + k;
+  m[0] = clamp64(__fsub_rn(c.x, (float)j));
+  m[hw] = clamp64(__fsub_rn(c.y, (float)i));
+  m[2 * hw] = clamp64(__fsub_rn(t.x, c.x));
+  m[3 * hw] = clamp64(__fsub_rn(t.y, c.y));
+}
+
+// Write-back of one update-operator call into the factor graph (reference factor_graph.py:234-238, :304-307):
+// rows r < n: target = coords + delta, weight, at graph edge e = edge_index[r] of the graph's [E,ht,wd,2] tensors and at row
+// n_inactive + e of BA's channel-major [E_ba,2,ht,wd] inputs; rows n + m: damping[src_frames[m]] = eta[m].
+__global__ void __launch_bounds__(256) graph_writeback_kernel(const float* __restrict__ delta, const float* __restrict__ weight,
+                                                              const float* __restrict__ coords, const int64_t* __restrict__ edge_index, int n,
+                                                              float* __restrict__ g_target, float* __restrict__ g_weight,
+                                                              float* __restrict__ ba_target, float* __restrict__ ba_weight, int n_inactive,
+                                                              const float* __restrict__ eta, const int64_t* __restrict__ src_frames,
+                                                              float* __restrict__ damping, int hw) {
+  const int r = blockIdx.x;
+  const int k = blockIdx.y * blockDim.x + threadIdx.x;
+  if (k >= hw) return;
+  if (r >= n) {
+    const int m = r - n;
+    damping[(size_t)src_frames[m] * hw + k] = eta[(size_t)m * hw + k];
+    return;
+  }
+  const size_t e = edge_index ? (size_t)edge_index[r] : (size_t)r;
+  const float2 c = reinterpret_cast<const float2*>(coords)[(size_t)r * hw + k];
+  const float2 d = reinterpret_cast<const float2*>(delta)[(size_t)r * hw + k];
+  const float2 w = reinterpret_cast<const float2*>(weight)[(size_t)r * hw + k];
+  const float2 t = make_float2(__fadd_rn(c.x, d.x), __fadd_rn(c.y, d.y));
+  reinterpret_cast<float2*>(g_target)[e * hw + k] = t;
+  reinterpret_cast<float2*>(g_weight)[e * hw + k] = w;
+  const size_t b = (size_t)n_inactive + e;
+  ba_target[b * 2 * hw + k] = t.x; ba_target[(b * 2 + 1) * hw + k] = t.y;
+  ba_weight[b * 2 * hw + k] = w.x; ba_weight[(b * 2 + 1) * hw + k] = w.y;
+}
+
+// BA's damping input: out[r] = .2 * damping[frames[r]] + ep with the reference's two roundings (factor_graph.py:251, :320)
+__global__ void __launch_bounds__(256) damping_gather_kernel(const float* __restrict__ damping, const int64_t* __restrict__ frames,
+                                                             float* __restrict__ out, float ep, int hw) {
+  const int r = blockIdx.x;
+  const int k = blockIdx.y * blockDim.x + threadIdx.x;
+  if (k >= hw) return;
+  out[(size_t)r * hw + k] = __fadd_rn(__fmul_rn(damping[(size_t)frames[r] * hw + k], 0.2f), ep);
 }
 
 }  // namespace dba
@@ -194,6 +278,46 @@ extern "C" int dba_reproject(const float* poses, const float* disps, const float
   dim3 grid(n_edges, (ht * wd + 255) / 256);
   reproject_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics_per_frame, ii, jj, coords, valid, ht, wd);
   DBA_CHECK_LAUNCH("reproject");
+  return DBA_OK;
+}
+
+extern "C" int dba_motion_features(const float* poses, const float* disps, const float* intrinsics_per_frame, const int64_t* ii,
+                                   const int64_t* jj, const int64_t* edge_index, const float* target, float* coords, float* coords_t,
+                                   float* motn, int n_rows, int ht, int wd, dba_stream_t stream) {
+  DBA_CHECK_ARG(n_rows >= 0 && ht >= 0 && wd >= 0, "negative extent");
+  if (n_rows == 0 || ht * wd == 0) return DBA_OK;
+  DBA_CHECK_ARG(poses && disps && intrinsics_per_frame && ii && jj && target && coords && coords_t && motn, "null pointer");
+  DBA_CHECK_ARG((ht * wd + 255) / 256 <= 65535, "image too large");
+  dim3 grid(n_rows, (ht * wd + 255) / 256);
+  motion_features_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics_per_frame, ii, jj, edge_index, target, coords,
+                                                                 coords_t, motn, ht, wd);
+  DBA_CHECK_LAUNCH("motion_features");
+  return DBA_OK;
+}
+
+extern "C" int dba_graph_writeback(const float* delta, const float* weight, const float* coords, const int64_t* edge_index, int n_rows,
+                                   float* target, float* weight_out, float* ba_target, float* ba_weight, int n_inactive,
+                                   const float* eta, const int64_t* src_frames, int n_src, float* damping,
+                                   const int64_t* ba_frames, int n_ba_frames, float* ba_damping, float ep, int ht, int wd,
+                                   dba_stream_t stream) {
+  DBA_CHECK_ARG(n_rows >= 0 && n_inactive >= 0 && n_src >= 0 && n_ba_frames >= 0 && ht >= 0 && wd >= 0, "negative extent");
+  const int hw = ht * wd;
+  if (hw == 0) return DBA_OK;
+  DBA_CHECK_ARG((hw + 255) / 256 <= 65535, "image too large");
+  DBA_CHECK_ARG(n_rows == 0 || (delta && weight && coords && target && weight_out && ba_target && ba_weight), "null pointer");
+  DBA_CHECK_ARG(n_src == 0 || (eta && src_frames && damping), "null pointer");
+  DBA_CHECK_ARG(n_ba_frames == 0 || (damping && ba_frames && ba_damping), "null pointer");
+  if (n_rows + n_src > 0) {
+    dim3 grid(n_rows + n_src, (hw + 255) / 256);
+    graph_writeback_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(delta, weight, coords, edge_index, n_rows, target, weight_out, ba_target,
+                                                                   ba_weight, n_inactive, eta, src_frames, damping, hw);
+    DBA_CHECK_LAUNCH("graph_writeback");
+  }
+  if (n_ba_frames > 0) {
+    dim3 grid(n_ba_frames, (hw + 255) / 256);
+    damping_gather_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(damping, ba_frames, ba_damping, ep, hw);
+    DBA_CHECK_LAUNCH("graph_writeback (damping gather)");
+  }
   return DBA_OK;
 }
 

@@ -17,12 +17,20 @@ kernel for is offered as a hook:
   * `reproject(...)`: `DepthVideo.reproject` (depth_video.py:171-179 -> geom/projective_ops.py:165-198) as one kernel.
   * `add_proximity_factors(graph, ...)` / `install_proximity_hook(FactorGraph)`: the edge selection of
     `FactorGraph.add_proximity_factors` (factor_graph.py:346-412) on the device (row F1).
+  * `update(graph, ...)` / `update_lowmem(graph, ...)` / `install_factor_graph_hook(FactorGraph)`: the glue of `FactorGraph.update` and
+    `update_lowmem` (factor_graph.py:214-330) planned with one host read per call, every step without a host synchronisation: fused
+    motion features (`droid_backends.motion_features`), the update operator on whole source frames, the write-back of its outputs
+    into the graph and BA's inputs (`droid_backends.graph_writeback`).
+  * `install_depth_video_hook(DepthVideo)`: `DepthVideo.reproject` / `DepthVideo.upsample` on `reproject` / `upsample` below.
 """
+import sys
+
 import torch
 
 from . import install
 
-__all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook"]
+__all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
+           "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks"]
 
 
 def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
@@ -251,4 +259,260 @@ def add_proximity_factors(graph, t0=0, t1=0, rad=2, nms=2, beta=0.25, thresh=16.
 def install_proximity_hook(factor_graph_class):
     """replace `add_proximity_factors` of the reference's FactorGraph class (factor_graph.py:346) by the device version"""
     factor_graph_class.add_proximity_factors = add_proximity_factors
+    return factor_graph_class
+
+
+def install_depth_video_hook(depth_video_class):
+    """replace `DepthVideo.reproject` (depth_video.py:171-179) and `DepthVideo.upsample` (:155-159) by `reproject` / `upsample` above, so
+    that `FactorGraph.add_factors` takes its initial targets from the kernel the update hooks reproject with"""
+    def _reproject(self, ii, jj):
+        return reproject(self.poses, self.disps, self.intrinsics, ii, jj)
+
+    def _upsample(self, ix, mask):
+        upsample(self.disps, self.disps_up, ix, mask)
+
+    depth_video_class.reproject = _reproject
+    depth_video_class.upsample = _upsample
+    return depth_video_class
+
+
+# ---- FactorGraph.update / update_lowmem ----------------------------------------------------------------------------------------------
+
+_LOWMEM_CHUNK_FRAMES = 8      # the reference's chunk of source frames (factor_graph.py:284); decides which edges a step updates
+
+
+def _factor_graph_unsupported(graph):
+    """why the update hooks cannot run this graph natively (None: they can)"""
+    from .update import UpdateModule
+    if not isinstance(graph.update_op, UpdateModule):
+        return "graph.update_op is %s, not droid_slam_b200.update.UpdateModule" % type(graph.update_op).__name__
+    video = graph.video
+    for name, t in (("graph.ii", graph.ii), ("graph.net", graph.net), ("graph.target", graph.target), ("graph.damping", graph.damping),
+                    ("video.poses", video.poses), ("video.disps", video.disps), ("video.intrinsics", video.intrinsics)):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda):
+            return "%s is not a CUDA tensor" % name
+    if graph.ii.numel() == 0:
+        return "the graph has no edges"
+    return None
+
+
+def _check_native(graph):
+    why = _factor_graph_unsupported(graph)
+    if why is not None:
+        raise RuntimeError("the native FactorGraph update cannot run this graph: %s" % why)
+
+
+def _to_device(dev, arrays):
+    """several CPU int64 tensors -> device views, in one pinned, non-blocking copy (no host synchronisation)"""
+    sizes = [a.numel() for a in arrays]
+    flat = torch.cat([a.reshape(-1).long() for a in arrays]).pin_memory().to(dev, non_blocking=True)
+    return list(torch.split(flat, sizes))
+
+
+def _segments(ii):
+    """ascending distinct source frames of ii and each edge's rank among them (GraphAgg's torch.unique, droid_net.py:61)"""
+    return torch.unique(ii, return_inverse=True)
+
+
+def _corr_features(be, corr, coords, coords_t, ii=None, jj=None):
+    """the graph's corr block looked up at coords [n,ht,wd,2] (coords_t: the same as [n,2,ht,wd]) -> [1,n,196,ht,wd].  A native block
+    (CorrBlock under install_corr_volume_hook, AltCorrBlock under install_alt_corr_hook) goes straight to its one-launch lookup on
+    coords_t; any other block is called through its own __call__."""
+    n, ht, wd, _ = coords.shape
+    if ii is None:
+        if getattr(corr, "_b200_native", False):
+            pyr = [v.contiguous() for v in corr.corr_pyramid]
+            return be.corr_lookup_pyramid(pyr, coords_t, corr._b200_tiled).view(1, n, -1, ht, wd)
+        return corr(coords[None])
+    pyramid = getattr(corr, "_b200_pyramid", None)
+    if pyramid is not None:
+        return be.altcorr_lookup_pyramid(pyramid, coords_t[None], ii, jj, corr.radius)
+    return corr(coords[None], ii, jj)
+
+
+def update(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
+    """FactorGraph.update (reference factor_graph.py:214-263) with the same signature and effects, `graph` being the reference's FactorGraph
+    (or an object with its attributes).  One host read plans the call (t0, the inactive edges BA uses, the source frames, BA's window);
+    the motion features are one launch, the update operator one call without torch.unique, the write-back of target / weight / damping
+    and BA's inputs one launch; then `video.ba` and `video.upsample` as in the reference.  Raises when the graph cannot run natively."""
+    _check_native(graph)
+    be = install()
+    video = graph.video
+    dev = graph.ii.device
+    ht, wd = graph.coords0.shape[:2]
+    E = graph.ii.numel()
+    n_inac_all = graph.ii_inac.numel() if use_inactive else 0
+    host = torch.cat([graph.ii, graph.jj] + ([graph.ii_inac, graph.jj_inac] if use_inactive else [])).long().cpu()   # the one host read
+    ii, jj = host[:E], host[E:2 * E]
+    if t0 is None:
+        t0 = max(1, int(ii.min()) + 1)
+    inac = torch.zeros(0, dtype=torch.long)
+    if use_inactive:
+        ii_inac, jj_inac = host[2 * E:2 * E + n_inac_all], host[2 * E + n_inac_all:]
+        inac = torch.nonzero((ii_inac >= t0 - 3) & (jj_inac >= t0 - 3))[:, 0]
+        ii_ba, jj_ba = torch.cat([ii_inac[inac], ii]), torch.cat([jj_inac[inac], jj])
+    else:
+        ii_ba, jj_ba = ii, jj
+    if t1 is None:                               # what DepthVideo.ba computes with a host read of its own
+        t1 = max(int(ii_ba.max()), int(jj_ba.max())) + 1
+    src, seg = _segments(ii)
+    seg_d, src_d, ba_frames_d, inac_d, ii_ba_d, jj_ba_d = _to_device(dev, [seg, src, torch.unique(ii_ba), inac, ii_ba, jj_ba])
+    n_inac = inac.numel()
+
+    with torch.autocast("cuda", enabled=False):
+        coords, coords_t, motn = be.motion_features(video.poses, video.disps, video.intrinsics, graph.ii, graph.jj, graph.target)
+        with torch.autocast("cuda", enabled=True):
+            corr = _corr_features(be, graph.corr, coords, coords_t)
+        graph.net, delta, weight, eta, upmask = graph.update_op.forward_segments(graph.net, graph.inp, corr, motn[None], seg_d, src.numel())
+        target, weight_out = torch.empty_like(graph.target), torch.empty_like(graph.target)
+        ba_target = torch.empty(n_inac + E, 2, ht, wd, device=dev)
+        ba_weight = torch.empty_like(ba_target)
+        if n_inac:
+            ba_target[:n_inac] = graph.target_inac[0, inac_d].permute(0, 3, 1, 2)
+            ba_weight[:n_inac] = graph.weight_inac[0, inac_d].permute(0, 3, 1, 2)
+        damping = torch.empty(ba_frames_d.numel(), ht, wd, device=dev)
+        be.graph_writeback(delta.reshape(E, ht, wd, 2), weight.reshape(E, ht, wd, 2), coords, None, target, weight_out, ba_target, ba_weight,
+                           n_inac, eta[0], src_d, graph.damping, ba_frames_d, damping, EP)
+        graph.target, graph.weight = target, weight_out
+        video.ba(ba_target, ba_weight, damping, ii_ba_d, jj_ba_d, t0, t1, itrs=itrs, lm=1e-4, ep=0.1, motion_only=motion_only)
+        if graph.upsample:
+            video.upsample(src_d, upmask)
+    graph.age += 1
+
+
+def _lowmem_edge_budget(be, ht, wd, device):
+    """the most edges one update-operator call of update_lowmem takes: a quarter of the free device memory over what one edge needs
+    (its share of the operator's workspace with every edge its own source frame, its corr features and the operator's outputs)"""
+    hw = ht * wd
+    per_edge = -(-be.update_workspace_bytes(64, 64, ht, wd) // 64) + hw * (196 * 2 + 128 * 2 + 2 * 2 * 4 + 4 + 576 * 2)
+    free, _ = torch.cuda.mem_get_info(device)
+    return max(1, (free // 4) // per_edge)
+
+
+def plan_lowmem_chunks(ii, jj, max_edges):
+    """Plan of one update_lowmem step over the graph edges ii, jj (CPU int64).
+
+    The edges the reference updates are those whose source frame falls in one of its chunks range(ii.min(), jj.max() + 1, 8) of 8 source
+    frames.  They are cut into chunks of whole source frames (ascending) holding at most max_edges edges, except a single source frame
+    with more edges, which is a chunk of its own.  GraphAgg averages over the edges of one source frame only, so any such cut computes
+    what the reference's chunks compute.
+    Returns (perm, chunks, src, seg): perm [n] graph edge ids in call order (chunk by chunk, graph order inside a chunk); chunks a list of
+    (row_lo, row_hi, src_lo, src_hi); src the ascending source frames of each chunk, concatenated; seg [n] each row's rank among its
+    chunk's source frames."""
+    ii, jj = ii.long(), jj.long()
+    first = int(ii.min())
+    n_ref = len(range(first, int(jj.max()) + 1, _LOWMEM_CHUNK_FRAMES))
+    covered = ii < first + _LOWMEM_CHUNK_FRAMES * n_ref
+    frames, counts = torch.unique(ii[covered], return_counts=True)
+    chunk_of_frame, frame_lo, acc = [], [], 0
+    for k, c in enumerate(counts.tolist()):
+        if not frame_lo or (acc > 0 and acc + c > max_edges):
+            frame_lo.append(k)
+            acc = 0
+        chunk_of_frame.append(len(frame_lo) - 1)
+        acc += c
+    edges = torch.nonzero(covered)[:, 0]
+    pos = torch.searchsorted(frames, ii[edges])
+    key = torch.as_tensor(chunk_of_frame, dtype=torch.long)[pos] if edges.numel() else pos
+    order = torch.sort(key, stable=True).indices
+    perm, key, pos = edges[order], key[order], pos[order]
+    seg = pos - torch.as_tensor(frame_lo, dtype=torch.long)[key] if edges.numel() else pos
+    chunks, row = [], 0
+    frame_hi = frame_lo[1:] + [frames.numel()]
+    for lo, hi in zip(frame_lo, frame_hi):
+        n = int(counts[lo:hi].sum())
+        chunks.append((row, row + n, lo, hi))
+        row += n
+    return perm, chunks, frames, seg
+
+
+def _alt_corr_class(graph):
+    """the AltCorrBlock the graph's module imported (the reference's factor_graph.py: `from modules.corr import CorrBlock, AltCorrBlock`);
+    under install_alt_corr_hook it is the native block"""
+    return sys.modules[type(graph).__module__].AltCorrBlock
+
+
+def update_lowmem(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, steps=8):
+    """FactorGraph.update_lowmem (reference factor_graph.py:266-330) with the same signature and effects.  One host read per call plans
+    every step: the edges the reference's 8-frame chunks cover, cut into chunks of whole source frames sized to the free device memory,
+    and BA's frame list.  The context features, the graph's net in call order and BA's inputs for the edges the operator does not touch
+    are gathered once per call.  Each step: one motion_features launch, per chunk the corr lookup, the update operator and
+    graph_writeback, then video.upsample (when graph.upsample) and video.ba -- no host synchronisation.  graph.net is scattered back into
+    graph order at the end of the call.  Raises when the graph cannot run natively."""
+    _check_native(graph)
+    be = install()
+    video = graph.video
+    dev = graph.ii.device
+    t = video.counter.value
+    num, rig, ch, ht, wd = video.fmaps.shape
+    E = graph.ii.numel()
+    n_inac = graph.ii_inac.numel() if use_inactive else 0
+    host = torch.cat([graph.ii, graph.jj] + ([graph.ii_inac] if use_inactive else [])).long().cpu()     # the one host read
+    ii, jj = host[:E], host[E:2 * E]
+    ii_ba = torch.cat([host[2 * E:], ii])
+    perm, chunks, src, seg = plan_lowmem_chunks(ii, jj, _lowmem_edge_budget(be, ht, wd, dev))
+    ip, jp = ii[perm], jj[perm]
+    perm_d, seg_d, src_d, ii_alt_d, jj_alt_d, ba_frames_d = _to_device(
+        dev, [perm, seg, src, rig * ip, rig * jp + (ip == jp).long(), torch.unique(ii_ba)])
+
+    with torch.autocast("cuda", enabled=False):
+        corr_op = _alt_corr_class(graph)(video.fmaps.view(1, num * rig, ch, ht, wd))
+        inp = video.inps[graph.ii[perm_d]]
+        if graph.net.dtype == torch.float16:     # channels-last: the update operator reads it without a layout change
+            net = torch.empty(perm.numel(), ht, wd, graph.net.shape[2], dtype=graph.net.dtype, device=dev).permute(0, 3, 1, 2)
+        else:
+            net = torch.empty(perm.numel(), *graph.net.shape[2:], dtype=graph.net.dtype, device=dev)
+        net.copy_(graph.net[0, perm_d])
+        if use_inactive:
+            ii_ba_d, jj_ba_d = torch.cat([graph.ii_inac, graph.ii]), torch.cat([graph.jj_inac, graph.jj])
+            ba_target = torch.cat([graph.target_inac[0], graph.target[0]]).permute(0, 3, 1, 2).contiguous()
+            ba_weight = torch.cat([graph.weight_inac[0], graph.weight[0]]).permute(0, 3, 1, 2).contiguous()
+        else:
+            ii_ba_d, jj_ba_d = graph.ii, graph.jj
+            ba_target = graph.target[0].permute(0, 3, 1, 2).contiguous()
+            ba_weight = graph.weight[0].permute(0, 3, 1, 2).contiguous()
+        damping = torch.empty(ba_frames_d.numel(), ht, wd, device=dev)
+        no_rows = torch.empty(0, ht, wd, 2, device=dev)
+
+        for _ in range(steps):
+            if chunks:
+                coords, coords_t, motn = be.motion_features(video.poses, video.disps, video.intrinsics, graph.ii, graph.jj, graph.target, perm_d)
+            for c, (a, b, s0, s1) in enumerate(chunks):
+                with torch.autocast("cuda", enabled=True):
+                    corr = _corr_features(be, corr_op, coords[a:b], coords_t[a:b], ii_alt_d[a:b], jj_alt_d[a:b])
+                    net_new, delta, weight, eta, upmask = graph.update_op.forward_segments(net[a:b][None], inp[a:b][None], corr, motn[a:b][None],
+                                                                                          seg_d[a:b], s1 - s0)
+                    if graph.upsample:
+                        video.upsample(src_d[s0:s1], upmask)
+                net[a:b] = net_new[0]
+                last = c == len(chunks) - 1
+                be.graph_writeback(delta[0], weight[0], coords[a:b], perm_d[a:b], graph.target, graph.weight, ba_target, ba_weight, n_inac,
+                                   eta[0], src_d[s0:s1], graph.damping, ba_frames_d if last else None, damping if last else None, EP)
+            if not chunks:                       # no edge in the reference's chunks: BA's damping still has to be gathered
+                be.graph_writeback(no_rows, no_rows, no_rows, None, graph.target, graph.weight, ba_target, ba_weight, n_inac,
+                                   None, None, graph.damping, ba_frames_d, damping, EP)
+            graph.age += 1
+            video.ba(ba_target, ba_weight, damping, ii_ba_d, jj_ba_d, 1, t, itrs=itrs, lm=1e-5, ep=1e-2, motion_only=False)
+            video.dirty[:t] = True
+        graph.net[0, perm_d] = net
+
+
+def install_factor_graph_hook(factor_graph_class, strict=True):
+    """replace `update` and `update_lowmem` of the reference's FactorGraph class (factor_graph.py:214, :266) by the native versions above.
+    strict: a graph they cannot run (update_op not droid_slam_b200.update.UpdateModule, tensors not on CUDA, no edges) raises, naming the
+    reason; with strict=False the reference's own method runs for it."""
+    ref_update, ref_lowmem = factor_graph_class.update, factor_graph_class.update_lowmem
+
+    def _update(self, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
+        if not strict and _factor_graph_unsupported(self) is not None:
+            return ref_update(self, t0, t1, itrs, use_inactive, EP, motion_only)
+        return update(self, t0, t1, itrs, use_inactive, EP, motion_only)
+
+    def _update_lowmem(self, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, steps=8):
+        if not strict and _factor_graph_unsupported(self) is not None:
+            return ref_lowmem(self, t0, t1, itrs, use_inactive, EP, steps)
+        return update_lowmem(self, t0, t1, itrs, use_inactive, EP, steps)
+
+    factor_graph_class.update = _update
+    factor_graph_class.update_lowmem = _update_lowmem
     return factor_graph_class

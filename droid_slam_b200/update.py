@@ -135,6 +135,18 @@ class UpdateModule(nn.Module):
     def forward(self, net, inp, corr, flow=None, ii=None, jj=None):
         if not net.is_cuda:
             raise RuntimeError("droid_slam_b200.UpdateModule runs on CUDA tensors only (hand-written sm_90a kernels, no CPU path)")
+        batch = net.shape[0]
+        seg, n_src = None, 0
+        if ii is not None:
+            uniq, seg = torch.unique(ii.to(net.device), return_inverse=True)                # like GraphAgg.forward, droid_net.py:61
+            if batch > 1:
+                seg = (seg[None] + uniq.numel() * torch.arange(batch, device=seg.device)[:, None]).reshape(-1)
+            n_src = int(uniq.numel()) * batch
+        return self.forward_segments(net, inp, corr, flow, seg, n_src)
+
+    def forward_segments(self, net, inp, corr, flow, seg, n_src):
+        """forward() with GraphAgg's segments given instead of ii: seg [B*E] int64 on the device = rank of each edge's source frame
+        among the distinct ones (batch b's ranks offset by b * M), n_src = B * M; seg None: no aggregation (net, delta, weight only)."""
         from . import install
         be = install()
         batch, num, ch, ht, wd = net.shape
@@ -146,17 +158,11 @@ class UpdateModule(nn.Module):
         inp_arg = inp.reshape(E, -1, ht, wd).contiguous()
         corr_arg = corr.reshape(E, -1, ht, wd).contiguous()
         flow_arg = None if flow is None else flow.reshape(E, -1, ht, wd)
-        seg, n_src = None, 0
-        if ii is not None:
-            uniq, seg = torch.unique(ii.to(net.device), return_inverse=True)                # like GraphAgg.forward, droid_net.py:61
-            if batch > 1:
-                seg = (seg[None] + uniq.numel() * torch.arange(batch, device=seg.device)[:, None]).reshape(-1)
-            n_src = int(uniq.numel()) * batch
         out = be.update_forward(net_arg, inp_arg, corr_arg, flow_arg, seg, n_src, self.packed_weights(net.device), cl)
         net_new = out[0].view(batch, num, ht, wd, 128).permute(0, 1, 4, 2, 3)
         delta = out[1].view(batch, num, ht, wd, 2)
         weight = out[2].view(batch, num, ht, wd, 2)
-        if ii is None:
+        if seg is None:
             return net_new, delta, weight
         eta = out[3].view(batch, -1, ht, wd)
         upmask = out[4].view(batch, -1, 8 * 8 * 9, ht, wd)

@@ -138,6 +138,26 @@ int dba_projmap(const float* poses, const float* disps, const float* intrinsics,
  * intrinsics_per_frame [n_frames,4]; coords [E,ht,wd,2], valid [E,ht,wd,1]; MIN_DEPTH 0.2, stereo baseline for ii == jj. */
 int dba_reproject(const float* poses, const float* disps, const float* intrinsics_per_frame,
                   const int64_t* ii, const int64_t* jj, float* coords, float* valid, int n_edges, int ht, int wd, dba_stream_t stream);
+
+/* ---- factor-graph step (FactorGraph.update / update_lowmem, reference droid_slam/factor_graph.py:214-330) -----------------
+ * Call row r stands for graph edge e = edge_index[r] (edge_index null: e = r); indices are not range-checked.
+ * dba_motion_features: the reprojection of dba_reproject (same device code, bit-identical coords) of edge (ii[e], jj[e]) fused with the
+ * motion features (:220-222, :280-282).  target [E,ht,wd,2] (the graph's); outputs per call row: coords [n,ht,wd,2],
+ * coords_t [n,2,ht,wd] (the layout dba_corr_lookup_pyramid / dba_altcorr_lookup_pyramid take), motn [n,4,ht,wd] =
+ * clamp(coords - (x,y), +-64), clamp(target - coords, +-64) in fp32; NaN stays NaN like torch.clamp. */
+int dba_motion_features(const float* poses, const float* disps, const float* intrinsics_per_frame, const int64_t* ii, const int64_t* jj,
+                        const int64_t* edge_index, const float* target, float* coords, float* coords_t, float* motn,
+                        int n_rows, int ht, int wd, dba_stream_t stream);
+/* dba_graph_writeback: the update operator's delta / weight [n,ht,wd,2] for call rows whose coordinates are coords [n,ht,wd,2] go back
+ * to the graph: target[e] = coords + delta and weight_out[e] = weight ([E,ht,wd,2]), and the same values to BA's channel-major inputs
+ * ba_target / ba_weight [E_ba,2,ht,wd] at row n_inactive + e (inactive edges first, then graph order, as the reference concatenates).
+ * damping [n_frames,ht,wd]: damping[src_frames[m]] = eta[m] for m < n_src (eta [n_src,ht,wd]).  Then, if n_ba_frames > 0 (after that
+ * scatter, stream-ordered): ba_damping[r] = .2f * damping[ba_frames[r]] + ep, two roundings (:251, :320). */
+int dba_graph_writeback(const float* delta, const float* weight, const float* coords, const int64_t* edge_index, int n_rows,
+                        float* target, float* weight_out, float* ba_target, float* ba_weight, int n_inactive,
+                        const float* eta, const int64_t* src_frames, int n_src, float* damping,
+                        const int64_t* ba_frames, int n_ba_frames, float* ba_damping, float ep, int ht, int wd, dba_stream_t stream);
+
 int dba_frame_distance(const float* poses, const float* disps, const float* intrinsics,
                        const int64_t* ii, const int64_t* jj, float* dist /*[K]*/,
                        int n_pairs, int ht, int wd, float beta, dba_stream_t stream);
