@@ -5,9 +5,9 @@ import os
 _LIB = None
 
 SYMBOLS = [
-    "dba_last_error", "dba_version", "dba_set_l2_fetch_granularity", "dba_get_l2_fetch_granularity",
-    "dba_corr_index_forward", "dba_corr_index_backward", "dba_corr_volume_pyramid", "dba_corr_volume_pyramid_tiled", "dba_corr_lookup_pyramid", "dba_corr_volume_supported",
-    "dba_corr_volume_tiled_supported", "dba_corr_volume_workspace_bytes", "dba_corr_volume_pyramid_ws", "dba_altcorr_forward", "dba_altcorr_backward",
+    "dba_last_error", "dba_version",
+    "dba_corr_index_forward", "dba_corr_index_backward", "dba_corr_volume_pyramid", "dba_corr_lookup_pyramid", "dba_corr_volume_supported",
+    "dba_corr_volume_workspace_bytes", "dba_altcorr_forward", "dba_altcorr_backward",
     "dba_altcorr_pyramid", "dba_altcorr_lookup_pyramid",
     "dba_projmap", "dba_reproject", "dba_motion_features", "dba_graph_writeback", "dba_cvx_upsample", "dba_frame_distance", "dba_depth_filter", "dba_iproj",
     "dba_ba_workspace_bytes", "dba_ba_system_offset", "dba_ba_system_bytes",
@@ -57,14 +57,11 @@ def load():
     vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
     L.dba_corr_index_forward.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]
     L.dba_corr_index_backward.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]
-    L.dba_corr_volume_pyramid.argtypes = [vp] * 8 + [ci] * 7 + [vp]
-    L.dba_corr_volume_pyramid_tiled.argtypes = [vp] * 8 + [ci] * 7 + [vp]
+    L.dba_corr_volume_pyramid.argtypes = [vp] * 8 + [ci] * 8 + [vp, ctypes.c_size_t, vp]
     L.dba_corr_lookup_pyramid.argtypes = [vp] * 6 + [ci] * 5 + [vp]
-    L.dba_corr_volume_supported.argtypes = [ci] * 4
-    L.dba_corr_volume_tiled_supported.argtypes = [ci] * 4
+    L.dba_corr_volume_supported.argtypes = [ci] * 5
     L.dba_corr_volume_workspace_bytes.restype = ctypes.c_size_t
     L.dba_corr_volume_workspace_bytes.argtypes = [ci] * 5
-    L.dba_corr_volume_pyramid_ws.argtypes = [vp] * 8 + [ci] * 7 + [vp, ctypes.c_size_t, vp]
     L.dba_altcorr_forward.argtypes = [vp, vp, vp, vp, vp, vp] + [ci] * 11 + [vp]
     L.dba_altcorr_backward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp] + [ci] * 11 + [vp]
     L.dba_altcorr_pyramid.argtypes = [vp] * 5 + [ci] * 7 + [vp]

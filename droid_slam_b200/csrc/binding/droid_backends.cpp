@@ -247,8 +247,8 @@ std::vector<torch::Tensor> altcorr_backward(torch::Tensor fmap1, torch::Tensor f
 
 // extension beyond the reference's nine callables: CorrBlock.__init__ in one tensor-core kernel
 // (reference droid_slam/modules/corr.py:24-38,63-71).  fmap1/fmap2 [N,128,ht,wd] f16 (ht, wd >= 8), ii/jj [E] -> 4 pyramid levels.
-// tiled (levels 0-1 in the private tiled layout) only where dba_corr_volume_tiled_supported; wd % 8 != 0 takes a staging workspace
-// from the caching allocator.
+// tiled (levels 0-1 in the private tiled layout) only where dba_corr_volume_supported(..., tiled = 1); wd % 8 != 0 takes a staging
+// workspace from the caching allocator.
 std::vector<torch::Tensor> corr_volume_pyramid(torch::Tensor fmap1, torch::Tensor fmap2, torch::Tensor ii, torch::Tensor jj, bool tiled) {
   CHECK_INPUT(fmap1); CHECK_INPUT(fmap2); CHECK_INPUT(ii); CHECK_INPUT(jj); CHECK_I64(ii); CHECK_I64(jj);
   TORCH_CHECK(fmap1.dim() == 4 && fmap2.dim() == 4, "fmaps must be [N,C,ht,wd]");
@@ -260,18 +260,12 @@ std::vector<torch::Tensor> corr_volume_pyramid(torch::Tensor fmap1, torch::Tenso
   std::vector<torch::Tensor> out;
   for (int l = 0; l < 4; l++) out.push_back(torch::empty({E, ht, wd, ht >> l, wd >> l}, fmap1.options()));
   const int n1 = (int)fmap1.size(0), n2 = (int)fmap2.size(0);
-  if (tiled) {
-    check_status(dba_corr_volume_pyramid_tiled(fmap1.data_ptr(), fmap2.data_ptr(), ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), out[0].data_ptr(),
-                                               out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), E, n1, n2, C, ht, wd, DBA_F16, cur_stream()),
-                 "corr_volume_pyramid");
-    return out;
-  }
   const size_t ws_bytes = dba_corr_volume_workspace_bytes(n1, n2, C, ht, wd);
   torch::Tensor ws;
   if (ws_bytes > 0 && E > 0) ws = torch::empty({(int64_t)ws_bytes}, fmap1.options().dtype(torch::kUInt8));
-  check_status(dba_corr_volume_pyramid_ws(fmap1.data_ptr(), fmap2.data_ptr(), ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), out[0].data_ptr(),
-                                          out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), E, n1, n2, C, ht, wd, DBA_F16,
-                                          ws.defined() ? ws.data_ptr() : nullptr, ws.defined() ? ws_bytes : 0, cur_stream()),
+  check_status(dba_corr_volume_pyramid(fmap1.data_ptr(), fmap2.data_ptr(), ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), out[0].data_ptr(),
+                                       out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), E, n1, n2, C, ht, wd, DBA_F16, tiled ? 1 : 0,
+                                       ws.defined() ? ws.data_ptr() : nullptr, ws.defined() ? ws_bytes : 0, cur_stream()),
                "corr_volume_pyramid");
   return out;
 }
@@ -629,7 +623,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("fmaps"), pybind11::arg("num_levels") = 4);
   m.def("altcorr_lookup_pyramid", &altcorr_lookup_pyramid, "AltCorrBlock lookup over all levels in one launch -> [B,M,L*49,H,W], native extension",
         pybind11::arg("pyramid"), pybind11::arg("coords"), pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("radius") = 3);
-  m.def("corr_volume_supported", [](int dim, int ht, int wd, bool tiled) { return (tiled ? dba_corr_volume_tiled_supported : dba_corr_volume_supported)(dim, ht, wd, DBA_F16) != 0; },
+  m.def("corr_volume_supported", [](int dim, int ht, int wd, bool tiled) { return dba_corr_volume_supported(dim, ht, wd, DBA_F16, tiled ? 1 : 0) != 0; },
         "does corr_volume_pyramid (tiled: with tiled=True) have a kernel for f16 [.,dim,ht,wd] feature maps", pybind11::arg("dim"), pybind11::arg("ht"),
         pybind11::arg("wd"), pybind11::arg("tiled") = false);
   m.def("reproject", &reproject, "fused pops.projective_transform(jacobian=False), native extension");

@@ -4,7 +4,6 @@
 #pragma once
 #include "common.cuh"
 #include "wgmma.cuh"
-#include <cuda.h>
 #include <string.h>
 
 namespace dba {
@@ -41,20 +40,8 @@ struct ConvParams {
   float* counts;
 };
 
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_w(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
 __device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  const __half2 t = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&t);
-}
 __device__ __forceinline__ float2 unpack2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
 
 __device__ __forceinline__ float2 ldh2(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
@@ -90,7 +77,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
       float v0 = acc[4 * j + 2 * i] + __ldg(bias + c), v1 = acc[4 * j + 2 * i + 1] + __ldg(bias + c + 1);
       if (EPI == EPI_STORE) {
         if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + nt * p.N + c) = pack2(v0, v1);
+        if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + nt * p.N + c) = pack_h2(v0, v1);
       } else if (EPI == EPI_GATE) {
         float g0 = 0.f, g1 = 0.f;
         if (valid) { const float2 hh = ldh2(p.h + pix * p.h_stride + c); g0 = sigmoid_fast(v0) * hh.x; g1 = sigmoid_fast(v1) * hh.y; }
@@ -101,10 +88,10 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
         v0 = sigmoid_fast(v0 + __ldg(g)); v1 = sigmoid_fast(v1 + __ldg(g + 1));
         if (valid) {
           if (c < 128) {
-            *reinterpret_cast<uint32_t*>(p.z + pix * 128 + c) = pack2(v0, v1);
+            *reinterpret_cast<uint32_t*>(p.z + pix * 128 + c) = pack_h2(v0, v1);
           } else {
             const float2 hh = ldh2(p.h + pix * p.h_stride + (c - 128));
-            *reinterpret_cast<uint32_t*>(p.rh + pix * 128 + (c - 128)) = pack2(v0 * hh.x, v1 * hh.y);
+            *reinterpret_cast<uint32_t*>(p.rh + pix * 128 + (c - 128)) = pack_h2(v0 * hh.x, v1 * hh.y);
           }
         }
       } else if (EPI == EPI_Q) {
@@ -112,7 +99,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
         if (valid) {
           const float2 hh = ldh2(p.h + pix * p.h_stride + c), zz = ldh2(p.z + pix * 128 + c);
           const float q0 = tanh_fast(v0 + __ldg(g)), q1 = tanh_fast(v1 + __ldg(g + 1));
-          *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack2((1.f - zz.x) * hh.x + zz.x * q0, (1.f - zz.y) * hh.y + zz.y * q1);
+          *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack_h2((1.f - zz.x) * hh.x + zz.x * q0, (1.f - zz.y) * hh.y + zz.y * q1);
         }
       } else if (EPI == EPI_F32) {
         if (valid && c < p.f32_cols) *reinterpret_cast<float2*>(p.f32a + pix * p.f32_stride + c) = make_float2(v0, v1);   // f32_cols even
@@ -124,12 +111,12 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
           o[HW] = __float2half_rn(v1);
         }
       } else if (EPI == EPI_STATS) {
-        if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack2(v0, v1);
+        if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack_h2(v0, v1);
       } else if (EPI == EPI_RELU_RES) {
         if (c < p.relu_cols) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
         if (valid) {
           if (p.h) { const float2 hh = ldh2(p.h + pix * p.h_stride + c); v0 = fmaxf(v0 + hh.x, 0.f); v1 = fmaxf(v1 + hh.y, 0.f); }
-          *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack2(v0, v1);
+          *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + c) = pack_h2(v0, v1);
         }
       }
     }
@@ -252,7 +239,7 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
               mbar_wait(b_empty + bs, ((bc / p.b_stages) & 1) ^ 1);
               mbar_expect_tx(b_full + bs, p.b_bytes);
               for (int n = 0; n < p.N; n += p.boxn)
-                tma_load_3d_w(sB + bs * p.b_bytes + n * 128, &tmW, b_full + bs, kb * 64, nt * p.N + n, dy * p.KS + dx);
+                tma_load_3d(sB + bs * p.b_bytes + n * 128, &tmW, b_full + bs, kb * 64, nt * p.N + n, dy * p.KS + dx);
               bc++;
             }
           }
@@ -329,44 +316,20 @@ __global__ void __launch_bounds__(kUpThreads, 1) conv_tc_kernel(const __grid_con
 // ---------------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFnU)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFnU get_encode_fn_u() {
-  static EncodeTiledFnU fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess) return nullptr;
-    fn = reinterpret_cast<EncodeTiledFnU>(ptr);
-  }
-  return fn;
-}
-
 // activation map: channels-last f16 [E][HT][WD][stride], channels [0, C) of the slice starting at `base`
 static int make_act_map(CUtensorMap* map, const void* base, int C, int stride, int WD, int HT, int E, int TW, int box_rows) {
-  EncodeTiledFnU enc = get_encode_fn_u();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return DBA_ERR_CUDA; }
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)WD, (cuuint64_t)HT, (cuuint64_t)E};
-  cuuint64_t strides[3] = {(cuuint64_t)stride * 2, (cuuint64_t)WD * stride * 2, (cuuint64_t)HT * WD * stride * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (activation, C=%d stride=%d %dx%d E=%d box %dx%d) failed with CUresult %d", C, stride, HT, WD, E, TW, box_rows, (int)r); return DBA_ERR_CUDA; }
-  return DBA_OK;
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)WD, (cuuint64_t)HT, (cuuint64_t)E};
+  const cuuint64_t strides[3] = {(cuuint64_t)stride * 2, (cuuint64_t)WD * stride * 2, (cuuint64_t)HT * WD * stride * 2};
+  const cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)box_rows, 1};
+  return tma_encode_f16(map, base, 4, dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "activation, C=%d stride=%d %dx%d E=%d box %dx%d",
+                        C, stride, HT, WD, E, TW, box_rows);
 }
 // weight map: [taps][Ntot][Kpad] f16
 static int make_weight_map(CUtensorMap* map, const void* base, int Kpad, int Ntot, int taps, int boxn) {
-  EncodeTiledFnU enc = get_encode_fn_u();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return DBA_ERR_CUDA; }
-  cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Ntot, (cuuint64_t)taps};
-  cuuint64_t strides[2] = {(cuuint64_t)Kpad * 2, (cuuint64_t)Ntot * Kpad * 2};
-  cuuint32_t box[3] = {64, (cuuint32_t)boxn, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (weights K=%d N=%d taps=%d) failed with CUresult %d", Kpad, Ntot, taps, (int)r); return DBA_ERR_CUDA; }
-  return DBA_OK;
+  const cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Ntot, (cuuint64_t)taps};
+  const cuuint64_t strides[2] = {(cuuint64_t)Kpad * 2, (cuuint64_t)Ntot * Kpad * 2};
+  const cuuint32_t box[3] = {64, (cuuint32_t)boxn, 1};
+  return tma_encode_f16(map, base, 3, dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "weights K=%d N=%d taps=%d", Kpad, Ntot, taps);
 }
 
 struct ConvSrc { const void* base; int C; int stride; };

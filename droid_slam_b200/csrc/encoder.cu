@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(256) image_im2col_kernel(const T* __restrict__
       const int kk = k + q, tap = kk / 3, c = kk - 3 * tap, dy = tap / 7, dx = tap - 7 * dy;
       v[q] = kk < kStemTaps ? halo[c][dy][2 * px + dx] : 0.f;
     }
-    *reinterpret_cast<uint32_t*>(out + (size_t)i * 2) = pack2(v[0], v[1]);
+    *reinterpret_cast<uint32_t*>(out + (size_t)i * 2) = pack_h2(v[0], v[1]);
   }
 }
 
@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(256) inorm_act_kernel(const __half* __restrict
   }
 #pragma unroll
   for (int k = 0; k < 8; k++) v[k] = fmaxf(v[k], 0.f);
-  *reinterpret_cast<uint4*>(out + pix * out_stride + c) = make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7]));
+  *reinterpret_cast<uint4*>(out + pix * out_stride + c) = make_uint4(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]), pack_h2(v[4], v[5]), pack_h2(v[6], v[7]));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------

@@ -72,8 +72,8 @@ __global__ void __launch_bounds__(256) nchw_to_nhwc_kernel(const T* __restrict__
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       const int cp = w + 8 * k;
-      tile[cbk][2 * lane][cp] = pack2(va[cbk][k].x, vb[cbk][k].x);
-      tile[cbk][2 * lane + 1][cp] = pack2(va[cbk][k].y, vb[cbk][k].y);
+      tile[cbk][2 * lane][cp] = pack_h2(va[cbk][k].x, vb[cbk][k].x);
+      tile[cbk][2 * lane + 1][cp] = pack_h2(va[cbk][k].y, vb[cbk][k].y);
     }
   __syncthreads();
 #pragma unroll
@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(256) flow_im2col_kernel(const float* __restric
     uint2 o = make_uint2(0u, 0u);
     if (slot < 49) {
       const int dy = slot / 7, dx = slot - dy * 7;
-      o = make_uint2(pack2(halo[0][dy][px + dx], halo[1][dy][px + dx]), pack2(halo[2][dy][px + dx], halo[3][dy][px + dx]));
+      o = make_uint2(pack_h2(halo[0][dy][px + dx], halo[1][dy][px + dx]), pack_h2(halo[2][dy][px + dx], halo[3][dy][px + dx]));
     }
     *reinterpret_cast<uint2*>(out + (size_t)i * 4) = o;
   }
@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(256) segment_mean_kernel(const __half* __restr
   }
   const float inv = en > b ? 1.f / (float)(en - b) : 0.f;
   *reinterpret_cast<uint4*>(dst + ((size_t)s * HW + pp) * 128 + cg) =
-      make_uint4(pack2(acc[0] * inv, acc[1] * inv), pack2(acc[2] * inv, acc[3] * inv), pack2(acc[4] * inv, acc[5] * inv), pack2(acc[6] * inv, acc[7] * inv));
+      make_uint4(pack_h2(acc[0] * inv, acc[1] * inv), pack_h2(acc[2] * inv, acc[3] * inv), pack_h2(acc[4] * inv, acc[5] * inv), pack_h2(acc[6] * inv, acc[7] * inv));
 }
 
 

@@ -35,9 +35,6 @@ enum {
 };
 
 const char* dba_last_error(void);   /* thread-local, human readable */
-/* device-wide L2 fetch granularity hint (32/64/128 B; cudaLimitMaxL2FetchGranularity); -1 when it cannot be read */
-int dba_set_l2_fetch_granularity(int bytes);
-int dba_get_l2_fetch_granularity(void);
 int dba_version(void);              /* 100 * major + minor */
 
 /* ---- correlation volume lookup ------------------------------------------------------------------
@@ -58,31 +55,23 @@ int dba_corr_index_backward(const float* coords, const void* corr_grad, void* vo
  * Any ht, wd >= 8 (DBA_ERR_INVALID below: the reference's avg_pool2d fails on a 1-pixel level).  Level l keeps only the complete
  * 2^l x 2^l blocks (avg_pool2d's floor rule): a trailing odd row or column is dropped at every level.  Level 0 is
  * fp16(sum_c f1 f2 / 16) from fp32 accumulators; levels 1-3 are the fp32 cascade of 2x2 means, each rounded once.
- * Checked before any launch: more than 65535 edges, null pointers, pointers not 16-byte aligned, a missing or small workspace. */
-/* 1 when dba_corr_volume_pyramid has a kernel for this shape / dtype (f16, 128 channels, ht >= 8, wd >= 8), else 0 */
-int dba_corr_volume_supported(int channels, int ht, int wd, int dtype);
-/* 1 when dba_corr_volume_pyramid_tiled has a kernel (f16, 128 channels, wd = 64, ht % 8 == 0), else 0 */
-int dba_corr_volume_tiled_supported(int channels, int ht, int wd, int dtype);
-/* device workspace of dba_corr_volume_pyramid_ws: 0 when wd % 8 == 0, else a copy of both feature-map tensors with rows padded to a
+ * Checked before any launch: more than 65535 edges, null pointers, pointers not 16-byte aligned, a missing or small workspace.
+ * tiled = 1: private layout, levels 0 and 1 of every plane stored as 4x8-element tiles ([h2/4][w2/8][4][8] f16 = one 64-byte DRAM atom
+ * per tile) for dba_corr_lookup_pyramid(tiled_mask = 3); levels 2, 3 and all tensor shapes are unchanged.  NOT readable by
+ * dba_corr_index_forward / the reference's CorrBlock.__call__.  Only for wd = 64, ht % 8 == 0 (DBA_ERR_INVALID elsewhere).
+ * workspace: 16-byte aligned, at least dba_corr_volume_workspace_bytes; may be NULL when that is 0. */
+/* 1 when dba_corr_volume_pyramid has a kernel for this shape / dtype / layout (f16, 128 channels, ht >= 8, wd >= 8; tiled: wd = 64,
+ * ht % 8 == 0), else 0 */
+int dba_corr_volume_supported(int channels, int ht, int wd, int dtype, int tiled);
+/* device workspace of dba_corr_volume_pyramid: 0 when wd % 8 == 0, else a copy of both feature-map tensors with rows padded to a
  * multiple of 8 pixels (TMA global strides are multiples of 16 bytes), about 2 * 2 * C * ht * wd bytes per frame.  Read and written once
  * per call: with one frame pair per edge about 1024 * ht * wd bytes per edge, against 2.66 * (ht * wd)^2 bytes of volume written. */
 size_t dba_corr_volume_workspace_bytes(int n_frames1, int n_frames2, int channels, int ht, int wd);
-/* every supported shape; workspace (16-byte aligned) of at least dba_corr_volume_workspace_bytes, may be NULL when that is 0 */
-int dba_corr_volume_pyramid_ws(const void* fmap1, const void* fmap2, const int64_t* ii, const int64_t* jj,
-                               void* out0, void* out1, void* out2, void* out3,
-                               int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype,
-                               void* workspace, size_t workspace_bytes, dba_stream_t stream);
-/* the same without a workspace: shapes with wd % 8 != 0 return DBA_ERR_INVALID */
 int dba_corr_volume_pyramid(const void* fmap1, const void* fmap2, const int64_t* ii, const int64_t* jj,
                             void* out0, void* out1, void* out2, void* out3,
-                            int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype, dba_stream_t stream);
+                            int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype, int tiled,
+                            void* workspace, size_t workspace_bytes, dba_stream_t stream);
 
-/* private-layout variant: levels 0 and 1 of every plane stored as 4x8-element tiles ([h2/4][w2/8][4][8] f16 = one 64-byte DRAM atom per
- * tile) for dba_corr_lookup_pyramid(tiled_mask = 3); levels 2, 3 and all tensor shapes are unchanged.  NOT readable by
- * dba_corr_index_forward / the reference's CorrBlock.__call__.  Only where dba_corr_volume_tiled_supported (DBA_ERR_INVALID elsewhere). */
-int dba_corr_volume_pyramid_tiled(const void* fmap1, const void* fmap2, const int64_t* ii, const int64_t* jj,
-                                  void* out0, void* out1, void* out2, void* out3,
-                                  int n_edges, int n_frames1, int n_frames2, int channels, int ht, int wd, int dtype, dba_stream_t stream);
 /* CorrBlock.__call__ (reference droid_slam/modules/corr.py:40-50) in one launch: out [n,196,h1,w1] = concatenation over the four levels
  * of corr_index_forward(volume_l, coords / 2^l, 3) -- bit-identical values; coords [n,2,h1,w1] f32 at level-0 scale are read once.
  * f16 volumes, h1, w1 >= 8, planes of level l [h1 >> l, w1 >> l], each level tensor 16-byte aligned; no load leaves a level tensor.

@@ -1,5 +1,5 @@
-"""Correlation pyramid at every image size, without a GPU: which shapes the C ABI accepts (dba_corr_volume_supported /
-dba_corr_volume_tiled_supported / dba_corr_volume_workspace_bytes), the argument checks that run before any launch, and the
+"""Correlation pyramid at every image size, without a GPU: which shapes the C ABI accepts (dba_corr_volume_supported with and
+without the tiled layout, dba_corr_volume_workspace_bytes), the argument checks that run before any launch, and the
 native / fallback / raise selection of install_corr_volume_hook on a stub backend."""
 import ctypes
 import types
@@ -14,8 +14,8 @@ INVALID = 1
 P = ctypes.c_void_p(1 << 20)            # a non-null, 16-byte aligned address: the calls below must return before touching it
 
 
-def test_new_symbols_are_exported(capi):
-    for name in ("dba_corr_volume_pyramid_ws", "dba_corr_volume_workspace_bytes", "dba_corr_volume_tiled_supported"):
+def test_single_entry_point_symbols_are_exported(capi):
+    for name in ("dba_corr_volume_pyramid", "dba_corr_volume_workspace_bytes", "dba_corr_volume_supported"):
         assert name in c_api.SYMBOLS and hasattr(capi, name)
 
 
@@ -25,10 +25,10 @@ def test_new_symbols_are_exported(capi):
     (128, 7, 64, F16, 0), (128, 48, 7, F16, 0), (128, 0, 0, F16, 0), (64, 48, 64, F16, 0), (256, 30, 40, F16, 0),
     (128, 48, 64, F32, 0), (128, 48, 64, BF16, 0),
 ])
-def test_volume_supported_truth_table(capi, channels, ht, wd, dtype, want):
-    assert capi.dba_corr_volume_supported(channels, ht, wd, dtype) == want
+def test_volume_supported_truth_table_with_tiled_flag(capi, channels, ht, wd, dtype, want):
+    assert capi.dba_corr_volume_supported(channels, ht, wd, dtype, 0) == want
     tiled = want and wd == 64 and ht % 8 == 0
-    assert capi.dba_corr_volume_tiled_supported(channels, ht, wd, dtype) == int(tiled)
+    assert capi.dba_corr_volume_supported(channels, ht, wd, dtype, 1) == int(tiled)
 
 
 def test_workspace_bytes(capi):
@@ -40,37 +40,35 @@ def test_workspace_bytes(capi):
         assert capi.dba_corr_volume_workspace_bytes(3, 5, 128, ht, wd) == one(3) + one(5)
 
 
-def _build(L, ht, wd, E=2, ws=None, ws_bytes=0, fn="dba_corr_volume_pyramid_ws", ptr=P):
-    args = [ptr] * 8 + [E, 4, 4, 128, ht, wd, F16]
-    if fn == "dba_corr_volume_pyramid_ws":
-        args += [ws, ws_bytes]
-    return getattr(L, fn)(*args, None)
+def _build(L, ht, wd, E=2, ws=None, ws_bytes=0, tiled=0, ptr=P):
+    return L.dba_corr_volume_pyramid(*[ptr] * 8, E, 4, 4, 128, ht, wd, F16, tiled, ws, ws_bytes, None)
 
 
 @pytest.mark.parametrize("ht, wd", [(7, 64), (48, 7), (5, 5)])
-def test_build_rejects_levels_without_a_pixel(capi, ht, wd):
-    for fn in ("dba_corr_volume_pyramid_ws", "dba_corr_volume_pyramid", "dba_corr_volume_pyramid_tiled"):
-        assert _build(capi, ht, wd, fn=fn) == INVALID
-        assert "at least 8" in capi.dba_last_error().decode()
+def test_single_entry_rejects_levels_without_a_pixel(capi, ht, wd):
+    for tiled in (0, 1):
+        for ws, ws_bytes in ((None, 0), (P, 1 << 30)):
+            assert _build(capi, ht, wd, ws=ws, ws_bytes=ws_bytes, tiled=tiled) == INVALID
+            assert "at least 8" in capi.dba_last_error().decode()
 
 
 @pytest.mark.parametrize("ht, wd", [(30, 40), (43, 70), (72, 96), (44, 64)])
-def test_tiled_builder_is_limited_to_wd64_shapes(capi, ht, wd):
-    assert _build(capi, ht, wd, fn="dba_corr_volume_pyramid_tiled") == INVALID
+def test_tiled_flag_is_limited_to_wd64_shapes(capi, ht, wd):
+    assert _build(capi, ht, wd, tiled=1) == INVALID
     assert "wd = 64" in capi.dba_last_error().decode()
 
 
-def test_build_checks_workspace_before_any_launch(capi):
+def test_single_entry_checks_workspace_before_any_launch(capi):
     need = capi.dba_corr_volume_workspace_bytes(4, 4, 128, 43, 70)
     assert need > 0
     assert _build(capi, 43, 70, ws=None, ws_bytes=need) == INVALID and "workspace" in capi.dba_last_error().decode()
     assert _build(capi, 43, 70, ws=P, ws_bytes=need - 1) == INVALID and "workspace" in capi.dba_last_error().decode()
-    assert _build(capi, 43, 70, fn="dba_corr_volume_pyramid") == INVALID and "workspace" in capi.dba_last_error().decode()
+    assert _build(capi, 43, 70, ws=None, ws_bytes=0) == INVALID and "workspace" in capi.dba_last_error().decode()
     assert _build(capi, 43, 70, ws=ctypes.c_void_p((1 << 20) + 8), ws_bytes=need) == INVALID
     assert "16-byte aligned" in capi.dba_last_error().decode()
 
 
-def test_build_checks_edges_pointers_alignment(capi):
+def test_single_entry_checks_edges_pointers_alignment(capi):
     assert _build(capi, 30, 40, E=65536) == INVALID and "65535" in capi.dba_last_error().decode()
     assert _build(capi, 30, 40, ptr=None) == INVALID and "null pointer" in capi.dba_last_error().decode()
     assert _build(capi, 30, 40, ptr=ctypes.c_void_p((1 << 20) + 2)) == INVALID and "16-byte aligned" in capi.dba_last_error().decode()
@@ -111,8 +109,7 @@ class _StubBackend:
         self.capi, self.calls = capi, []
 
     def corr_volume_supported(self, dim, ht, wd, tiled=False):
-        fn = self.capi.dba_corr_volume_tiled_supported if tiled else self.capi.dba_corr_volume_supported
-        return fn(dim, ht, wd, F16) != 0
+        return self.capi.dba_corr_volume_supported(dim, ht, wd, F16, int(tiled)) != 0
 
     def corr_volume_pyramid(self, f1, f2, ii, jj, tiled):
         self.calls.append(("build", tiled))
@@ -146,7 +143,7 @@ def _cls(**kw):
 
 
 @pytest.mark.parametrize("ht, wd, tiled", [(48, 64, True), (16, 64, True), (30, 40, False), (43, 70, False), (41, 73, False), (8, 8, False)])
-def test_hook_goes_native_at_every_supported_shape(stub, ht, wd, tiled):
+def test_hook_builds_natively_at_every_supported_shape(stub, ht, wd, tiled):
     f = _FakeCudaFmap((1, 3, 128, ht, wd))
     blk = _cls()(f, f)
     assert stub.calls == [("build", False)] and not hasattr(blk, "calls")
