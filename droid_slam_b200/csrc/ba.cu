@@ -68,11 +68,13 @@ __host__ inline Layout make_layout(int N, int E, int ht, int wd, int t0, int t1)
 enum { HDR_STATUS = 0, HDR_M = 1, HDR_CHOL_FAIL = 2, HDR_NBIG = 3 };
 enum { ST_BAD_INDEX = 1, ST_ETA_ROWS = 2, ST_CHOL_FAIL = 4, ST_DEGREE = 8 };
 
+constexpr int kSchurMaxRows = 255;   // Schur rows per depth frame (out-degree + 1); larger frames raise ST_DEGREE
+
 // ---------------------------------------------------------------------------------------------------------
 // prepare: kx = sorted unique(ii U [t0,t1)), frame2k, CSR of edges by source frame (stable in edge order)
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restrict__ ii, const int64_t* __restrict__ jj, int E, int N,
-                                                          int t0, int t1, int eta_rows, int* __restrict__ hdr,
+                                                          int t0, int t1, int eta_rows, int motion_only, int* __restrict__ hdr,
                                                           int* __restrict__ frame2k, int* __restrict__ kx, int* __restrict__ rowptr, int* __restrict__ big,
                                                           int HW, float* __restrict__ Eij, float* __restrict__ C, float* __restrict__ w,
                                                           float* __restrict__ Ei) {
@@ -154,6 +156,11 @@ __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restr
     if (tid == blockDim.x - 1) s_carry += s_scan[tid];
     __syncthreads();
   }
+  // the Schur kernels hold at most kSchurMaxRows rows per depth frame: flag a larger frame here, so that the caller can raise before
+  // build and solve change any state (motion-only runs no Schur kernel and has no such limit)
+  if (!motion_only)
+    for (int m = tid; m < M; m += blockDim.x)
+      if (rowptr[m + 1] - rowptr[m] > kSchurMaxRows - 1) atomicOr(&hdr[HDR_STATUS], ST_DEGREE);
   // depth frames that can have more than kTcRowsMax (21) rows = out-degree + 1: the pair-mode Schur launch only visits these
   // (ascending order; there are at most E / 21 of them, which is what sizes that launch's grid)
   if (tid == 0) s_carry = 0;
@@ -485,8 +492,6 @@ constexpr int kPairRowsMax = 100;
 // anyway (inf -> NaN system -> zero pose update and NaN depths at that pixel).  All Schur kernels and the back-substitution here
 // drop such a pixel instead (Q = 0, dz = 0): one rule on every path, documented in INTEGRATION.md.
 __device__ __forceinline__ float safe_rcp(float c) { return c > 0.f ? 1.0f / c : 0.f; }
-
-constexpr int kSchurMaxRows = 255;   // rows per frame (out-degree + 1); larger frames raise ST_DEGREE
 
 // Row list of a depth frame: (pose ix, Ei) first when ix is inside the window, then (pose jj[e], Eij[e]) for its out-edges in CSR
 // order whose target pose is inside the window.  Built by the whole CTA: thread a handles out-edge a, an order-preserving
@@ -1106,6 +1111,7 @@ extern "C" int dba_ba_prepare(const dba_ba_args* a) {
   Layout L; int rc = check_ba_args(a, L); if (rc) return rc;
   cudaStream_t st = (cudaStream_t)a->stream;
   ba_prepare_kernel<<<1, 1024, 0, st>>>(a->ii, a->jj, a->n_edges, a->n_frames, a->t0, a->t1, (a->motion_only || a->eta_by_frame) ? 1 : a->eta_rows,
+                                        a->motion_only,
                                         WS(int, L.off_hdr), WS(int, L.off_frame2k), WS(int, L.off_kx), WS(int, L.off_rowptr), WS(int, L.off_big),
                                         a->ht * a->wd, WS(float, L.off_Eij), WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei));
   DBA_CHECK_LAUNCH("ba_prepare");
@@ -1125,7 +1131,8 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
   double* bsys = Hsys + (size_t)L.n * L.n;
   DBA_CHECK_CUDA(cudaMemsetAsync(Hsys, 0, ((size_t)L.n * L.n + L.n) * sizeof(double), st), "ba_build memset");
   DBA_CHECK_CUDA(cudaMemsetAsync(WS(int, L.off_hdr) + HDR_CHOL_FAIL, 0, sizeof(int), st), "ba_build memset");
-  if (L.P == 0) return DBA_OK;
+  // an empty window still has depth blocks to build (and back-substitute with dx = 0) unless the call is motion-only
+  if (L.P == 0 && a->motion_only) return DBA_OK;
   // frames that can own edges on this rank (edge-sharded runs own a sub-range): size the pixel chunks so the grid fills the GPU
   const int eff_frames = std::max(1, std::min(a->n_frames, a->own_hi - a->own_lo));
   static int sms = 0;
@@ -1140,7 +1147,7 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
   if (ppt == 4) LAUNCH_BUILD(4); else if (ppt == 2) LAUNCH_BUILD(2); else LAUNCH_BUILD(1);
 #undef LAUNCH_BUILD
   DBA_CHECK_LAUNCH("ba_build");
-  if (!a->motion_only) {
+  if (!a->motion_only && L.P > 0) {
     const size_t smem2 = (size_t)2 * kSgK * kSgStride * sizeof(float);
     // the SGEMM-style kernel keeps its accumulators in registers over the whole pixel chunk: few long chunks, tile pairs over z
     const int px_per_cta2 = ((HW + 2) / 3 + kSgK - 1) / kSgK * kSgK;
@@ -1180,13 +1187,13 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
 
 extern "C" int dba_ba_solve(const dba_ba_args* a) {
   Layout L; int rc = check_ba_args(a, L); if (rc) return rc;
-  if (L.P == 0) return DBA_OK;
+  if (L.P == 0 && a->motion_only) return DBA_OK;
   cudaStream_t st = (cudaStream_t)a->stream;
   const int HW = a->ht * a->wd;
   double* Hsys = system_ptr(a, L);
   double* bsys = Hsys + (size_t)L.n * L.n;
   float* dx = WS(float, L.off_dx);
-  {
+  if (L.P > 0) {      // an empty window has no pose system: dx = 0, which the back-substitution never reads (0 < pose < P)
     CholPeers peers; peers.world = 0;
     if (a->p2p_world > 1) {
       const size_t nd = (size_t)L.n * L.n + L.n;
@@ -1206,8 +1213,10 @@ extern "C" int dba_ba_solve(const dba_ba_args* a) {
                                             WS(float, L.off_Ei), dx, a->disps, a->dz_out, a->own_lo, a->own_hi);
     DBA_CHECK_LAUNCH("ba_backsub");
   }
-  ba_pose_retr_kernel<<<(L.P + 127) / 128, 128, 0, st>>>(a->poses, dx, a->t0, L.P, a->dx_out, WS(int, L.off_hdr));
-  DBA_CHECK_LAUNCH("ba_pose_retr");
+  if (L.P > 0) {
+    ba_pose_retr_kernel<<<(L.P + 127) / 128, 128, 0, st>>>(a->poses, dx, a->t0, L.P, a->dx_out, WS(int, L.off_hdr));
+    DBA_CHECK_LAUNCH("ba_pose_retr");
+  }
   return DBA_OK;
 }
 

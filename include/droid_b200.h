@@ -182,6 +182,7 @@ int dba_proximity_edges(const float* d, int t0, int t1, int t, const int64_t* ii
  * [E,2,ht,wd]; eta [M,ht,wd] with M = |unique(ii U [t0,t1))| rows in ascending frame order (or 1 row,
  * broadcast); ii,jj [E] int64.  Outputs of the LAST Gauss-Newton iteration: dx_out [t1-t0,6], dz_out [M,ht*wd]
  * (dz_out untouched when motion_only).  Everything runs on `stream` with no host synchronisation.
+ * An empty window (t0 == t1) has no pose system; unless motion_only, the inverse depths still take dz = Q w (dx = 0).
  *
  * The call is split at the one point where a multi-GPU run exchanges data:
  *   dba_ba_prepare   graph bookkeeping (unique / CSR by source frame), once per call
@@ -231,7 +232,8 @@ int dba_ba_p2p_signal(const dba_ba_args* a);   /* after dba_ba_build, before dba
 /* synchronises `stream` and reads back M = number of depth frames found by the last dba_ba_prepare on this
  * workspace and the sticky device status word (0 = ok, bit0 = index out of range, bit1 = eta rows != M,
  * bit2 = Cholesky hit a non-positive pivot in some iteration -> that iteration's dx = 0 like the reference,
- * bit3 = a source frame has more than 254 out-edges: its Schur complement would be truncated, the result is not usable). */
+ * bit3 = a source frame has more than 254 out-edges and motion_only == 0: its Schur complement would be truncated, the result is
+ * not usable; dba_ba_prepare already sets it, so a caller can check before the first dba_ba_build changes any state). */
 int dba_ba_read_info(const dba_ba_args* a, int* n_depth_frames, int* device_status);
 
 /* ---- update operator (ConvGRU + heads + GraphAgg) on the tensor cores -----------------------------------

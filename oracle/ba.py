@@ -18,7 +18,8 @@ def ba_edge_terms(poses, disps, intrinsics, targets, weights, ii, jj):
     """projective_transform_kernel, src/droid_kernels.cu:185-433, vectorised over edges and pixels.
 
     Returns dict with Hs [4,E,6,6], vs [2,E,6], Eii,Eij [E,6,HW], Cii,bz [E,HW] (same meaning/layout as
-    the reference workspace, :1359-1364)."""
+    the reference workspace, :1359-1364), r2 [E,HW], the weighted squared residual wu*ru^2 + wv*rv^2, and
+    bz_mag [E,HW], the magnitude of bz's operands wu |Jz_u| (|ru| + |target_u|) + wv |Jz_v| (|rv| + |target_v|)."""
     dt = poses.dtype
     N, ht, wd = disps.shape
     E = ii.shape[0]
@@ -49,6 +50,9 @@ def ba_edge_terms(poses, disps, intrinsics, targets, weights, ii, jj):
     Jz_v = fy * (tij[:, None, 1] * d - tij[:, None, 2] * (y * d2))                                    # :361
     Cii = wu * Jz_u * Jz_u + wv * Jz_v * Jz_v                            # :329,362
     bz = wu * ru * Jz_u + wv * rv * Jz_v                                  # :330,363
+    r2 = wu * ru * ru + wv * rv * rv                                      # weighted squared residual (not in the reference)
+    # magnitude of the operands of bz: |w Jz| (|r| + |target|) covers both the residual's subtraction and the sum (not in the reference)
+    bz_mag = wu * Jz_u.abs() * (ru.abs() + tg[:, 0].abs()) + wv * Jz_v.abs() * (rv.abs() + tg[:, 1].abs())
     stereo = (ii == jj)[:, None]
     wu = torch.where(stereo, torch.zeros_like(wu), wu)                    # :332,365 (Q1)
     wv = torch.where(stereo, torch.zeros_like(wv), wv)
@@ -62,7 +66,7 @@ def ba_edge_terms(poses, disps, intrinsics, targets, weights, ii, jj):
     Eij = ((wu * Jz_u)[..., None] * Jj_u + (wv * Jz_v)[..., None] * Jj_v).permute(0, 2, 1).contiguous()
     Hs = torch.stack([H[:, :6, :6], H[:, :6, 6:], H[:, 6:, :6], H[:, 6:, 6:]], dim=0)                 # :416-427 (Q5)
     vs = torch.stack([vv[:, :6], vv[:, 6:]], dim=0)
-    return dict(Hs=Hs, vs=vs, Eii=Eii, Eij=Eij, Cii=Cii, bz=bz)
+    return dict(Hs=Hs, vs=vs, Eii=Eii, Eij=Eij, Cii=Cii, bz=bz, r2=r2, bz_mag=bz_mag)
 
 
 def ba_graph(ii, jj, t0, t1):
@@ -100,9 +104,10 @@ def _solve(A, b, lm, ep, P):
         return torch.zeros(P, 6, dtype=A.dtype), False
 
 
-def ba_system(terms, disps, disps_sens, eta, ii, jj, t0, t1, motion_only, dtype):
+def ba_system(terms, disps, disps_sens, eta, ii, jj, t0, t1, motion_only, dtype, drop_nonpositive_c=False):
     """Assemble the reduced pose system exactly like ba_cuda/schur_block (:1385-1415, :1231-1320).
-    Returns (A64, b64, aux) with A,b in fp64 BEFORE damping."""
+    Returns (A64, b64, aux) with A,b in fp64 BEFORE damping.
+    drop_nonpositive_c: Q = 0 where C <= 0, the native rule (INTEGRATION.md section 5), instead of the reference's 1/C."""
     P = t1 - t0
     E = ii.shape[0]
     ts, ii_exp, jj_exp, kx, kk_exp = ba_graph(ii, jj, t0, t1)
@@ -128,27 +133,29 @@ def ba_system(terms, disps, disps_sens, eta, ii, jj, t0, t1, motion_only, dtype)
     C = _segsum(terms["Cii"], ii, kx) + m * alpha + (1 - m) * eta.reshape(-1, HW).to(dtype)   # :1407
     w = _segsum(terms["bz"], ii, kx) - m * alpha * (disps[kx] - disps_sens[kx]).reshape(-1, HW)  # :1408
     Q = 1.0 / C                                                           # :1409
+    if drop_nonpositive_c:
+        Q = torch.where(C > 0, Q, torch.zeros_like(Q))
     Ei = _segsum(terms["Eii"], ii, ts)                                    # :1411  [P,6,HW]
     Erows = torch.cat([Ei, terms["Eij"]], dim=0)                         # :1412  [P+E,6,HW]
     pose = (jj_exp - t0)
     # S and bS (K9/K10): aggregate rows per (pose, depth frame), then E Q E^T per depth frame
-    S = torch.zeros(P, 6, P, 6, dtype=torch.float64)
+    S = torch.zeros(P, P, 6, 6, dtype=torch.float64)                      # [pose, pose, 6, 6]
     bS = torch.zeros(P, 6, dtype=torch.float64)
     M = kx.shape[0]
-    pl = pose.tolist(); kl = kk_exp.tolist()
+    in_window = (pose >= 0) & (pose < P)                                  # j in [t0,t1) (:1257; j==t1 is UB, Q8)
     for k in range(M):
-        rows = [n for n in range(P + E) if kl[n] == k and 0 <= pl[n] < P]  # j in [t0,t1) (:1257; j==t1 is UB, Q8)
-        if not rows:
+        rows = torch.nonzero((kk_exp == k) & in_window)[:, 0]
+        if rows.numel() == 0:
             continue
         Ek = Erows[rows]                                                  # [R,6,HW]
         G = torch.einsum("rap,p,sbp->rasb", Ek, Q[k], Ek).double()        # fp32 products like K9 (:1039-1046)
         gv = torch.einsum("rap,p->ra", Ek, Q[k] * w[k]).double()          # K10 (:1084-1087)
-        for a_, r in enumerate(rows):
-            bS[pl[r]] += gv[a_]
-            for c_, s in enumerate(rows):
-                S[pl[r], :, pl[s], :] += G[a_, :, c_, :]
+        pr = pose[rows]
+        R = pr.shape[0]
+        S.index_put_((pr[:, None].expand(R, R), pr[None, :].expand(R, R)), G.permute(0, 2, 1, 3), accumulate=True)
+        bS.index_add_(0, pr, gv)
     aux.update(C=C, w=w, Q=Q, Erows=Erows, pose=pose)
-    return A - S.reshape(6 * P, 6 * P), b - bS.reshape(6 * P), aux        # :1184-1186, :1415
+    return A - S.permute(0, 2, 1, 3).reshape(6 * P, 6 * P), b - bS.reshape(6 * P), aux        # :1184-1186, :1415
 
 
 def ba(poses, disps, intrinsics, disps_sens, targets, weights, eta, ii, jj, t0, t1,
