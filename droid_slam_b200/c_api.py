@@ -14,6 +14,7 @@ SYMBOLS = [
     "dba_ba_prepare", "dba_ba_build", "dba_ba_solve", "dba_ba", "dba_ba_read_info", "dba_ba_p2p_signal",
     "dba_solve_workspace_bytes", "dba_solve_spd", "dba_solve_tile_placement",
     "dba_update_workspace_bytes", "dba_update_forward", "dba_conv_nhwc", "dba_encoder_workspace_bytes", "dba_encoder_forward", "dba_proximity_workspace_bytes", "dba_proximity_edges",
+    "dba_fill_interpolate", "dba_pose_only_ba",
 ]
 
 DBA_F32, DBA_F16, DBA_F64, DBA_BF16 = 0, 1, 2, 3
@@ -88,6 +89,8 @@ def load():
     L.dba_proximity_workspace_bytes.restype = ctypes.c_size_t
     L.dba_proximity_workspace_bytes.argtypes = [ci, ci, ci]
     L.dba_proximity_edges.argtypes = [vp, ci, ci, ci, vp, vp, ci, ci, ci, cf, ci, ci, vp, ci, vp, vp, ctypes.c_size_t, vp]
+    L.dba_fill_interpolate.argtypes = [vp, vp, ci, vp, ci, vp, vp, vp, vp]
+    L.dba_pose_only_ba.argtypes = [vp] * 7 + [ci] * 8 + [cf, cf] + [vp] * 4
     _LIB = L
     return L
 

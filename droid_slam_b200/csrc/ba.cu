@@ -19,6 +19,7 @@
 //   * back-substitution dz = Q (w - E^T dx) keeps the reference quirk Q9 (rows whose pose index is <= 0 are skipped,
 //     src/droid_kernels.cu:1114), then retraction of poses (left-multiplicative Exp, no renormalisation) and disps.
 #include "common.cuh"
+#include "ba_pixel.cuh"
 #include "wgmma.cuh"
 #include <math.h>
 #include <algorithm>
@@ -207,21 +208,6 @@ __global__ void __launch_bounds__(256) ba_fill_csr_kernel(const int64_t* __restr
 // ---------------------------------------------------------------------------------------------------------
 // build: per (depth frame, pixel chunk): geometry of all out-edges, depth-block sums, per-edge pose blocks
 // ---------------------------------------------------------------------------------------------------------
-// total of value i ends up in lane i  (v[0] on return), 31 shuffles
-__device__ __forceinline__ float transpose_reduce32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; i++) {
-      const float send = up ? v[i] : v[i + off];
-      const float keep = up ? v[i + off] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  return v[0];
-}
-
 struct EdgeSm {
   float t[3], q[4];      // G_ij
   float A[36];           // Ji = -A Jj   (A = transposed adjoint, applied with the reference's adjSE3 arithmetic)
@@ -320,7 +306,6 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
     }
     for (int b = 0; b < nb; b++) {
       const EdgeSm& S = s_edge[b];
-      const float t0_ = S.t[0], t1_ = S.t[1], t2_ = S.t[2];
       const int e = S.e;
       float cw_u[kPPT], cw_v[kPPT], ct_u[kPPT], ct_v[kPPT];
 #pragma unroll
@@ -349,31 +334,15 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
       for (int s = 0; s < kPPT; s++) {
         const int p = pix[s];
         if (p < HW) {
-          float Xi[4] = {Xi0[s], Xi1[s], 1.f, dsp[s]}, Xj[4];
-          act_se3(S.t, S.q, Xi, Xj);
-          const float x = Xj[0], y = Xj[1], h = Xj[3];
-          const bool close = (double)Xj[2] < 0.25;   // MIN_DEPTH is a double literal in the reference
-          const float d = close ? 0.f : 1.0f / Xj[2];
-          const float d2 = d * d;
-          // `.001 * weight`: fp64 product rounded to fp32 (reference :314-315)
-          float wu = close ? 0.f : (float)(.001 * (double)cw_u[s]);
-          float wv = close ? 0.f : (float)(.001 * (double)cw_v[s]);
-          const float ru = ct_u[s] - (fx * d * x + cx);
-          const float rv = ct_v[s] - (fy * d * y + cy);
-          float Ju[6], Jv[6];
-          Ju[0] = fx * (h * d); Ju[1] = fx * 0; Ju[2] = fx * (-x * h * d2);
-          Ju[3] = fx * (-x * y * d2); Ju[4] = fx * (1 + x * x * d2); Ju[5] = fx * (-y * d);
-          Jv[0] = fy * 0; Jv[1] = fy * (h * d); Jv[2] = fy * (-y * h * d2);
-          Jv[3] = fy * (-1 - y * y * d2); Jv[4] = fy * (x * y * d2); Jv[5] = fy * (x * d);
-          const float Jzu = fx * (t0_ * d - t2_ * (x * d2));
-          const float Jzv = fy * (t1_ * d - t2_ * (y * d2));
-          Cacc[s] += wu * Jzu * Jzu + wv * Jzv * Jzv;
-          wacc[s] += wu * ru * Jzu + wv * rv * Jzv;
-          if (stereo) { wu = 0.f; wv = 0.f; }       // pose weights vanish AFTER the depth terms (Q1)
-          const float au = wu * Jzu, av = wv * Jzv;
+          PixelTerms P;
+          ba_pixel_terms(S.t, S.q, Xi0[s], Xi1[s], dsp[s], cw_u[s], cw_v[s], ct_u[s], ct_v[s], fx, fy, cx, cy, P);
+          Cacc[s] += P.wu * P.Jzu * P.Jzu + P.wv * P.Jzv * P.Jzv;
+          wacc[s] += P.wu * P.ru * P.Jzu + P.wv * P.rv * P.Jzv;
+          if (stereo) { P.wu = 0.f; P.wv = 0.f; }   // pose weights vanish AFTER the depth terms (Q1)
+          const float au = P.wu * P.Jzu, av = P.wv * P.Jzv;
           float Ej[6];
 #pragma unroll
-          for (int c = 0; c < 6; c++) Ej[c] = au * Ju[c] + av * Jv[c];
+          for (int c = 0; c < 6; c++) Ej[c] = au * P.Ju[c] + av * P.Jv[c];
           if (!motion_only) {
 #pragma unroll
             for (int c = 0; c < 6; c++) Eij[((size_t)e * 6 + c) * pitch + p] = Ej[c];
@@ -386,15 +355,7 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
               Eiacc[s][r] -= acc;
             }
           }
-          const float wru = wu * ru, wrv = wv * rv;
-          int l = 0;
-#pragma unroll
-          for (int a = 0; a < 6; a++) {
-            vj[a] += wru * Ju[a] + wrv * Jv[a];
-            const float wa_u = wu * Ju[a], wa_v = wv * Jv[a];
-#pragma unroll
-            for (int c = 0; c <= a; c++) { Hjj[l] += wa_u * Ju[c] + wa_v * Jv[c]; l++; }
-          }
+          ba_pose_accum(P, Hjj, vj);
         }
       }
       // warp reduction of the 27 sums (padded to 32): transpose-reduction, 31 shuffles; lane k ends with the total of value k
@@ -966,43 +927,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
 // ---------------------------------------------------------------------------------------------------------
 // back substitution + retractions
 // ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void exp_so3(const float* phi, float* q) {
-  const float theta_sq = phi[0] * phi[0] + phi[1] * phi[1] + phi[2] * phi[2];
-  const float theta_p4 = theta_sq * theta_sq;
-  const float theta = sqrtf(theta_sq);
-  float imag, real;
-  if ((double)theta_sq < 1e-8) {        // double literal comparison in the reference (:128)
-    imag = (float)(0.5 - (1.0 / 48.0) * (double)theta_sq + (1.0 / 3840.0) * (double)theta_p4);
-    real = (float)(1.0 - (1.0 / 8.0) * (double)theta_sq + (1.0 / 384.0) * (double)theta_p4);
-  } else {
-    imag = (float)((double)sinf((float)(0.5 * (double)theta)) / (double)theta);
-    real = cosf((float)(0.5 * (double)theta));
-  }
-  q[0] = imag * phi[0]; q[1] = imag * phi[1]; q[2] = imag * phi[2]; q[3] = real;
-}
-
-__device__ __forceinline__ void cross_inplace(const float* a, float* b) {
-  const float x0 = a[1] * b[2] - a[2] * b[1], x1 = a[2] * b[0] - a[0] * b[2], x2 = a[0] * b[1] - a[1] * b[0];
-  b[0] = x0; b[1] = x1; b[2] = x2;
-}
-
-__device__ __forceinline__ void exp_se3(const float* xi, float* t, float* q) {
-  exp_so3(xi + 3, q);
-  float tau[3] = {xi[0], xi[1], xi[2]};
-  const float phi[3] = {xi[3], xi[4], xi[5]};
-  const float theta_sq = phi[0] * phi[0] + phi[1] * phi[1] + phi[2] * phi[2];
-  const float theta = sqrtf(theta_sq);
-  t[0] = tau[0]; t[1] = tau[1]; t[2] = tau[2];
-  if ((double)theta > 1e-4) {
-    const float a = (1 - cosf(theta)) / theta_sq;
-    cross_inplace(phi, tau);
-    t[0] += a * tau[0]; t[1] += a * tau[1]; t[2] += a * tau[2];
-    const float b = (theta - sinf(theta)) / (theta * theta_sq);
-    cross_inplace(phi, tau);
-    t[0] += b * tau[0]; t[1] += b * tau[1]; t[2] += b * tau[2];
-  }
-}
-
 __global__ void __launch_bounds__(256) ba_backsub_kernel(
     const int64_t* __restrict__ jj, const int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
     const int* __restrict__ edgeidx, int HW, int t0, int P,
@@ -1048,20 +972,10 @@ __global__ void ba_pose_retr_kernel(float* __restrict__ poses, const float* __re
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k == 0 && hdr[HDR_CHOL_FAIL]) atomicOr(&hdr[HDR_STATUS], ST_CHOL_FAIL);   // sticky: some iteration was not SPD (its dx is 0)
   if (k >= P) return;
-  float xi[6], t[3], q[4], dt[3] = {0, 0, 0}, dq[4] = {0, 0, 0, 1}, t1[3], q1[4];
-  float* ps = poses + 7 * (size_t)(t0 + k);
+  float xi[6];
 #pragma unroll
   for (int c = 0; c < 6; c++) { xi[c] = dx[k * 6 + c]; if (dx_out) dx_out[k * 6 + c] = xi[c]; }
-  t[0] = ps[0]; t[1] = ps[1]; t[2] = ps[2];
-  q[0] = ps[3]; q[1] = ps[4]; q[2] = ps[5]; q[3] = ps[6];
-  exp_se3(xi, dt, dq);
-  q1[0] = dq[3] * q[0] + dq[0] * q[3] + dq[1] * q[2] - dq[2] * q[1];
-  q1[1] = dq[3] * q[1] + dq[1] * q[3] + dq[2] * q[0] - dq[0] * q[2];
-  q1[2] = dq[3] * q[2] + dq[2] * q[3] + dq[0] * q[1] - dq[1] * q[0];
-  q1[3] = dq[3] * q[3] - dq[0] * q[0] - dq[1] * q[1] - dq[2] * q[2];
-  act_so3(dq, t, t1);
-  ps[0] = t1[0] + dt[0]; ps[1] = t1[1] + dt[1]; ps[2] = t1[2] + dt[2];
-  ps[3] = q1[0]; ps[4] = q1[1]; ps[5] = q1[2]; ps[6] = q1[3];
+  retract_pose(xi, poses + 7 * (size_t)(t0 + k));
 }
 
 }  // namespace dba

@@ -442,6 +442,74 @@ void graph_writeback(torch::Tensor delta, torch::Tensor weight, torch::Tensor co
                                    n_src, damping.data_ptr<float>(), baf, n_ba, bad, (float)ep, ht, wd, cur_stream()), "graph_writeback");
 }
 
+// extension: the pose interpolation of PoseTrajectoryFiller.__fill (reference trajectory_filler.py:51-65).  poses [N,7] and tstamps [N] of
+// the keyframes, t [F] f32 -> [t0 [F] int64, t1 [F] int64, poses [F,7]].
+std::vector<torch::Tensor> fill_interpolate(torch::Tensor poses, torch::Tensor tstamps, torch::Tensor t) {
+  CHECK_INPUT(poses); CHECK_INPUT(tstamps); CHECK_INPUT(t);
+  CHECK_F32(poses); CHECK_F32(tstamps); CHECK_F32(t);
+  TORCH_CHECK(poses.dim() == 2 && poses.size(1) == 7, "poses must be [N,7]");
+  TORCH_CHECK(tstamps.dim() == 1 && tstamps.size(0) == poses.size(0), "tstamps must be [N] with N = len(poses)");
+  TORCH_CHECK(t.dim() == 1, "t must be [F]");
+  TORCH_CHECK(poses.size(0) >= 1, "fill_interpolate: no keyframe to interpolate from (the reference indexes an empty tensor here)");
+  const auto dev = poses.device();
+  TORCH_CHECK(tstamps.device() == dev && t.device() == dev, "fill_interpolate: all tensors on one device");
+  c10::cuda::CUDAGuard guard(dev);
+  const int F = (int)t.size(0);
+  auto t0 = torch::empty({F}, poses.options().dtype(torch::kInt64));
+  auto t1 = torch::empty({F}, poses.options().dtype(torch::kInt64));
+  auto out = torch::empty({F, 7}, poses.options());
+  check_status(dba_fill_interpolate(poses.data_ptr<float>(), tstamps.data_ptr<float>(), (int)poses.size(0), t.data_ptr<float>(), F,
+                                    t0.data_ptr<int64_t>(), t1.data_ptr<int64_t>(), out.data_ptr<float>(), cur_stream()), "fill_interpolate");
+  return {t0, t1, out};
+}
+
+// extension: motion-only BA of the trajectory filler's graph (every edge from a fixed frame ii < t0 to one frame t0 <= jj < t1), all
+// iterations in one launch.  Arguments as ba (intrinsics: the single camera; disps: only the rows of the fixed frames are read).  Returns
+// [status (int32 [1] on the device)], with diagnostics also dx [t1-t0,6] and the undamped blocks sys [t1-t0,42] f64 (H row-major, then b)
+// of the last iteration.  check: read the status back (one stream synchronisation) and raise when an edge breaks the structure (no pose has then
+// changed) / warn when a block was not positive definite; skipped while the stream is being captured.
+std::vector<torch::Tensor> pose_only_ba(torch::Tensor poses, torch::Tensor disps, torch::Tensor intrinsics, torch::Tensor targets,
+                                        torch::Tensor weights, torch::Tensor ii, torch::Tensor jj, const int t0, const int t1, const int iterations,
+                                        const float lm, const float ep, const bool check, const bool diagnostics) {
+  CHECK_INPUT(targets); CHECK_INPUT(weights); CHECK_INPUT(poses); CHECK_INPUT(disps); CHECK_INPUT(intrinsics); CHECK_INPUT(ii); CHECK_INPUT(jj);
+  CHECK_F32(targets); CHECK_F32(weights); CHECK_F32(poses); CHECK_F32(disps); CHECK_F32(intrinsics);
+  CHECK_I64(ii); CHECK_I64(jj);
+  TORCH_CHECK(poses.dim() == 2 && poses.size(1) == 7, "poses must be [N,7]");
+  TORCH_CHECK(disps.dim() == 3, "disps must be [n,ht,wd]");
+  TORCH_CHECK(intrinsics.numel() >= 4, "intrinsics must hold fx,fy,cx,cy");
+  const auto dev = poses.device();
+  for (auto* x : {&disps, &intrinsics, &targets, &weights, &ii, &jj}) TORCH_CHECK(x->device() == dev, "pose_only_ba: all tensors on one device");
+  const int N = (int)poses.size(0), ht = (int)disps.size(1), wd = (int)disps.size(2);
+  const int E = (int)ii.numel();
+  TORCH_CHECK(jj.numel() == E, "ii and jj must have the same length");
+  TORCH_CHECK(targets.numel() == (int64_t)E * 2 * ht * wd && weights.numel() == (int64_t)E * 2 * ht * wd, "targets/weights must be [E,2,ht,wd]");
+  TORCH_CHECK(t0 >= 0 && t1 >= t0 && t1 <= N, "invalid window [t0,t1)");
+  TORCH_CHECK(iterations >= 0, "iterations must be >= 0");
+  c10::cuda::CUDAGuard guard(dev);
+  auto status = torch::empty({1}, poses.options().dtype(torch::kInt32));
+  torch::Tensor dx, sys;
+  if (diagnostics) {
+    dx = torch::zeros({t1 - t0, 6}, poses.options());
+    sys = torch::zeros({t1 - t0, 42}, poses.options().dtype(torch::kFloat64));
+  }
+  check_status(dba_pose_only_ba(poses.data_ptr<float>(), disps.data_ptr<float>(), intrinsics.data_ptr<float>(), targets.data_ptr<float>(),
+                                weights.data_ptr<float>(), ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), N, (int)disps.size(0), E, ht, wd, t0, t1,
+                                iterations, lm, ep, status.data_ptr<int>(), diagnostics ? sys.data_ptr<double>() : nullptr,
+                                diagnostics ? dx.data_ptr<float>() : nullptr, cur_stream()),
+               "pose_only_ba");
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  cudaStreamIsCapturing((cudaStream_t)cur_stream(), &cap);
+  if (check && cap == cudaStreamCaptureStatusNone) {
+    const int st = status.cpu().data_ptr<int>()[0];
+    TORCH_CHECK(!(st & 1), "droid_backends.pose_only_ba: an edge is not (0 <= ii < min(t0, len(disps)), t0 <= jj < t1); no pose was changed");
+    if (st & 2)
+      TORCH_WARN("droid_backends.pose_only_ba: a damped pose block was not positive definite in at least one iteration; that frame's update "
+                 "is zero in that iteration (the reference zeroes the whole window's update)");
+  }
+  if (!diagnostics) return {status};
+  return {status, dx, sys};
+}
+
 // extension: the update operator (reference droid_slam/droid_net.py:111-143, modules/gru.py:19-32, droid_net.py:59-75) on the tensor
 // cores.  net [E,128,ht,wd] f16/f32 (or channels-last f16 [E,ht,wd,128] when net_channels_last), inp [E,128,ht,wd], corr [E,196,ht,wd],
 // flow [E,4,ht,wd] f32 or None, seg [E] int64 (torch.unique inverse of the source frames) or None, n_src distinct sources,
@@ -643,5 +711,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_nhwc", &conv_nhwc,"channels-last 1x1/3x3 convolution on wgmma, native extension");
   m.def("cvx_upsample", &cvx_upsample, "convex upsampling of inverse depth maps (droid_net.cvx_upsample, dim = 1), native extension");
   m.def("proximity_edges", &proximity_edges, "edge selection of FactorGraph.add_proximity_factors (factor_graph.py:357-411), native extension");
+  m.def("fill_interpolate", &fill_interpolate, "pose interpolation of PoseTrajectoryFiller.__fill -> [t0, t1, poses], native extension",
+        pybind11::arg("poses"), pybind11::arg("tstamps"), pybind11::arg("t"));
+  m.def("pose_only_ba", &pose_only_ba, "motion-only BA of the trajectory filler's graph, all iterations in one launch -> [status(, dx, sys)], native extension",
+        pybind11::arg("poses"), pybind11::arg("disps"), pybind11::arg("intrinsics"), pybind11::arg("targets"), pybind11::arg("weights"),
+        pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("t0"), pybind11::arg("t1"), pybind11::arg("iterations") = 2,
+        pybind11::arg("lm") = 1e-4f, pybind11::arg("ep") = 0.1f, pybind11::arg("check") = true,
+        pybind11::arg("diagnostics") = false);
   m.def("_b200_native", []() { return true; });
 }

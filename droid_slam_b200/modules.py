@@ -22,6 +22,9 @@ kernel for is offered as a hook:
     motion features (`droid_backends.motion_features`), the update operator on whole source frames, the write-back of its outputs
     into the graph and BA's inputs (`droid_backends.graph_writeback`).
   * `install_depth_video_hook(DepthVideo)`: `DepthVideo.reproject` / `DepthVideo.upsample` on `reproject` / `upsample` below.
+  * `fill_trajectory(filler, stream)` / `install_trajectory_filler_hook(trajectory_filler)`: `PoseTrajectoryFiller.__call__`
+    (trajectory_filler.py:42-110) with on-device pose interpolation (`droid_backends.fill_interpolate`), batches sized by free device
+    memory and a one-launch motion-only BA per update (`droid_backends.pose_only_ba`).
 """
 import sys
 
@@ -30,7 +33,8 @@ import torch
 from . import install
 
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
-           "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks"]
+           "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
+           "install_trajectory_filler_hook"]
 
 
 def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
@@ -211,6 +215,7 @@ def install_encoder_hook(extractor_module, strict=True):
             out = out.to(x.dtype)
         return out.view(b, n, -1, h // 8, w // 8)
 
+    forward._b200_native = True
     cls.forward = forward
     return extractor_module
 
@@ -516,3 +521,143 @@ def install_factor_graph_hook(factor_graph_class, strict=True):
     factor_graph_class.update = _update
     factor_graph_class.update_lowmem = _update_lowmem
     return factor_graph_class
+
+
+# ---- PoseTrajectoryFiller ------------------------------------------------------------------------------------------------------------
+
+_FILL_UPDATES = 6     # graph.update(N, N+M, motion_only=True) calls per batch (trajectory_filler.py:78-79)
+_FNET_IMAGES = 16     # images per fnet call: the reference's batch
+
+
+def _filler_unsupported(filler):
+    """why fill_trajectory cannot run this PoseTrajectoryFiller natively (None: it can)"""
+    from .update import UpdateModule
+    if not isinstance(filler.update, UpdateModule):
+        return "filler.update is %s, not droid_slam_b200.update.UpdateModule" % type(filler.update).__name__
+    if not getattr(type(filler.fnet).forward, "_b200_native", False):
+        return "filler.fnet (%s) is not a BasicEncoder under install_encoder_hook" % type(filler.fnet).__name__
+    video = filler.video
+    for name in ("poses", "disps", "intrinsics", "tstamp", "fmaps", "nets", "inps"):
+        t = getattr(video, name, None)
+        if not (isinstance(t, torch.Tensor) and t.is_cuda):
+            return "video.%s is not a CUDA tensor" % name
+    if video.counter.value < 1:
+        return "the video has no keyframe"
+    return None
+
+
+def _filler_frame_budget(be, ht, wd, device):
+    """the most frames one fill_trajectory batch takes: a quarter of the free device memory over what one frame needs -- two edges, each
+    with its volume pyramid (f16, four levels), its share of the update operator's workspace, its corr features, hidden state and outputs;
+    and the frame's image (64 hw pixels x 3 channels) as uint8 on the device, its normalised fp32 copy and the fp32 temporary made on the
+    way, its feature map (f16, 128 channels) and its pose / intrinsics rows"""
+    hw = ht * wd
+    volume = 2 * sum(hw * (ht >> l) * (wd >> l) for l in range(4))
+    per_edge = volume + -(-be.update_workspace_bytes(64, 64, ht, wd) // 64) + hw * (196 * 2 + 128 * 2 * 3 + 2 * 2 * 4 * 4 + 4 * 4)
+    per_image = 64 * hw * 3 * (1 + 4 + 4) + hw * 128 * 2 + 4 * (7 + 4)
+    free, _ = torch.cuda.mem_get_info(device)
+    return max(1, (free // 4) // (2 * per_edge + per_image))
+
+
+def _pinned_to(dev, t):
+    """a CPU tensor to the device without a host synchronisation (pinned staging, non-blocking copy); device tensors pass through"""
+    return t.to(dev) if t.is_cuda else t.pin_memory().to(dev, non_blocking=True)
+
+
+def _fill_batch(be, filler, tstamps, images, intrinsics):
+    """PoseTrajectoryFiller.__fill (trajectory_filler.py:42-84) for one batch of any size, with one host read -> (poses [M,7] on the
+    device, the host copies of t0 and t1 [M] and of the edge list ii / jj in combined-frame indices).
+    Frames [0, B) of the combined state are the video's buffer slots, frames [B, B+M) this batch; the video is only read."""
+    video = filler.video
+    dev = video.poses.device
+    N, B, M = video.counter.value, video.poses.shape[0], len(tstamps)
+    num, rig, ch, ht, wd = video.fmaps.shape
+    tt = _pinned_to(dev, torch.as_tensor(tstamps))
+    images = _pinned_to(dev, torch.stack(images, 0))
+    intr = _pinned_to(dev, torch.stack(intrinsics, 0)) / 8.0
+    inputs = (images.flip(2) / 255.0).sub_(filler.MEAN).div_(filler.STDV)        # images[:, :, [2, 1, 0]] without an index upload
+    with torch.autocast("cuda", enabled=True):
+        fmap = torch.cat([filler.fnet(inputs[a:a + _FNET_IMAGES]) for a in range(0, M, _FNET_IMAGES)])
+    t0, t1, G = be.fill_interpolate(video.poses[:N].contiguous(), video.tstamp[:N].contiguous(), tt.float().contiguous())
+
+    host = torch.stack([t0, t1]).cpu()                                   # the one host read: the edge list
+    k = torch.arange(M)
+    two = host[1] != host[0]                 # add_factors(t1, ...) drops the duplicates of the t0 edges (__filter_repeated_edges)
+    ii = torch.cat([host[0], host[1][two]])
+    jj = torch.cat([k, k[two]])
+    ii = torch.where(ii < 0, ii + B, ii)     # t0 = -1: the reference's graph indexes slot -1 of the video's buffers, the last one
+    E = ii.numel()
+    ii_d, jj_d, jloc_d = _to_device(dev, [ii, jj + B, jj])
+
+    with torch.autocast("cuda", enabled=False):
+        poses = torch.cat([video.poses, G])
+        intr_all = torch.cat([video.intrinsics, intr.float()])
+        f1 = video.fmaps[:, 0]
+        if f1.is_contiguous():
+            vol_i = ii_d
+        else:                                # stereo buffers: gather the edges' left images
+            f1, vol_i = video.fmaps[ii_d, 0], torch.arange(E, device=dev)
+        tiled = be.corr_volume_supported(ch, ht, wd, True)
+        pyr = be.corr_volume_pyramid(f1, fmap[:, 0].contiguous(), vol_i, jloc_d, tiled)
+        target = be.reproject(poses, video.disps, intr_all, ii_d, jj_d)[0]
+        weight = torch.zeros_like(target)
+        net, inp = video.nets[ii_d][None], video.inps[ii_d][None]
+        ba_target = torch.empty(E, 2, ht, wd, device=dev)
+        ba_weight = torch.empty_like(ba_target)
+        damping = torch.empty(1, ht, wd, device=dev)                    # graph_writeback's shape argument; motion-only BA has no eta
+        intr0 = video.intrinsics[0].contiguous()
+        for _ in range(_FILL_UPDATES):
+            coords, coords_t, motn = be.motion_features(poses, video.disps, intr_all, ii_d, jj_d, target)
+            corr = be.corr_lookup_pyramid(pyr, coords_t, tiled).view(1, E, -1, ht, wd)
+            net, delta, w = filler.update.forward_segments(net, inp, corr, motn[None], None, 0)
+            be.graph_writeback(delta[0], w[0], coords, None, target, weight, ba_target, ba_weight, 0, None, None, damping, None, None, 0.0)
+            be.pose_only_ba(poses, video.disps, intr0, ba_target, ba_weight, ii_d, jj_d, B, B + M, 2, 1e-4, 0.1, False)
+    return poses[B:], (host[0], host[1], ii, jj + B)
+
+
+def fill_trajectory(filler, image_stream):
+    """PoseTrajectoryFiller.__call__ (reference trajectory_filler.py:86-110) on the native kernels -> poses [T,7] of every frame of the
+    stream, `filler` being the reference's PoseTrajectoryFiller (or an object with its attributes: fnet, update, video, MEAN, STDV).
+
+    Same steps per frame as the reference: pose interpolation between the bracketing keyframes (droid_backends.fill_interpolate), fnet,
+    the edges from the keyframes t0 and t1 to the frame, their correlation volumes, initial targets from the reprojection, then six times
+    the motion features, the corr lookup, the update operator (no GraphAgg: the filler graph neither upsamples nor uses eta) and two
+    Gauss-Newton iterations of motion-only BA (droid_backends.pose_only_ba).  Every frame is independent of the others, so frames are
+    batched by free device memory instead of by 16; one host read per batch.  Differences from the reference: the video is left as it
+    was (the reference leaves the last batch in slots [N, N+16)), and a frame whose damped pose block is not positive definite keeps its
+    pose in that iteration on its own (the reference zeroes the update of its whole 16-frame batch).  Raises when the filler cannot run
+    natively (see install_trajectory_filler_hook)."""
+    why = _filler_unsupported(filler)
+    if why is not None:
+        raise RuntimeError("the native trajectory filler cannot run this filler: %s" % why)
+    be = install()
+    video = filler.video
+    budget = _filler_frame_budget(be, video.fmaps.shape[3], video.fmaps.shape[4], video.poses.device)
+    out, batch = [], ([], [], [])
+    with torch.no_grad():
+        for tstamp, image, intrinsic in image_stream:
+            for lst, x in zip(batch, (tstamp, image, intrinsic)):
+                lst.append(x)
+            if len(batch[0]) == budget:
+                out.append(_fill_batch(be, filler, *batch)[0])
+                batch = ([], [], [])
+        if batch[0]:
+            out.append(_fill_batch(be, filler, *batch)[0])
+    return torch.cat(out) if out else video.poses.new_zeros(0, 7)
+
+
+def install_trajectory_filler_hook(trajectory_filler_module, strict=True):
+    """trajectory_filler_module = the imported reference module `trajectory_filler`.  Replaces `PoseTrajectoryFiller.__call__` by
+    fill_trajectory; the result is an SE3 of that module's own lietorch, as the reference returns.  strict: a filler the native path
+    cannot run (update operator not droid_slam_b200.update.UpdateModule, fnet not a BasicEncoder under install_encoder_hook, video tensors
+    not on CUDA) raises, naming the reason; with strict=False the reference's own method runs for it."""
+    cls = trajectory_filler_module.PoseTrajectoryFiller
+    ref_call = cls.__call__
+
+    def __call__(self, image_stream):
+        if not strict and _filler_unsupported(self) is not None:
+            return ref_call(self, image_stream)
+        return trajectory_filler_module.SE3(fill_trajectory(self, image_stream))
+
+    cls.__call__ = __call__
+    return trajectory_filler_module

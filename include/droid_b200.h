@@ -236,6 +236,27 @@ int dba_ba_p2p_signal(const dba_ba_args* a);   /* after dba_ba_build, before dba
  * not usable; dba_ba_prepare already sets it, so a caller can check before the first dba_ba_build changes any state). */
 int dba_ba_read_info(const dba_ba_args* a, int* n_depth_frames, int* device_status);
 
+/* ---- non-keyframe pose filling (PoseTrajectoryFiller, reference droid_slam/trajectory_filler.py) -----------------------
+ * dba_fill_interpolate: the linear pose interpolation of `__fill` (:51-65), one thread per frame.  poses [n_keyframes,7], tstamps
+ * [n_keyframes] f32 (any order), t [n] f32 -> t0_out / t1_out [n] int64, poses_out [n,7]:  t0 = #{k : tstamps[k] <= t} - 1,
+ * t1 = t0 + 1 if t0 < n_keyframes - 1 else t0, dt = tstamps[t1] - tstamps[t0] + 1e-3,
+ * G = Exp(Log(P[t1] P[t0]^-1) / dt * (t - tstamps[t0])) P[t0] with lietorch's SE3 formulas in fp32.  t0 = -1 (t before every keyframe) is
+ * written as is; index -1 then reads keyframe n_keyframes - 1, like Python's negative indexing in the reference.  n_keyframes >= 1.
+ * dba_pose_only_ba: `iterations` Gauss-Newton iterations of motion-only BA (dba_ba with motion_only = 1) in one launch, for graphs whose
+ * every edge goes from a fixed frame to one optimised frame: 0 <= ii < min(t0, n_disps), t0 <= jj < t1.  The pose system is then block
+ * diagonal: per optimised frame the Hjj / vj sums of its edges (ascending edge order, fp64 across warps and edges, no atomics: bit-
+ * reproducible whatever other frames share the call), damping diag += ep + lm * diag, a 6x6 fp64 Cholesky, poses <- Exp(dx) poses.
+ * poses [n_frames,7] (rows [t0,t1) updated in place), disps [n_disps,ht,wd], intrinsics [4] (the single camera of dba_ba), targets /
+ * weights [E,2,ht,wd], ii / jj [E] int64.  status: device int32 [1], overwritten: bit 0 = an edge breaks the structure above (checked by
+ * a first launch; no pose changes), bit 1 = some frame's damped block was not positive definite (its dx = 0 in that iteration; dba_ba
+ * zeroes the whole window's update instead).  Optional outputs of the last iteration (may be NULL): sys_out [t1-t0][42] f64 = the
+ * undamped block H (6x6 row-major) and b (6), dx_out [t1-t0][6].  No host synchronisation. */
+int dba_fill_interpolate(const float* poses, const float* tstamps, int n_keyframes, const float* t, int n, int64_t* t0_out,
+                         int64_t* t1_out, float* poses_out, dba_stream_t stream);
+int dba_pose_only_ba(float* poses, const float* disps, const float* intrinsics, const float* targets, const float* weights,
+                     const int64_t* ii, const int64_t* jj, int n_frames, int n_disps, int n_edges, int ht, int wd, int t0, int t1,
+                     int iterations, float lm, float ep, int* status, double* sys_out, float* dx_out, dba_stream_t stream);
+
 /* ---- update operator (ConvGRU + heads + GraphAgg) on the tensor cores -----------------------------------
  * replaces UpdateModule.forward (reference droid_slam/droid_net.py:111-143), ConvGRU.forward (droid_slam/modules/gru.py:19-32) and
  * GraphAgg.forward (droid_net.py:59-75) -- in the reference a chain of 19 cuDNN convolutions + ~25 elementwise launches.
