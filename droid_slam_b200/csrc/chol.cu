@@ -59,7 +59,9 @@ __device__ __forceinline__ double fast_rsqrt(double d) {
 }
 
 // Cholesky of a 32x32 tile, one row per lane in registers; the pivot column is broadcast through `col` (2 x 32 doubles of shared memory
-// private to the warp).  rdiag_out receives 1/L[k][k] (lane k's value).  Returns false on a non-positive pivot.  Fully unrolled (~1800
+// private to the warp).  rdiag_out receives 1/L[k][k] (lane k's value).  Returns false on a pivot that is not positive and finite.
+// `d > 0` passes +Inf, whose fast_rsqrt is NaN: in columns 0-30 that NaN makes the next pivot NaN, which the same test catches, so only the
+// last column's r is tested as well (one comparison: a per-column test of r costs this routine stack spills).  Fully unrolled (~1800
 // straight-line instructions): used only for tile (0,0) of chol_cluster_kernel, which every other warp of the cluster waits for.  There
 // it is faster than warp_potrf_compact (measured on H100: the compact routine made banded n = 2394 solves 3-10 us slower) with the
 // same bits.
@@ -87,6 +89,7 @@ __device__ __forceinline__ bool warp_potrf(double (&a)[kT], int lane, double* co
 #pragma unroll
     for (int j = k + 2; j < kT; j++) a[j] -= l * cb[j];   // only rows >= j are meaningful
   }
+  if (!(r > 0.0)) ok = false;                              // r of column 31: NaN for an infinite last pivot
   return ok;
 }
 
@@ -97,13 +100,13 @@ __device__ __forceinline__ bool warp_potrf(double (&a)[kT], int lane, double* co
 // a rolled loop; four loops of eight columns with widths 32/24/16/8 keep the extra arithmetic at 608 instead of 496 DFMAs.  The pivot
 // column is published twice (offset by one double) so that the operands of the rank-1 update can be fetched with aligned 16-byte loads
 // whatever the parity of the column.  Per element the operations and their order are those of warp_potrf: identical bits.
-// out[lane][k] receives L (zeros above the diagonal).
+// out[lane][k] receives L (zeros above the diagonal).  The pivot test is on r = fast_rsqrt(d), NaN for d <= 0, NaN and +Inf alike.
 template <int W>
 __device__ __forceinline__ void potrf_phase(double (&a)[kT], int lane, int k0, double* cx, double* cy, double (*out)[kTP], double& d, double& r, bool& ok,
                                             double& rdiag_out) {
 #pragma unroll 1
   for (int k = k0; k < k0 + 8; k++) {
-    if (!(d > 0.0)) ok = false;
+    if (!(r > 0.0)) ok = false;
     const double l = (lane == k) ? d * r : a[0] * r;
     if (lane == k) rdiag_out = r;
     out[lane][k] = (lane >= k) ? l : 0.0;

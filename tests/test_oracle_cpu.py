@@ -319,32 +319,3 @@ def test_synthetic_graph_properties():
         ii2, jj2 = synth.make_graph(c["E"], c["N"], stereo=c["stereo"], seed=0)
         assert torch.equal(ii, ii2) and torch.equal(jj, jj2)      # deterministic
 
-
-def test_resident_cholesky_tile_placement_invariants():
-    """host logic of csrc/chol.cu (resident_tile_map): every tile of the lower triangle and every right-hand-side piece has exactly one
-    warp slot, diagonal tile s sits on CTA s, and a tile of column c shares an SM with diagonal tile s only if it is finished before
-    potrf(s) runs (c < s) -- or the SM has no diagonal tile / is CTA 0 (potrf(0) runs before anything else has operands)."""
-    import ctypes
-    from droid_slam_b200 import c_api
-    L = c_api.load()
-    for n in [1, 6, 30, 42, 96, 100, 200, 256, 300, 426, 448]:
-        mi = (ctypes.c_ubyte * 128)(); mj = (ctypes.c_ubyte * 128)()
-        ncta = L.dba_solve_tile_placement(n, ctypes.cast(mi, ctypes.c_void_p), ctypes.cast(mj, ctypes.c_void_p))
-        nt = (n + 31) // 32
-        assert ncta in (1, 2, 4, 8, 16) and ncta >= nt and ncta * 8 >= nt * (nt + 1) // 2 + nt
-        seen = {}
-        for slot in range(128):
-            if mi[slot] == 0xFF:
-                continue
-            assert slot < ncta * 8
-            i, j = int(mi[slot]), int(mj[slot])
-            assert 0 <= j < nt and j <= i <= nt and (i, j) not in seen
-            seen[(i, j)] = slot // 8
-        assert set(seen) == {(i, j) for j in range(nt) for i in range(j, nt + 1)}
-        for (i, j), cta in seen.items():
-            if i == j:
-                assert cta == j
-            else:
-                assert cta > j or cta >= nt or cta == 0, (n, i, j, cta)
-    mi = (ctypes.c_ubyte * 128)(); mj = (ctypes.c_ubyte * 128)()
-    assert L.dba_solve_tile_placement(449, ctypes.cast(mi, ctypes.c_void_p), ctypes.cast(mj, ctypes.c_void_p)) == 0     # barrier kernel beyond 14 tile rows
