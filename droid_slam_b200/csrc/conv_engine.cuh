@@ -374,17 +374,12 @@ static int launch_conv_n(const ConvParams& p, const CUtensorMap& tA0, const CUte
   }
 }
 
-// one convolution launch.  src0 (+ optional src1) = channels-last sources concatenated along K; wpk = packed weights
-// [KS*KS][n_ntiles*N][Kpad] with Kpad = 64 * (kblocks(src0) + kblocks(src1)).
-// ROW_FLAT (the update operator): widths that are not a multiple of 8 take the row-flattened tiles of conv_tc_kernel where 2 halo
+// the tiling of one convolution (host only, no device query): fills the N tiles, TW, RM, MT, tiles_x / tiles_y, nk0 / nk1, boxn,
+// stage counts and sizes and slots of p from p.E, HT, WD, KS, N, n_ntiles, w_rows and the channel counts c0, c1 (0: no second source);
+// *flat = row-flattened tiles, *box_rows = halo box rows.
+// row_flat (the update operator): widths that are not a multiple of 8 take the row-flattened tiles of conv_tc_kernel where 2 halo
 // and 2 weight stages of them fit in shared memory; the rectangular tiles, correct at every width, run everywhere else.
-template <int EPI, bool ROW_FLAT = false>
-static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cudaStream_t st, int* slots_out = nullptr) {
-  if (!g_num_sms) {
-    int dev = 0; cudaGetDevice(&dev);
-    cudaDeviceProp prop; DBA_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties");
-    g_num_sms = prop.multiProcessorCount;
-  }
+static int conv_plan(ConvParams& p, int c0, int c1, bool row_flat, bool* flat_out, int* box_rows_out) {
   if (p.N > 256) {                // 384 outputs: two 192-wide N tiles (the register accumulator holds at most 256 columns)
     if (p.w_rows == 0) p.w_rows = p.n_ntiles * p.N;
     p.n_ntiles *= p.N / 192;
@@ -392,10 +387,10 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   }
   if (p.N % 32 != 0 || p.N < 32) { set_error("update operator: %d output channels per tile", p.N); return DBA_ERR_INVALID; }
   const int budget = 227 * 1024 - 2048;
-  const int nk = (s0.C + 63) / 64 + (s1.base ? (s1.C + 63) / 64 : 0);
+  const int nk = (c0 + 63) / 64 + (c1 + 63) / 64;
   int box_rows = 0;
   bool flat = false;
-  if constexpr (ROW_FLAT) {
+  if (row_flat) {
     if (p.WD % 8 != 0) {
       // row-flattened tiles (conv_tc_kernel): 128 MT consecutive pixels on the row pitch twp; the halo box spans the rows those
       // pixels touch from any start column c0 <= twp - 8, plus KS - 1 halo rows.  MT as for the rectangular tiles below.
@@ -425,8 +420,8 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
     p.tiles_y = (p.HT + p.MT * p.RM - 1) / (p.MT * p.RM);
     box_rows = p.MT * p.RM + p.KS - 1;
   }
-  p.nk0 = (s0.C + 63) / 64;
-  p.nk1 = s1.base ? (s1.C + 63) / 64 : 0;
+  p.nk0 = (c0 + 63) / 64;
+  p.nk1 = (c1 + 63) / 64;
   p.boxn = p.N;
   p.a_bytes = box_rows * p.TW * 128;
   p.b_bytes = p.N * 128;
@@ -438,10 +433,27 @@ static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cu
   if (p.b_stages > 8) p.b_stages = 8;
   if (p.b_stages < 2) { set_error("update operator: tile does not fit shared memory"); return DBA_ERR_INVALID; }
   p.slots = p.tiles_x * p.tiles_y * p.MT * kSlotsPerMTile;
+  *flat_out = flat;
+  *box_rows_out = box_rows;
+  return DBA_OK;
+}
+
+// one convolution launch.  src0 (+ optional src1) = channels-last sources concatenated along K; wpk = packed weights
+// [KS*KS][n_ntiles*N][Kpad] with Kpad = 64 * (kblocks(src0) + kblocks(src1)); tiled by conv_plan.
+template <int EPI, bool ROW_FLAT = false>
+static int launch_conv(ConvParams p, ConvSrc s0, ConvSrc s1, const void* wpk, cudaStream_t st, int* slots_out = nullptr) {
+  if (!g_num_sms) {
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceProp prop; DBA_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev), "cudaGetDeviceProperties");
+    g_num_sms = prop.multiProcessorCount;
+  }
+  bool flat = false;
+  int box_rows = 0;
+  int rc = conv_plan(p, s0.C, s1.base ? s1.C : 0, ROW_FLAT, &flat, &box_rows); if (rc) return rc;
   if (slots_out) *slots_out = p.slots;
   const int smem = p.a_stages * p.a_bytes + p.b_stages * p.b_bytes + 1024 + 256;
   CUtensorMap tA0, tA1, tW;
-  int rc = make_act_map(&tA0, s0.base, s0.C, s0.stride, p.WD, p.HT, p.E, p.TW, box_rows); if (rc) return rc;
+  rc = make_act_map(&tA0, s0.base, s0.C, s0.stride, p.WD, p.HT, p.E, p.TW, box_rows); if (rc) return rc;
   if (s1.base) { rc = make_act_map(&tA1, s1.base, s1.C, s1.stride, p.WD, p.HT, p.E, p.TW, box_rows); if (rc) return rc; }
   else tA1 = tA0;
   rc = make_weight_map(&tW, wpk, 64 * (p.nk0 + p.nk1), p.w_rows > 0 ? p.w_rows : p.n_ntiles * p.N, p.KS * p.KS, p.boxn); if (rc) return rc;

@@ -362,17 +362,26 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
   return DBA_OK;
 }
 
+// the shape checks dba_conv_nhwc and dba_conv_nhwc_plan share (c1 = 0: no second source)
+static int conv_nhwc_check_shape(int c0, int c1, int ht, int wd, int ksize, int n_out) {
+  DBA_CHECK_ARG(ht > 0 && wd > 0, "bad extents");
+  DBA_CHECK_ARG(ksize == 1 || ksize == 3, "kernel size must be 1 or 3");
+  DBA_CHECK_ARG(n_out >= 32 && n_out <= 384 && (n_out <= 256 ? n_out % 32 == 0 : n_out == 384), "n_out must be 32..256 (multiple of 32) or 384");
+  DBA_CHECK_ARG(c0 > 0 && c1 >= 0, "bad channel counts");
+  DBA_CHECK_ARG(c1 == 0 || c0 % 64 == 0, "with two sources the first must hold a multiple of 64 channels");
+  return DBA_OK;
+}
+
 // channels-last tensor-core convolution building block (the kernel behind every layer of dba_update_forward), exported for
 // tests and for callers that keep activations channels-last: out[e,y,x,n] = act(bias[n] + sum_{tap,k} src[e,y+dy,x+dx,k] w[tap][n][k]).
 // Any ht, wd > 0, tiled by the same rule as dba_update_forward.
 extern "C" int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* src1, int c1, int stride1, const void* wpk, const float* bias,
                              void* out, int out_stride, int n_images, int ht, int wd, int ksize, int n_out, int relu, dba_stream_t stream) {
   DBA_CHECK_ARG(src0 && wpk && bias && out, "null pointer");
-  DBA_CHECK_ARG(n_images >= 0 && ht > 0 && wd > 0, "bad extents");
-  DBA_CHECK_ARG(ksize == 1 || ksize == 3, "kernel size must be 1 or 3");
-  DBA_CHECK_ARG(n_out >= 32 && n_out <= 384 && (n_out <= 256 ? n_out % 32 == 0 : n_out == 384), "n_out must be 32..256 (multiple of 32) or 384");
-  DBA_CHECK_ARG(c0 > 0 && stride0 % 8 == 0 && stride0 >= c0 && (!src1 || (c1 > 0 && stride1 % 8 == 0 && stride1 >= c1)), "row pitches must be multiples of 8 elements and hold the channels");
-  DBA_CHECK_ARG(!src1 || c0 % 64 == 0, "with two sources the first must hold a multiple of 64 channels");
+  DBA_CHECK_ARG(n_images >= 0, "bad extents");
+  DBA_CHECK_ARG(!src1 || c1 > 0, "bad channel counts");
+  int rc = conv_nhwc_check_shape(c0, src1 ? c1 : 0, ht, wd, ksize, n_out); if (rc) return rc;
+  DBA_CHECK_ARG(stride0 % 8 == 0 && stride0 >= c0 && (!src1 || (stride1 % 8 == 0 && stride1 >= c1)), "row pitches must be multiples of 8 elements and hold the channels");
   DBA_CHECK_ARG(out_stride % 8 == 0 && out_stride >= n_out, "bad output stride");
   if (n_images == 0) return DBA_OK;
   ConvParams p;
@@ -380,4 +389,18 @@ extern "C" int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* 
   p.E = n_images; p.HT = ht; p.WD = wd; p.n_ntiles = 1; p.KS = ksize; p.N = n_out; p.bias = bias; p.relu = relu;
   p.out = (__half*)out; p.out_stride = out_stride;
   return launch_conv<EPI_STORE, true>(p, ConvSrc{src0, c0, stride0}, ConvSrc{src1, c1, stride1}, wpk, (cudaStream_t)stream);
+}
+
+extern "C" int dba_conv_nhwc_plan(int ht, int wd, int c0, int c1, int ksize, int n_out, int* plan) {
+  DBA_CHECK_ARG(plan, "null pointer");
+  int rc = conv_nhwc_check_shape(c0, c1, ht, wd, ksize, n_out); if (rc) return rc;
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.E = 1; p.HT = ht; p.WD = wd; p.n_ntiles = 1; p.KS = ksize; p.N = n_out;
+  bool flat = false;
+  int box_rows = 0;
+  rc = conv_plan(p, c0, c1, true, &flat, &box_rows); if (rc) return rc;
+  const int v[8] = {flat ? 1 : 0, p.TW, p.MT, p.N, p.n_ntiles, p.tiles_x * p.tiles_y, p.a_stages, p.b_stages};
+  memcpy(plan, v, sizeof(v));
+  return DBA_OK;
 }

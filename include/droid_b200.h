@@ -308,6 +308,11 @@ int dba_update_forward(const dba_update_args* a);
  * dba_update_forward. */
 int dba_conv_nhwc(const void* src0, int c0, int stride0, const void* src1, int c1, int stride1, const void* wpk, const float* bias,
                   void* out, int out_stride, int n_images, int ht, int wd, int ksize, int n_out, int relu, dba_stream_t stream);
+/* host only: the tiling dba_conv_nhwc launches for these extents (c1 = 0: no second source), computed by the same code.
+ * plan [8] = {row-flattened tiles (0 / 1), TW (tile width, or the row pitch of row-flattened tiles), MT (128-pixel M tiles per CTA
+ * tile), N tile width, number of N tiles, CTA tiles per image, halo stages, weight stages}.  DBA_ERR_INVALID for extents
+ * dba_conv_nhwc rejects. */
+int dba_conv_nhwc_plan(int ht, int wd, int c0, int c1, int ksize, int n_out, int* plan);
 
 /* ---- feature / context encoders (BasicEncoder) on the tensor cores ---------------------------------------------------
  * replaces BasicEncoder.forward (reference droid_slam/modules/extractor.py:183-198) for the two encoders DroidNet builds

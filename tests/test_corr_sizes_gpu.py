@@ -4,7 +4,6 @@ the c5 bench config (72x96) and the smallest legal ones (8x8, 9x13), plus 16x64 
 import pytest
 import torch
 
-import oracle
 from util import assert_bit_identical
 
 pytestmark = pytest.mark.gpu
@@ -33,15 +32,6 @@ def _cublas_pyramid(f1, f2):
     return pyr
 
 
-def _oracle_pyramid(f1, f2):
-    """oracle.corr_pyramid's four levels.  Below 16 pixels in ht or wd level 3 has one row or column, and the reference's constructor,
-    which pools once more after appending the last level, raises there; level 3 is therefore the floor 2x2 mean of level 2 here."""
-    pyr = oracle.corr_pyramid(f1, f2, 3)
-    E, ht, wd, h2, w2 = pyr[2].shape
-    l3 = torch.nn.functional.avg_pool2d(pyr[2].reshape(E * ht * wd, 1, h2, w2), 2, stride=2)
-    return pyr + [l3.view(E, ht, wd, h2 // 2, w2 // 2)]
-
-
 def _coords(E, ht, wd, seed):
     g = torch.Generator().manual_seed(seed)
     c = torch.stack([torch.rand(E, ht, wd, generator=g) * (wd + 10) - 5, torch.rand(E, ht, wd, generator=g) * (ht + 10) - 5], dim=1)
@@ -55,18 +45,17 @@ def _coords(E, ht, wd, seed):
 
 @pytest.mark.parametrize("ht, wd", SIZES)
 def test_volume_matches_oracle_and_cublas_pipeline(backends, ht, wd):
+    """the binding's volume against the reference's f16 cuBLAS + avg_pool2d pipeline, which rounds every level to fp16 before pooling
+    the next (the values themselves are held to fp64 in tests/test_tensor_core_fp64_gpu.py)"""
     N, E = 4, _edges(ht, wd)
     fm = _fmaps(ht, wd, N, 100 + ht * wd)
     g = torch.Generator().manual_seed(ht + wd)
     ii, jj = torch.randint(0, N, (E,), generator=g), torch.randint(0, N, (E,), generator=g)
     f = fm.to(dev)
     got = backends.corr_volume_pyramid(f, f, ii.to(dev), jj.to(dev))
-    ref = _oracle_pyramid(fm[None, ii].float(), fm[None, jj].float())            # fp32 math on the fp16 inputs
     lib = _cublas_pyramid(f[ii.to(dev)], f[jj.to(dev)])
     for l in range(4):
-        assert got[l].shape == (E, ht, wd, ht >> l, wd >> l) == ref[l].shape
-        err = float((got[l].float().cpu() - ref[l]).abs().max())
-        assert err < 2e-2 + 2e-3 * float(ref[l].abs().max()), (l, err)
+        assert got[l].shape == (E, ht, wd, ht >> l, wd >> l) == lib[l].shape
         assert float((got[l].float() - lib[l].float()).abs().max()) < 6e-2, l
 
 

@@ -1,6 +1,7 @@
 """The update operator (csrc/update_op.cu) at feature widths that are not a multiple of 8, where its convolutions run the row-flattened
 tiles of csrc/conv_engine.cuh: 1/8 of ETH3D through the reference's eval script (43x70), raw EuRoC through demo.py (44x69), 16:9 video
-through demo.py (41x73) and a tiny 9x13.  Tolerances are those of tests/test_update_gpu.py and of the other stages' own tests."""
+through demo.py (41x73) and a tiny 9x13.  Tolerances are those of tests/test_update_gpu.py and of the other stages' own tests; the
+single convolutions at these widths are held to fp64 in tests/test_tensor_core_fp64_gpu.py."""
 import ctypes
 import os
 import sys
@@ -48,31 +49,6 @@ def _conv_native(backends, x0, x1, wpk, b, ks, n, relu):
         c_api.check(L.dba_conv_nhwc(ptr(xd), 196, 200, None, 0, 0, ptr(wd_), ptr(bd), ptr(out), n, E, ht, wd, ks, n, int(relu), stream()), "conv_nhwc")
         return out
     return backends.conv_nhwc(x0.to(DEV), x1.to(DEV) if x1 is not None else None, wpk.to(DEV), b.to(DEV), ks, relu)
-
-
-@pytest.mark.parametrize("E,ht,wd,c0,c1,ks,n,relu", [
-    (12, 43, 70, 128, 0, 3, 128, True),      # 13 CTA tiles per image (MT = 2): 156 tiles, more than SMs
-    (12, 44, 69, 128, 320, 3, 256, False),   # two sources, N = 256 (MT = 1)
-    (6, 41, 73, 128, 0, 3, 384, True),       # N = 384: two 192-wide N tiles
-    (12, 44, 69, 200, 0, 1, 128, True),      # 1x1, 196 channels on a 200-element pitch (no halo rows)
-    (12, 43, 70, 128, 0, 3, 64, True),
-    (12, 41, 73, 64, 0, 3, 32, False),
-    (24, 41, 73, 256, 0, 1, 32, False),      # the eta head's shape
-    (3, 9, 13, 128, 0, 3, 128, True),        # one CTA tile, most of it past the image
-    (3, 9, 13, 64, 0, 1, 32, True),
-    (2, 12, 157, 128, 0, 3, 128, True),      # pitch 160: 2 halo + 2 weight stages do not fit -> rectangular tiles
-    (2, 6, 261, 64, 0, 3, 64, True),         # pitch 264 > the 256-pixel TMA box -> rectangular tiles
-])
-def test_conv_nhwc_odd_widths_match_torch_conv(backends, E, ht, wd, c0, c1, ks, n, relu):
-    x0, x1, w, b, wpk, cuse0 = _conv_case(E, ht, wd, c0, c1, ks, n, E * 1000 + ht + wd + n)
-    xin = x0[..., :cuse0] if x1 is None else torch.cat([x0, x1], -1)
-    ref = F.conv2d(xin.float().permute(0, 3, 1, 2), w.float(), b, padding=ks // 2)
-    if relu:
-        ref = F.relu(ref)
-    got = _conv_native(backends, x0, x1, wpk, b, ks, n, relu)
-    torch.cuda.synchronize()
-    err = float((got.float().cpu() - ref.permute(0, 2, 3, 1)).abs().max())
-    assert err < 6e-3, err
 
 
 @pytest.mark.parametrize("c0,c1,ks,n", [(128, 0, 3, 128), (128, 320, 3, 256), (128, 0, 3, 384), (256, 0, 1, 64)])

@@ -69,6 +69,72 @@ def frac_equal(a, b):
     return float((a == b).float().mean())
 
 
+F16_OVERFLOW = 65520.0          # the midpoint between 65504, the largest finite fp16, and 2^16: from here on round-to-nearest gives inf
+
+
+def f16_rounding_interval(h):
+    """for fp16 values h: the fp64 bounds (lo, hi) of the reals that round to h under round-to-nearest-even, and whether they belong to
+    it (h's significand even: ties round to h).  Computed exactly from h's exponent; ±0 -> ±2^-25; ±inf -> [65520, inf] and its negative
+    (NaN gives NaN bounds)."""
+    x = h.double()
+    a = x.abs()
+    m, e = torch.frexp(a)                                       # a = m 2^e, 0.5 <= m < 1
+    tiny = 2.0 ** -24
+    up = torch.ldexp(torch.ones_like(a), e - 11).clamp(min=tiny)                 # gap to the next larger magnitude
+    down = torch.where((m == 0.5) & (e - 1 > -14), up / 2, up)                     # a normal power of two above 2^-14: finer below
+    down = torch.where(a == 0, torch.full_like(a, tiny), down)
+    up = torch.where(a == 0, torch.full_like(a, tiny), up)
+    mag_lo, mag_hi = a - down / 2, a + up / 2
+    mag_lo = torch.where(a == 0, -mag_hi, mag_lo)                                  # zero: symmetric about 0
+    inf = torch.isinf(a)
+    mag_lo = torch.where(inf, torch.full_like(a, F16_OVERFLOW), mag_lo)
+    mag_hi = torch.where(inf, torch.full_like(a, float("inf")), mag_hi)
+    neg = torch.signbit(x) & (a != 0)
+    lo = torch.where(neg, -mag_hi, mag_lo)
+    hi = torch.where(neg, -mag_lo, mag_hi)
+    even = (h.view(torch.int16) & 1) == 0
+    return lo, hi, even | inf
+
+
+def faithful_f16(got, exact, beta):
+    """elementwise: is the fp16 value `got` round-to-nearest-even of some real in [exact - beta, exact + beta]?  Also returns the
+    distance from `exact` to the rounding interval of `got` (0 inside it; inf for NaN).  fp64 arithmetic on got's device."""
+    assert got.dtype == torch.float16 and got.shape == exact.shape == beta.shape, (got.dtype, got.shape, exact.shape, beta.shape)
+    exact = exact.to(got.device, torch.float64)
+    beta = beta.to(got.device, torch.float64)
+    lo, hi, closed = f16_rounding_interval(got)
+    a, b = exact - beta, exact + beta
+    ok = torch.where(closed, (lo <= b) & (hi >= a), (lo < b) & (hi > a))
+    ok &= ~torch.isnan(got) & ~torch.isnan(beta) & (beta >= 0)                     # NaN is never a rounding of a finite value
+    both_nan = torch.isnan(got) & torch.isnan(exact)
+    ok |= both_nan
+    dist = torch.clamp(torch.maximum(lo - exact, exact - hi), min=0)
+    dist = torch.where(torch.isnan(got), torch.full_like(dist, float("inf")), dist)
+    dist = torch.where(both_nan, torch.zeros_like(dist), dist)
+    return ok, dist
+
+
+def assert_faithful_f16(got, exact, beta, what="", unit=None):
+    """Every fp16 output h must equal round-to-nearest fp16 of some real in [exact - beta, exact + beta] (exact, beta: fp64 or anything
+    torch converts exactly; the expected value is never formed by a cast, which may round twice).  Returns (fraction of outputs equal
+    to the correctly rounded `exact`, smallest multiple of `unit` that would serve as beta -- the smallest passing kappa when
+    beta = kappa * unit; max dist / beta without a unit)."""
+    beta = torch.as_tensor(beta, dtype=torch.float64, device=got.device).expand(got.shape)
+    ok, dist = faithful_f16(got, exact, beta)
+    correct, _ = faithful_f16(got, exact, torch.zeros_like(beta))
+    scale = beta if unit is None else torch.as_tensor(unit, dtype=torch.float64, device=got.device).expand(got.shape)
+    need = torch.where(dist > 0, dist / scale, torch.zeros_like(dist))
+    worst = float(need.max()) if need.numel() else 0.0
+    frac = float(correct.double().mean()) if correct.numel() else 1.0
+    if not bool(ok.all()):
+        bad = (~ok).nonzero()
+        first = [tuple(int(v) for v in i) for i in bad[:4].tolist()]
+        detail = ["%s: got %r exact %.9g beta %.3g" % (i, float(got[i]), float(exact[i]), float(beta[i])) for i in first]
+        raise AssertionError("%s: %d of %d fp16 outputs are not a rounding of a value within beta of the fp64 reference (needs %.3g); %s"
+                             % (what, bad.shape[0], got.numel(), worst, "; ".join(detail)))
+    return frac, worst
+
+
 def assert_bit_identical(a, b, what=""):
     """torch.equal with a useful message (how many elements differ and by how much)"""
     a = a.cpu(); b = b.cpu()
