@@ -13,7 +13,7 @@ SYMBOLS = [
     "dba_ba_workspace_bytes", "dba_ba_system_offset", "dba_ba_system_bytes",
     "dba_ba_prepare", "dba_ba_build", "dba_ba_solve", "dba_ba", "dba_ba_read_info", "dba_ba_p2p_signal",
     "dba_solve_workspace_bytes", "dba_solve_spd", "dba_solve_tile_placement",
-    "dba_update_workspace_bytes", "dba_update_forward", "dba_conv_nhwc", "dba_conv_nhwc_plan", "dba_encoder_workspace_bytes", "dba_encoder_forward", "dba_proximity_workspace_bytes", "dba_proximity_edges",
+    "dba_update_workspace_bytes", "dba_update_workspace_layout", "dba_update_forward", "dba_conv_nhwc", "dba_conv_nhwc_plan", "dba_encoder_workspace_bytes", "dba_encoder_forward", "dba_proximity_workspace_bytes", "dba_proximity_edges",
     "dba_fill_interpolate", "dba_pose_only_ba",
 ]
 
@@ -73,6 +73,7 @@ def load():
     L.dba_graph_writeback.argtypes = [vp] * 4 + [ci] + [vp] * 4 + [ci] + [vp, vp, ci, vp, vp, ci, vp, cf, ci, ci, vp]
     L.dba_update_workspace_bytes.restype = ctypes.c_size_t
     L.dba_update_workspace_bytes.argtypes = [ci] * 4
+    L.dba_update_workspace_layout.argtypes = [ci] * 4 + [vp, vp]
     L.dba_frame_distance.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, cf, vp]
     L.dba_depth_filter.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp]
     L.dba_iproj.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp]

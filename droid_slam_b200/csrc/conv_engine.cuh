@@ -42,6 +42,8 @@ struct ConvParams {
 
 __device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
+// ReLU that keeps NaN, like torch.relu: fmaxf alone would turn a NaN input into 0 and hide it from every later stage
+__device__ __forceinline__ float relu_nan(float x) { return isnan(x) ? x : fmaxf(x, 0.f); }
 __device__ __forceinline__ float2 unpack2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
 
 __device__ __forceinline__ float2 ldh2(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
@@ -76,7 +78,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvParams& p, const float (
       const int c = 8 * j + 2 * qd;
       float v0 = acc[4 * j + 2 * i] + __ldg(bias + c), v1 = acc[4 * j + 2 * i + 1] + __ldg(bias + c + 1);
       if (EPI == EPI_STORE) {
-        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (p.relu) { v0 = relu_nan(v0); v1 = relu_nan(v1); }
         if (valid) *reinterpret_cast<uint32_t*>(p.out + pix * p.out_stride + nt * p.N + c) = pack_h2(v0, v1);
       } else if (EPI == EPI_GATE) {
         float g0 = 0.f, g1 = 0.f;

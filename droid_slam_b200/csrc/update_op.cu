@@ -209,8 +209,10 @@ __global__ void __launch_bounds__(256) segment_mean_kernel(const __half* __restr
 
 static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
+// byte offsets of the intermediates in the caller's workspace; yh ([E,HW,36] f32 head partials) reuses cc and ye ([n_src,HW,12] f32
+// eta partials) reuses f0, both dead by then.  The fields up to b2 are in the order of DBA_UPWS_* (droid_b200.h).
 struct UpWs {
-  size_t hin, x320, cc, f0, c1, f1, z, rh, s, partial, glo, am, b2, segptr, segedges, total;
+  size_t hin, x320, cc, f0, c1, f1, z, rh, s, partial, glo, am, b2, yh, ye, segptr, segedges, total;
 };
 static UpWs up_layout(int E, int n_src, int ht, int wd) {
   UpWs w;
@@ -237,11 +239,23 @@ static UpWs up_layout(int E, int n_src, int ht, int wd) {
   w.glo = o; o += al256((size_t)E * 384 * 4);
   w.am = o; o += al256(spx * 128 * 2);
   w.b2 = o; o += al256(spx * 128 * 2);
+  w.yh = w.cc;
+  w.ye = w.f0;
   w.segptr = o; o += al256((size_t)(n_src + 2) * 4);
   w.segedges = o; o += al256((size_t)(E + 1) * 4);
   w.total = o;
   return w;
 }
+
+// the extents every convolution of the operator starts from, and the ConvGRU gate convolution (1x1 128 -> 128, EPI_GATE) built on
+// them: dba_update_forward launches it and dba_update_workspace_layout plans it, so both count the same partial-sum slots
+static ConvParams up_base(int E, int ht, int wd) {
+  ConvParams p;
+  memset(&p, 0, sizeof(p));
+  p.E = E; p.HT = ht; p.WD = wd; p.n_ntiles = 1;
+  return p;
+}
+static ConvParams gate_conv(const ConvParams& base) { ConvParams p = base; p.KS = 1; p.N = 128; return p; }
 
 }  // namespace dba
 using namespace dba;
@@ -249,6 +263,20 @@ using namespace dba;
 extern "C" size_t dba_update_workspace_bytes(int n_edges, int n_src, int ht, int wd) {
   if (n_edges <= 0 || ht <= 0 || wd <= 0) return 0;
   return up_layout(n_edges, n_src, ht, wd).total;
+}
+
+extern "C" int dba_update_workspace_layout(int n_edges, int n_src, int ht, int wd, size_t* offsets, int* gate_slots) {
+  DBA_CHECK_ARG(offsets && gate_slots, "null pointer");
+  DBA_CHECK_ARG(n_edges > 0 && ht > 0 && wd > 0 && n_src >= 0, "bad extents");
+  const UpWs L = up_layout(n_edges, n_src, ht, wd);
+  const size_t v[DBA_UPWS_COUNT] = {L.hin, L.x320, L.cc, L.f0, L.c1, L.f1, L.z, L.rh, L.s, L.partial, L.glo, L.am, L.b2, L.yh, L.ye};
+  memcpy(offsets, v, sizeof(v));
+  ConvParams p = gate_conv(up_base(n_edges, ht, wd));
+  bool flat = false;
+  int box_rows = 0;
+  int rc = conv_plan(p, 128, 0, true, &flat, &box_rows); if (rc) return rc;
+  *gate_slots = p.slots;
+  return DBA_OK;
 }
 
 extern "C" int dba_update_forward(const dba_update_args* a) {
@@ -304,9 +332,7 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
   flow_im2col_kernel<<<dim3((wd + 63) / 64, ht, E), 256, 0, st>>>(a->flow, F0, ht, wd);
   DBA_CHECK_LAUNCH("update layout kernels");
 
-  ConvParams base;
-  memset(&base, 0, sizeof(base));
-  base.E = E; base.HT = ht; base.WD = wd; base.n_ntiles = 1;
+  const ConvParams base = up_base(E, ht, wd);
   const ConvSrc none = {nullptr, 0, 0};
   int rc;
   // ---- corr_encoder: 1x1 196->128 + ReLU, 3x3 128->128 + ReLU -> X[:, 128:256]   (droid_net.py:83-87)
@@ -321,7 +347,7 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
     rc = launch_conv<EPI_STORE, true>(p, ConvSrc{F1, 128, 128}, none, W->w_flow2, st); if (rc) return rc; }
   // ---- ConvGRU (gru.py:19-32): global context
   int slots = 0;
-  { ConvParams p = base; p.KS = 1; p.N = 128; p.bias = W->b_gate; p.h = H; p.h_stride = 128; p.partial = partial;
+  { ConvParams p = gate_conv(base); p.bias = W->b_gate; p.h = H; p.h_stride = 128; p.partial = partial;
     rc = launch_conv<EPI_GATE, true>(p, ConvSrc{H, 128, 128}, none, W->w_gate, st, &slots); if (rc) return rc; }
   glo_kernel<<<E, 384, 0, st>>>(partial, slots, 1.f / (float)HW, W->w_glo, W->b_glo, glo);
   DBA_CHECK_LAUNCH("glo_kernel");
@@ -338,7 +364,7 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
     rc = launch_conv<EPI_STORE, true>(p, ConvSrc{a->net_out, 128, 128}, none, W->w_stem, st); if (rc) return rc; }
   // delta.2 and weight.2 (3x3 128->2 each): per-tap partial sums by one 1x1 convolution 256 -> 36 (block-diagonal weights), then the
   // 9-tap gather with bias / sigmoid
-  float* Yh = (float*)(ws + L.cc);                        // [E,HW,36] f32 on the (dead) corr staging buffer
+  float* Yh = (float*)(ws + L.yh);                        // [E,HW,36] f32 on the (dead) corr staging buffer
   { ConvParams p = base; p.KS = 1; p.N = 64; p.bias = W->b_zero; p.f32a = Yh; p.f32_cols = 36; p.f32_stride = 36;
     rc = launch_conv<EPI_F32, true>(p, ConvSrc{S, 256, 384}, none, W->w_heads, st); if (rc) return rc; }
   head_gather_kernel<<<(unsigned)(((size_t)E * HW + 255) / 256), 256, 0, st>>>(Yh, 36, 4, W->b_heads, 0, a->delta, a->weight, E, ht, wd);
@@ -351,7 +377,7 @@ extern "C" int dba_update_forward(const dba_update_args* a) {
     ConvParams fb = base; fb.E = n_src;
     { ConvParams p = fb; p.KS = 3; p.N = 128; p.bias = W->b_agg2; p.relu = 1; p.out = B2; p.out_stride = 128;
       rc = launch_conv<EPI_STORE, true>(p, ConvSrc{Am, 128, 128}, none, W->w_agg2, st); if (rc) return rc; }
-    float* Ye = (float*)(ws + L.f0);                      // [n_src,HW,12] f32 (9 used) on the (dead) flow im2col buffer
+    float* Ye = (float*)(ws + L.ye);                      // [n_src,HW,12] f32 (9 used) on the (dead) flow im2col buffer
     { ConvParams p = fb; p.KS = 1; p.N = 32; p.bias = W->b_zero; p.f32a = Ye; p.f32_cols = 12; p.f32_stride = 12;
       rc = launch_conv<EPI_F32, true>(p, ConvSrc{B2, 128, 128}, none, W->w_eta, st); if (rc) return rc; }
     head_gather_kernel<<<(unsigned)(((size_t)n_src * HW + 255) / 256), 256, 0, st>>>(Ye, 12, 1, W->b_eta, 1, a->eta, nullptr, n_src, ht, wd);

@@ -301,6 +301,20 @@ typedef struct {
 size_t dba_update_workspace_bytes(int n_edges, int n_src, int ht, int wd);
 int dba_update_forward(const dba_update_args* a);
 
+/* host only: where dba_update_forward leaves its intermediates in the workspace, from the layout it uses itself (for tests that
+ * check each stage on the inputs the previous one wrote).  offsets[DBA_UPWS_COUNT] = byte offsets from the workspace start of:
+ *   HIN  f16 [E,HW,128]  hidden state, channels-last (written for net_layout 0 only)
+ *   X320 f16 [E,HW,320]  inp | corr encoder | flow encoder          CC   f16 [E,HW,200]  corr, channels-last (196 used)
+ *   F0   f16 [E,HW,200]  7x7 im2col of flow (196 used)               C1, F1 f16 [E,HW,128]  first corr / flow encoder layers
+ *   Z, RH f16 [E,HW,128] GRU z and r*h                               S    f16 [E,HW,384]  stems delta.0 | weight.0 | agg.conv1
+ *   PARTIAL f32 [E,gate_slots,128]  sums of sigmoid(gru.w(h)) * h over 16-pixel slots            GLO f32 [E,384]  z | r | q terms
+ *   AM, B2 f16 [n_src,HW,128]  segment mean of agg.conv1, agg.conv2
+ *   YH f32 [E,HW,36]   per-tap partials of delta.2 / weight.2 (reuses CC)    YE f32 [n_src,HW,12]  of agg.eta.0, 9 used (reuses F0)
+ * *gate_slots = the partial-sum slots glo_kernel adds per edge.  DBA_ERR_INVALID for extents dba_update_forward rejects. */
+enum { DBA_UPWS_HIN, DBA_UPWS_X320, DBA_UPWS_CC, DBA_UPWS_F0, DBA_UPWS_C1, DBA_UPWS_F1, DBA_UPWS_Z, DBA_UPWS_RH, DBA_UPWS_S,
+       DBA_UPWS_PARTIAL, DBA_UPWS_GLO, DBA_UPWS_AM, DBA_UPWS_B2, DBA_UPWS_YH, DBA_UPWS_YE, DBA_UPWS_COUNT };
+int dba_update_workspace_layout(int n_edges, int n_src, int ht, int wd, size_t* offsets, int* gate_slots);
+
 /* the building block of dba_update_forward, exported: 1x1 / 3x3 'same' convolution of channels-last f16 activations on the tensor
  * cores.  src0 (+ optional src1, concatenated along channels after src0) [n_images,ht,wd,stride] using channels [0,c); wpk f16
  * [ksize*ksize][n_out][Kpad] with Kpad = 64*ceil(c0/64) + 64*ceil(c1/64), K contiguous; bias f32 [n_out]; out f16

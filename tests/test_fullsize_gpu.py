@@ -41,14 +41,18 @@ def test_corr_index_full_size_properties(backends, metric_scene, dtype):
             assert float(d.max()) <= 2e-3 * float(out2.float().abs().max())
         outc = torch.cat([backends.corr_index_forward(vol[a:a + 64], c[a:a + 64].contiguous(), 3)[0] for a in range(0, E, 64)])
         assert torch.equal(outc, out)
-    # (c) adjointness of forward/backward at level 2 (f32 only: sums are exact enough)
+    # (c) adjointness of forward/backward at level 2 (f32 only: sums are exact enough).  <fwd, g> and <vol, bwd> are the same sum in
+    # exact arithmetic; what separates them is the fp32 rounding of each fwd and bwd element, which cancels at random.  So the bound is
+    # a fraction of u times the size of the terms, not of |<fwd, g>|: that sum has random sign and is near zero for some g (on an H100,
+    # |a - b| stays below 1e-3 u sum |fwd g| over 12 seeds).  g has its own generator, so the result does not depend on test order.
     if dtype == torch.float32:
         vol = pyr[2]; c = (coords / 4).contiguous()
-        g = torch.randn(E, 7, 7, 48, 64, device=dev)
+        g = torch.randn(E, 7, 7, 48, 64, device=dev, generator=torch.Generator(device=dev).manual_seed(0))
         fwd, = backends.corr_index_forward(vol, c, 3)
         bwd, = backends.corr_index_backward(vol, c, g, 3)
         a = float((fwd.double() * g.double()).sum()); b = float((vol.double() * bwd.double()).sum())
-        assert abs(a - b) <= 1e-5 * max(abs(a), 1.0)
+        terms = float((fwd.double() * g.double()).abs().sum())
+        assert abs(a - b) <= 0.01 * 2.0 ** -24 * terms, (a, b, terms)
 
 
 def test_ba_full_size_matches_oracle_and_descends(backends, metric_scene):

@@ -102,18 +102,19 @@ def _report(kind, name, stats):
 
 
 class Guarded:
-    """a NaN-filled fp16 buffer holding `shape` with GUARD elements of NaN before and after it"""
+    """a NaN-filled fp16 (or fp32) buffer holding `shape` with GUARD elements of NaN before and after it"""
 
-    def __init__(self, *shape):
+    def __init__(self, *shape, dtype=torch.float16):
         n = 1
         for s in shape:
             n *= s
-        self.buf = torch.full((n + 2 * GUARD,), float("nan"), dtype=torch.float16, device=dev)
-        self.fill = self.buf[:1].view(torch.int16).clone()
+        self.bits = torch.int16 if dtype == torch.float16 else torch.int32
+        self.buf = torch.full((n + 2 * GUARD,), float("nan"), dtype=dtype, device=dev)
+        self.fill = self.buf[:1].view(self.bits).clone()
         self.t = self.buf[GUARD:GUARD + n].view(*shape)
 
     def untouched(self, region):
-        return bool((region.contiguous().view(torch.int16) == self.fill).all())
+        return bool((region.contiguous().view(self.bits) == self.fill).all())
 
     def check_guards(self, what):
         assert self.untouched(self.buf[:GUARD]) and self.untouched(self.buf[-GUARD:]), "%s wrote outside its output" % what
