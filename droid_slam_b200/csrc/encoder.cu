@@ -13,6 +13,7 @@
 //   * no norm (cnet): the epilogue EPI_RELU_RES applies the ReLU and the residual relu(x + relu(acc + bias)); no separate pass;
 //   * conv2 (1x1 128 -> output_dim) writes NCHW f16 through EPI_NCHW.
 #include "conv_engine.cuh"
+#include <limits.h>
 
 namespace dba {
 
@@ -122,8 +123,8 @@ __global__ void __launch_bounds__(256) inorm_act_kernel(const __half* __restrict
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       const float2 f = unpack2(uw[k]), m0 = m[2 * k], m1 = m[2 * k + 1];
-      v[2 * k] = fmaxf((f.x - m0.x) * m0.y, 0.f);
-      v[2 * k + 1] = fmaxf((f.y - m1.x) * m1.y, 0.f);
+      v[2 * k] = relu_nan1((f.x - m0.x) * m0.y);
+      v[2 * k + 1] = relu_nan1((f.y - m1.x) * m1.y);
     }
   }
   if (b) {
@@ -147,7 +148,7 @@ __global__ void __launch_bounds__(256) inorm_act_kernel(const __half* __restrict
     }
   }
 #pragma unroll
-  for (int k = 0; k < 8; k++) v[k] = fmaxf(v[k], 0.f);
+  for (int k = 0; k < 8; k++) v[k] = relu_nan1(v[k]);
   *reinterpret_cast<uint4*>(out + pix * out_stride + c) = make_uint4(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]), pack_h2(v[4], v[5]), pack_h2(v[6], v[7]));
 }
 
@@ -162,7 +163,7 @@ static size_t enc_slot_bound(int ht, int wd) {
   return (size_t)((wd + tw - 1) / tw) * ((ht + rm - 1) / rm) * kSlotsPerMTile * 2;
 }
 
-struct EncWs { size_t big, act[4], partial, counts, ms[2], total; };
+struct EncWs { size_t big, act[4], partial, counts, ms[2], total, big_bytes, act_bytes, partial_bytes, counts_bytes, ms_bytes; };
 static EncWs enc_layout(int E, int H, int W) {
   EncWs L;
   const int h1 = H / 2, w1 = W / 2, h2 = H / 4, w2 = W / 4, h3 = H / 8, w3 = W / 8;
@@ -174,11 +175,16 @@ static EncWs enc_layout(int E, int H, int W) {
   if (enc_slot_bound(h2, w2) * 128 > stat_cols) stat_cols = enc_slot_bound(h2, w2) * 128;
   if (enc_slot_bound(h3, w3) * 256 > stat_cols) stat_cols = enc_slot_bound(h3, w3) * 256;
   size_t o = 0;
-  L.big = o; o += enc_al256(big * 2);
-  for (int k = 0; k < 4; k++) { L.act[k] = o; o += enc_al256(px1 * 32 * 2); }   // the largest activation: [E][H/2][W/2][32] = [E][H/4][W/4][128]
-  L.partial = o; o += enc_al256((size_t)E * stat_cols * 2 * 4);
-  L.counts = o; o += enc_al256((size_t)E * enc_slot_bound(h1, w1) * 4);
-  for (int k = 0; k < 2; k++) { L.ms[k] = o; o += enc_al256((size_t)E * 256 * 8); }
+  L.big_bytes = enc_al256(big * 2);
+  L.act_bytes = enc_al256(px1 * 32 * 2);                           // the largest activation: [E][H/2][W/2][32] = [E][H/4][W/4][128]
+  L.partial_bytes = enc_al256((size_t)E * stat_cols * 2 * 4);
+  L.counts_bytes = enc_al256((size_t)E * enc_slot_bound(h1, w1) * 4);
+  L.ms_bytes = enc_al256((size_t)E * 256 * 8);
+  L.big = o; o += L.big_bytes;
+  for (int k = 0; k < 4; k++) { L.act[k] = o; o += L.act_bytes; }
+  L.partial = o; o += L.partial_bytes;
+  L.counts = o; o += L.counts_bytes;
+  for (int k = 0; k < 2; k++) { L.ms[k] = o; o += L.ms_bytes; }
   L.total = o;
   return L;
 }
@@ -188,11 +194,18 @@ struct Enc {
   cudaStream_t st;
   float* partial;
   float* counts;
+  int limit;        // launches to run: the schedule stops launching after this many (dba_encoder_forward_prefix; 0 plans only)
+  int launches;     // launches the schedule has reached so far
+  int* plans;       // when set: [DBA_ENCODER_CONVS][5] = TW, MT, tiles_x, tiles_y, EPI_STATS slots (0 without statistics) per convolution
+  int convs;        // convolutions reached so far
 };
+
+// every launch of the schedule asks this first, so a prefix and the launch count come from the one schedule
+static bool enc_next(Enc& c) { return c.launches++ < c.limit; }
 
 // one convolution of the encoder (E images of ht x wd, channels-last source)
 template <int EPI>
-static int enc_conv(const Enc& c, int ht, int wd, int ks, ConvSrc src, const void* w, const float* b, int N, __half* out, int out_stride,
+static int enc_conv(Enc& c, int ht, int wd, int ks, ConvSrc src, const void* w, const float* b, int N, __half* out, int out_stride,
                     int relu_cols = 0, const __half* res = nullptr, int res_stride = 0, int* slots = nullptr) {
   ConvParams p;
   memset(&p, 0, sizeof(p));
@@ -200,22 +213,34 @@ static int enc_conv(const Enc& c, int ht, int wd, int ks, ConvSrc src, const voi
   p.out = out; p.out_stride = out_stride; p.relu_cols = relu_cols; p.h = res; p.h_stride = res_stride;
   p.partial = c.partial; p.counts = c.counts;
   if (EPI == EPI_NCHW) { p.nchw = out; p.nchw_C = N; }
-  return launch_conv<EPI>(p, src, ConvSrc{nullptr, 0, 0}, w, c.st, slots);
+  const int k = c.convs++;
+  if (enc_next(c)) return launch_conv<EPI>(p, src, ConvSrc{nullptr, 0, 0}, w, c.st, slots);
+  bool flat = false;
+  int box_rows = 0;
+  const int rc = conv_plan(p, src.C, 0, false, &flat, &box_rows); if (rc) return rc;      // the tiling launch_conv would take
+  if (slots) *slots = p.slots;
+  if (c.plans) {
+    const int v[5] = {p.TW, p.MT, p.tiles_x, p.tiles_y, EPI == EPI_STATS ? p.slots : 0};
+    memcpy(c.plans + 5 * k, v, sizeof(v));
+  }
+  return DBA_OK;
 }
 
 // convolution + instance-norm statistics: raw f16 output in out, ms[e*N + n] = (mean, rstd)
-static int enc_conv_stats(const Enc& c, int ht, int wd, int ks, ConvSrc src, const void* w, const float* b, int N, __half* out, float2* ms) {
+static int enc_conv_stats(Enc& c, int ht, int wd, int ks, ConvSrc src, const void* w, const float* b, int N, __half* out, float2* ms) {
   int slots = 0;
   int rc = enc_conv<EPI_STATS>(c, ht, wd, ks, src, w, b, N, out, N, 0, nullptr, 0, &slots);
   if (rc) return rc;
+  if (!enc_next(c)) return DBA_OK;
   inorm_finalize_kernel<<<dim3(N / 32, c.E), dim3(32, 32), 0, c.st>>>(c.partial, c.counts, slots, N, ms);
   DBA_CHECK_LAUNCH("inorm_finalize_kernel");
   return DBA_OK;
 }
 
-static int enc_act(const Enc& c, const __half* a, int a_stride, const float2* ms_a, int msa_stride, const __half* b, int b_stride, const float2* ms_b,
+static int enc_act(Enc& c, const __half* a, int a_stride, const float2* ms_a, int msa_stride, const __half* b, int b_stride, const float2* ms_b,
                    int msb_stride, const __half* x, int x_stride, __half* out, int out_stride, int C, int HW) {
   const long long total = (long long)c.E * HW * (C / 8);
+  if (!enc_next(c)) return DBA_OK;
   inorm_act_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c.st>>>(a, a_stride, ms_a, msa_stride, b, b_stride, ms_b, msb_stride, x, x_stride, out,
                                                                      out_stride, C, HW, total);
   DBA_CHECK_LAUNCH("inorm_act_kernel");
@@ -223,7 +248,7 @@ static int enc_act(const Enc& c, const __half* a, int a_stride, const float2* ms
 }
 
 // ResidualBlock(P, P, stride 1) (extractor.py:47-55) on X [E][ht][wd][P], result written back into X; T1, T2 scratch
-static int enc_block_s1(const Enc& c, bool inorm, int ht, int wd, int P, __half* X, __half* T1, __half* T2, float2* msA, float2* msB,
+static int enc_block_s1(Enc& c, bool inorm, int ht, int wd, int P, __half* X, __half* T1, __half* T2, float2* msA, float2* msB,
                         const void* w1, const float* b1, const void* w2, const float* b2) {
   int rc;
   if (inorm) {
@@ -238,12 +263,14 @@ static int enc_block_s1(const Enc& c, bool inorm, int ht, int wd, int P, __half*
 
 // ResidualBlock(Cin, P, stride 2) on X [E][ht][wd][Cin] -> X [E][ht/2][wd/2][P].  conv1 and the downsample are one GEMM on the gathered
 // taps, output T1 [.][2P] = conv1 | downsample; T2 scratch
-static int enc_block_s2(const Enc& c, bool inorm, int ht, int wd, int Cin, int P, __half* X, __half* big, __half* T1, __half* T2, float2* msA, float2* msB,
+static int enc_block_s2(Enc& c, bool inorm, int ht, int wd, int Cin, int P, __half* X, __half* big, __half* T1, __half* T2, float2* msA, float2* msB,
                         const void* w1, const float* b1, const void* w2, const float* b2) {
   const int ho = ht / 2, wo = wd / 2;
   const long long total = (long long)c.E * ho * wo * 9 * (Cin / 8);
-  s2_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c.st>>>(X, big, Cin, ht, wd, total);
-  DBA_CHECK_LAUNCH("s2_gather_kernel");
+  if (enc_next(c)) {
+    s2_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c.st>>>(X, big, Cin, ht, wd, total);
+    DBA_CHECK_LAUNCH("s2_gather_kernel");
+  }
   const ConvSrc taps{big, 9 * Cin, 9 * Cin};
   int rc;
   if (inorm) {
@@ -256,28 +283,12 @@ static int enc_block_s2(const Enc& c, bool inorm, int ht, int wd, int Cin, int P
   return enc_conv<EPI_RELU_RES>(c, ho, wo, 3, ConvSrc{T1, P, 2 * P}, w2, b2, P, X, P, P, T1 + P, 2 * P);
 }
 
-}  // namespace dba
-using namespace dba;
-
-extern "C" size_t dba_encoder_workspace_bytes(int n_images, int H, int W, int output_dim) {
-  if (n_images < 1 || H <= 0 || W <= 0 || H % 8 || W % 8 || (output_dim != 128 && output_dim != 256)) return 0;
-  return enc_layout(n_images, H, W).total;
-}
-
-extern "C" int dba_encoder_forward(const dba_encoder_args* a) {
-  DBA_CHECK_ARG(a, "null args");
+// the schedule of both encoders: launches its first `limit` kernels (limit 0: none, the tilings and the launch count only, with a
+// null workspace) and reports how many it has in all and, in plans, each convolution's tiling
+static int enc_forward(const dba_encoder_args* a, int limit, int* n_launches, int* plans) {
   const int E = a->n_images, H = a->H, W = a->W;
-  DBA_CHECK_ARG(E > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, "encoder: n_images must be positive and H, W positive multiples of 8");
-  DBA_CHECK_ARG(a->norm == 0 || a->norm == 1, "encoder: norm must be 0 (none) or 1 (instance)");
-  DBA_CHECK_ARG(a->output_dim == 128 || a->output_dim == 256, "encoder: output_dim must be 128 or 256");
-  DBA_CHECK_ARG(a->images_dtype == DBA_F32 || a->images_dtype == DBA_F16, "encoder: images must be DBA_F32 or DBA_F16");
-  DBA_CHECK_ARG(a->images && a->weights && a->out && a->workspace, "null pointer");
   const dba_encoder_weights* Wt = a->weights;
-  for (int k = 0; k < DBA_ENCODER_CONVS; k++)
-    DBA_CHECK_ARG(Wt->w[k] && Wt->b[k] && ((uintptr_t)Wt->w[k] & 15) == 0, "encoder: packed weights must be non-null, w[k] 16-byte aligned");
   const EncWs L = enc_layout(E, H, W);
-  if (a->workspace_bytes < L.total) { set_error("invalid argument: workspace too small (dba_encoder_workspace_bytes)"); return DBA_ERR_WORKSPACE; }
-  DBA_CHECK_ARG(((uintptr_t)a->workspace & 255) == 0, "encoder: workspace must be 256-byte aligned");
   cudaStream_t st = (cudaStream_t)a->stream;
   uint8_t* ws = (uint8_t*)a->workspace;
   __half* big = (__half*)(ws + L.big);
@@ -286,15 +297,17 @@ extern "C" int dba_encoder_forward(const dba_encoder_args* a) {
   __half* T2 = (__half*)(ws + L.act[2]);
   float2* msA = (float2*)(ws + L.ms[0]);
   float2* msB = (float2*)(ws + L.ms[1]);
-  const Enc c{E, st, (float*)(ws + L.partial), (float*)(ws + L.counts)};
+  Enc c{E, st, (float*)(ws + L.partial), (float*)(ws + L.counts), limit, 0, plans, 0};
   const bool inorm = a->norm == 1;
   const int h1 = H / 2, w1 = W / 2;
   int rc;
   // conv1 7x7/2 3->32, norm1, relu1 (extractor.py:187-189)
-  const dim3 g((w1 + 63) / 64, h1, E);
-  if (a->images_dtype == DBA_F32) image_im2col_kernel<float><<<g, 256, 0, st>>>((const float*)a->images, big, H, W);
-  else image_im2col_kernel<__half><<<g, 256, 0, st>>>((const __half*)a->images, big, H, W);
-  DBA_CHECK_LAUNCH("image_im2col_kernel");
+  if (enc_next(c)) {
+    const dim3 g((w1 + 63) / 64, h1, E);
+    if (a->images_dtype == DBA_F32) image_im2col_kernel<float><<<g, 256, 0, st>>>((const float*)a->images, big, H, W);
+    else image_im2col_kernel<__half><<<g, 256, 0, st>>>((const __half*)a->images, big, H, W);
+    DBA_CHECK_LAUNCH("image_im2col_kernel");
+  }
   const ConvSrc stem{big, kStemTaps, kStemPitch};
   if (inorm) {
     if ((rc = enc_conv_stats(c, h1, w1, 1, stem, Wt->w[0], Wt->b[0], 32, T1, msA))) return rc;
@@ -310,5 +323,51 @@ extern "C" int dba_encoder_forward(const dba_encoder_args* a) {
   if ((rc = enc_block_s2(c, inorm, H / 4, W / 4, 64, 128, X, big, T1, T2, msA, msB, Wt->w[9], Wt->b[9], Wt->w[10], Wt->b[10]))) return rc;
   if ((rc = enc_block_s1(c, inorm, H / 8, W / 8, 128, X, T1, T2, msA, msB, Wt->w[11], Wt->b[11], Wt->w[12], Wt->b[12]))) return rc;
   // conv2 1x1 128->output_dim, NCHW f16 (:195)
-  return enc_conv<EPI_NCHW>(c, H / 8, W / 8, 1, ConvSrc{X, 128, 128}, Wt->w[13], Wt->b[13], a->output_dim, (__half*)a->out, 0);
+  rc = enc_conv<EPI_NCHW>(c, H / 8, W / 8, 1, ConvSrc{X, 128, 128}, Wt->w[13], Wt->b[13], a->output_dim, (__half*)a->out, 0);
+  if (n_launches) *n_launches = c.launches;
+  return rc;
 }
+
+}  // namespace dba
+using namespace dba;
+
+extern "C" size_t dba_encoder_workspace_bytes(int n_images, int H, int W, int output_dim) {
+  if (n_images < 1 || H <= 0 || W <= 0 || H % 8 || W % 8 || (output_dim != 128 && output_dim != 256)) return 0;
+  return enc_layout(n_images, H, W).total;
+}
+
+extern "C" int dba_encoder_workspace_layout(int n_images, int H, int W, int norm, size_t* offsets, size_t* sizes, int* n_launches, int* plans) {
+  DBA_CHECK_ARG(offsets && sizes && n_launches && plans, "null pointer");
+  DBA_CHECK_ARG(n_images > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, "encoder: n_images must be positive and H, W positive multiples of 8");
+  DBA_CHECK_ARG(norm == 0 || norm == 1, "encoder: norm must be 0 (none) or 1 (instance)");
+  const EncWs L = enc_layout(n_images, H, W);
+  const size_t off[DBA_ENCWS_COUNT] = {L.big, L.act[0], L.act[1], L.act[2], L.partial, L.counts, L.ms[0], L.ms[1]};
+  const size_t sz[DBA_ENCWS_COUNT] = {L.big_bytes, L.act_bytes, L.act_bytes, L.act_bytes, L.partial_bytes, L.counts_bytes, L.ms_bytes, L.ms_bytes};
+  memcpy(offsets, off, sizeof(off));
+  memcpy(sizes, sz, sizeof(sz));
+  dba_encoder_weights none;
+  memset(&none, 0, sizeof(none));
+  dba_encoder_args a;
+  memset(&a, 0, sizeof(a));
+  a.n_images = n_images; a.H = H; a.W = W; a.norm = norm; a.output_dim = norm ? 128 : 256; a.weights = &none;
+  return enc_forward(&a, 0, n_launches, plans);
+}
+
+extern "C" int dba_encoder_forward_prefix(const dba_encoder_args* a, int n_launches) {
+  DBA_CHECK_ARG(a, "null args");
+  const int E = a->n_images, H = a->H, W = a->W;
+  DBA_CHECK_ARG(n_launches >= 0, "encoder: negative launch count");
+  DBA_CHECK_ARG(E > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, "encoder: n_images must be positive and H, W positive multiples of 8");
+  DBA_CHECK_ARG(a->norm == 0 || a->norm == 1, "encoder: norm must be 0 (none) or 1 (instance)");
+  DBA_CHECK_ARG(a->output_dim == 128 || a->output_dim == 256, "encoder: output_dim must be 128 or 256");
+  DBA_CHECK_ARG(a->images_dtype == DBA_F32 || a->images_dtype == DBA_F16, "encoder: images must be DBA_F32 or DBA_F16");
+  DBA_CHECK_ARG(a->images && a->weights && a->out && a->workspace, "null pointer");
+  const dba_encoder_weights* Wt = a->weights;
+  for (int k = 0; k < DBA_ENCODER_CONVS; k++)
+    DBA_CHECK_ARG(Wt->w[k] && Wt->b[k] && ((uintptr_t)Wt->w[k] & 15) == 0, "encoder: packed weights must be non-null, w[k] 16-byte aligned");
+  if (a->workspace_bytes < enc_layout(E, H, W).total) { set_error("invalid argument: workspace too small (dba_encoder_workspace_bytes)"); return DBA_ERR_WORKSPACE; }
+  DBA_CHECK_ARG(((uintptr_t)a->workspace & 255) == 0, "encoder: workspace must be 256-byte aligned");
+  return enc_forward(a, n_launches, nullptr, nullptr);
+}
+
+extern "C" int dba_encoder_forward(const dba_encoder_args* a) { return dba_encoder_forward_prefix(a, INT_MAX); }

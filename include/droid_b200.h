@@ -366,6 +366,21 @@ typedef struct {
 size_t dba_encoder_workspace_bytes(int n_images, int H, int W, int output_dim);
 int dba_encoder_forward(const dba_encoder_args* a);
 
+/* host only: where dba_encoder_forward keeps its intermediates, from the layout and the schedule it uses itself (for tests that check
+ * each launch on what the previous one wrote).  offsets / sizes [DBA_ENCWS_COUNT]: byte offset from the workspace start and size of
+ *   BIG  f16  the im2col rows [n,H/2,W/2,152] (147 used), then the gathered 3x3/2 taps [n,h/2,w/2,9C] of layer2.0 and layer3.0
+ *   X, T1, T2 f16 channels-last activations [n,h,w,C]: X a block's input and output, T1 / T2 its scratch (T1 [.,2P] = conv1 |
+ *        downsample in the stride-2 blocks)
+ *   PARTIAL f32 [n,slots,N,2] (mean, M2) per 16-pixel slot of the last statistics convolution, COUNTS f32 [n,slots] its valid pixels
+ *   MSA, MSB f32 [n,N,2] (mean, rstd) per image and channel
+ * *n_launches = kernels dba_encoder_forward launches; plans [DBA_ENCODER_CONVS][5] = per convolution k the tile width TW, the M tiles
+ * per CTA tile MT, CTA tiles per image along x and y, and the slots its statistics use per image (0 where it takes none: every
+ * convolution of norm 0, conv2 of norm 1).  DBA_ERR_INVALID for extents dba_encoder_forward rejects. */
+enum { DBA_ENCWS_BIG, DBA_ENCWS_X, DBA_ENCWS_T1, DBA_ENCWS_T2, DBA_ENCWS_PARTIAL, DBA_ENCWS_COUNTS, DBA_ENCWS_MSA, DBA_ENCWS_MSB, DBA_ENCWS_COUNT };
+int dba_encoder_workspace_layout(int n_images, int H, int W, int norm, size_t* offsets, size_t* sizes, int* n_launches, int* plans);
+/* dba_encoder_forward stopped after its first n_launches kernels (the same schedule; out is written by the last one only) */
+int dba_encoder_forward_prefix(const dba_encoder_args* a, int n_launches);
+
 /* ---- standalone damped SPD solve (the solver inside dba_ba_solve) ---------------------------------------
  * (H + diag(ep + lm*diag(H))) x = b with H [n,n] fp64 (symmetric; only its lower triangle is read), b [n] fp64 -> x [n] fp32,
  * on the device in fp64; replaces SparseBlock::solve (reference src/droid_kernels.cu:1201-1222).  *fail_flag_device is set to 1
