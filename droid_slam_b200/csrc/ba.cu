@@ -74,13 +74,36 @@ constexpr int kSchurMaxRows = 255;   // Schur rows per depth frame (out-degree +
 // ---------------------------------------------------------------------------------------------------------
 // prepare: kx = sorted unique(ii U [t0,t1)), frame2k, CSR of edges by source frame (stable in edge order)
 // ---------------------------------------------------------------------------------------------------------
+// Exclusive prefix sum over i in [0, count) by the whole block, blockDim.x elements at a time: value(i) gives element i, and
+// emit(i, v, before) receives it with the sum of the elements before it.  Every thread gets the total.  Ends with a __syncthreads().
+template <class Value, class Emit>
+__device__ __forceinline__ int block_exclusive_scan(int count, int* s_scan, Value value, Emit emit) {
+  const int tid = threadIdx.x;
+  int carry = 0;
+  for (int base = 0; base < count; base += blockDim.x) {
+    const int i = base + tid;
+    const int v = (i < count) ? value(i) : 0;
+    s_scan[tid] = v;
+    __syncthreads();
+    for (int off = 1; off < (int)blockDim.x; off <<= 1) {
+      const int t = (tid >= off) ? s_scan[tid - off] : 0;
+      __syncthreads();
+      s_scan[tid] += t;
+      __syncthreads();
+    }
+    if (i < count) emit(i, v, carry + s_scan[tid] - v);
+    carry += s_scan[blockDim.x - 1];
+    __syncthreads();                               // s_scan is rewritten by the next chunk
+  }
+  return carry;
+}
+
 __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restrict__ ii, const int64_t* __restrict__ jj, int E, int N,
                                                           int t0, int t1, int eta_rows, int motion_only, int* __restrict__ hdr,
                                                           int* __restrict__ frame2k, int* __restrict__ kx, int* __restrict__ rowptr, int* __restrict__ big,
                                                           int HW, float* __restrict__ Eij, float* __restrict__ C, float* __restrict__ w,
                                                           float* __restrict__ Ei) {
   __shared__ int s_scan[1024];
-  __shared__ int s_carry;
   const int tid = threadIdx.x;
   if (tid == 0) { hdr[HDR_STATUS] = 0; hdr[HDR_CHOL_FAIL] = 0; }
   // pad pixels [HW, pitch) of the per-pixel rows Eij [6E], C [N], w [N], Ei [6N]: the tensor-core Schur kernel reads them with the
@@ -104,59 +127,23 @@ __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restr
   }
   __syncthreads();
   // exclusive scan of the presence flags -> dense index
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < N; base += blockDim.x) {
-    const int f = base + tid;
-    const int flag = (f < N) ? frame2k[f] : 0;
-    s_scan[tid] = flag;
-    __syncthreads();
-    for (int off = 1; off < (int)blockDim.x; off <<= 1) {
-      int v = (tid >= off) ? s_scan[tid - off] : 0;
-      __syncthreads();
-      s_scan[tid] += v;
-      __syncthreads();
-    }
-    const int incl = s_scan[tid];
-    const int idx = s_carry + incl - flag;
-    if (f < N) {
-      frame2k[f] = flag ? idx : -1;
-      if (flag) kx[idx] = f;
-    }
-    __syncthreads();
-    if (tid == blockDim.x - 1) s_carry += incl;
-    __syncthreads();
-  }
-  const int M = s_carry;
+  const int M = block_exclusive_scan(N, s_scan, [&](int f) { return frame2k[f]; }, [&](int f, int flag, int idx) {
+    frame2k[f] = flag ? idx : -1;
+    if (flag) kx[idx] = f;
+  });
   if (tid == 0) {
     hdr[HDR_M] = M;
     if (eta_rows != M && eta_rows != 1) atomicOr(&hdr[HDR_STATUS], ST_ETA_ROWS);
   }
-  // out-degree per depth frame -> rowptr (exclusive scan, serial per chunk is fine: M <= N small)
+  // out-degree per depth frame -> rowptr
   for (int e = tid; e < E; e += blockDim.x) {
     const long long i = ii[e], j = jj[e];
     if (i < 0 || i >= N || j < 0 || j >= N) continue;
     atomicAdd(&rowptr[frame2k[i] + 1], 1);
   }
   __syncthreads();
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base <= M; base += blockDim.x) {
-    const int m = base + tid;
-    const int cnt = (m <= M) ? rowptr[m] : 0;     // rowptr[m] currently holds deg(m-1), rowptr[0] = 0
-    s_scan[tid] = cnt;
-    __syncthreads();
-    for (int off = 1; off < (int)blockDim.x; off <<= 1) {
-      int v = (tid >= off) ? s_scan[tid - off] : 0;
-      __syncthreads();
-      s_scan[tid] += v;
-      __syncthreads();
-    }
-    if (m <= M) rowptr[m] = s_carry + s_scan[tid];
-    __syncthreads();
-    if (tid == blockDim.x - 1) s_carry += s_scan[tid];
-    __syncthreads();
-  }
+  // rowptr[m] holds deg(m - 1) and rowptr[0] = 0, so the inclusive sum over [0, m] is the start of frame m's segment
+  block_exclusive_scan(M + 1, s_scan, [&](int m) { return rowptr[m]; }, [&](int m, int cnt, int before) { rowptr[m] = before + cnt; });
   // the Schur kernels hold at most kSchurMaxRows rows per depth frame: flag a larger frame here, so that the caller can raise before
   // build and solve change any state (motion-only runs no Schur kernel and has no such limit)
   if (!motion_only)
@@ -164,25 +151,9 @@ __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restr
       if (rowptr[m + 1] - rowptr[m] > kSchurMaxRows - 1) atomicOr(&hdr[HDR_STATUS], ST_DEGREE);
   // depth frames that can have more than kTcRowsMax (21) rows = out-degree + 1: the pair-mode Schur launch only visits these
   // (ascending order; there are at most E / 21 of them, which is what sizes that launch's grid)
-  if (tid == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < M; base += blockDim.x) {
-    const int m = base + tid;
-    const int flag = (m < M && rowptr[m + 1] - rowptr[m] + 1 > 21) ? 1 : 0;
-    s_scan[tid] = flag;
-    __syncthreads();
-    for (int off = 1; off < (int)blockDim.x; off <<= 1) {
-      int v = (tid >= off) ? s_scan[tid - off] : 0;
-      __syncthreads();
-      s_scan[tid] += v;
-      __syncthreads();
-    }
-    if (flag) big[s_carry + s_scan[tid] - 1] = m;
-    __syncthreads();
-    if (tid == blockDim.x - 1) s_carry += s_scan[tid];
-    __syncthreads();
-  }
-  if (tid == 0) hdr[HDR_NBIG] = s_carry;
+  const int nbig = block_exclusive_scan(M, s_scan, [&](int m) { return rowptr[m + 1] - rowptr[m] + 1 > 21 ? 1 : 0; },
+                                        [&](int m, int flag, int idx) { if (flag) big[idx] = m; });
+  if (tid == 0) hdr[HDR_NBIG] = nbig;
 }
 
 // stable placement of every edge inside its source frame's segment: rank = #earlier edges with the same source.
@@ -443,21 +414,19 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
 // is outside [t0,t1) are dropped (they contribute nothing, reference :1155,:1257).
 // The rows of a frame decide the kernel, for every image size (the workspace rows are padded to ba_pitch, i.e. 16-byte aligned):
 //   <= kTcRowsMax rows (every frame of a sliding-window graph)   ba_schur_tc_kernel<false>: tensor cores, packed or single tile
-//   kTcRowsMax+1 .. kPairRowsMax rows (dense graphs, sharded)    ba_schur_tc_kernel<true>:  tensor cores, pairs of row tiles
-//   more rows                                                    ba_schur_gemm_kernel:      SIMT fp32 block pairs
-// Each flushes once with fp64 atomics into the LOWER triangle of the reduced system.
+//   kTcRowsMax+1 .. kSchurMaxRows rows (dense graphs, sharded)   ba_schur_tc_kernel<true>:  tensor cores, pairs of row tiles
+// Both flush once per tile (pair) with fp64 atomics into the LOWER triangle of the reduced system.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int kTcRowsMax = 21;
-constexpr int kPairRowsMax = 100;
+constexpr int kTcThreads = 256;
 // Q = 1/C of the eliminated depth block.  C <= 0 only for a pixel with eta = 0 and no weight on any edge; the reference divides
-// anyway (inf -> NaN system -> zero pose update and NaN depths at that pixel).  All Schur kernels and the back-substitution here
+// anyway (inf -> NaN system -> zero pose update and NaN depths at that pixel).  The Schur kernel and the back-substitution here
 // drop such a pixel instead (Q = 0, dz = 0): one rule on every path, documented in INTEGRATION.md.
 __device__ __forceinline__ float safe_rcp(float c) { return c > 0.f ? 1.0f / c : 0.f; }
 
 // Row list of a depth frame: (pose ix, Ei) first when ix is inside the window, then (pose jj[e], Eij[e]) for its out-edges in CSR
 // order whose target pose is inside the window.  Built by the whole CTA: thread a handles out-edge a, an order-preserving
 // ballot compaction keeps the reference's row order.  Ends with a __syncthreads().
-template <int kThreads>
 __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ edgeidx,
                                                int e_begin, int deg, int ix, int m, int pitch, int t0, int P, const float* __restrict__ Eij,
                                                const float* __restrict__ Eiin, int* s_pose, const float** s_ptr, int* s_nrows, int* s_wcount) {
@@ -478,7 +447,7 @@ __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, i
   if (tid == 0) {
     if (self) { s_pose[0] = ix - t0; s_ptr[0] = Eiin + (size_t)m * 6 * pitch; }
     int tot = self ? 1 : 0;
-    for (int w = 0; w < kThreads / 32; w++) tot += s_wcount[w];
+    for (int w = 0; w < kTcThreads / 32; w++) tot += s_wcount[w];
     *s_nrows = tot;
     if (deg > kSchurMaxRows - 1) atomicOr(&hdr[HDR_STATUS], ST_DEGREE);
   }
@@ -486,149 +455,7 @@ __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, i
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Schur complement for frames with more than kPairRowsMax rows (dense graphs / edge-sharded ranks): SGEMM-style kernel.
-// C = A diag(Q) A^T with A = [6R x pixels].  A CTA computes one 16-row x 16-row tile pair (96 x 96 scalars) for a pixel
-// chunk: thread (ty,tx) owns the 6x6 block pair (row 16*ti+ty, row 16*tj+tx) in registers for the WHOLE chunk (no per-tile
-// reductions), the K loop walks 64-pixel shared-memory tiles stored pixel-major so that a thread reads its 6+6 operands as
-// three 64-bit broadcasts each: 36 FMA per 6 LDS.64.  Tile pairs (ti >= tj) go over blockIdx.z.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int kSgRows = 16;                 // rows per tile
-constexpr int kSgK = 64;                    // pixels per shared-memory tile
-constexpr int kSgStride = kSgRows * 6 + 2;  // 98 floats per pixel line (even -> 8-byte aligned LDS.64)
-constexpr int kSgThreads = 256;
-
-__global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
-    const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
-    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta,
-    const float* __restrict__ Eij, const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
-    double* __restrict__ Hsys, double* __restrict__ bsys) {
-  const int m = blockIdx.y;
-  if (m >= hdr[HDR_M]) return;
-  const int ix = kx[m];
-  const int e_begin = rowptr[m];
-  const int deg = rowptr[m + 1] - e_begin;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int ty = tid >> 4, tx = tid & 15;
-  const int n = 6 * P;
-  const int pitch = ba_pitch(HW);
-
-  __shared__ int s_pose[kSchurMaxRows + 1];
-  __shared__ const float* s_ptr[kSchurMaxRows + 1];
-  __shared__ int s_nrows;
-  __shared__ int s_wcount[kSgThreads / 32];
-  extern __shared__ float sg_dyn[];
-  float* sA = sg_dyn;
-  float* sB = sg_dyn + kSgK * kSgStride;
-  __shared__ float sQw[kSgK];
-  __shared__ float sQ[kSgK];
-
-  if (deg + 1 <= kPairRowsMax) return;                 // at most deg + 1 rows: not this kernel's frame (skips the row-list build)
-  build_row_list<kSgThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
-  const int nrows = s_nrows;
-  if (nrows <= kPairRowsMax) return;                   // smaller frames belong to ba_schur_tc_kernel
-  const int nT = (nrows + kSgRows - 1) / kSgRows;
-  const int npairs = nT * (nT + 1) / 2;
-  const int px_begin = blockIdx.x * px_per_cta;
-  const int px_end = min(HW, px_begin + px_per_cta);
-  if (px_begin >= px_end) return;
-
-  for (int pr = blockIdx.z; pr < npairs; pr += gridDim.z) {
-    int ti = (int)((sqrtf(8.f * (float)pr + 1.f) - 1.f) * 0.5f);
-    while (ti * (ti + 1) / 2 > pr) ti--;
-    while ((ti + 1) * (ti + 2) / 2 <= pr) ti++;
-    const int tj = pr - ti * (ti + 1) / 2;             // ti >= tj
-    const int ra = min(kSgRows, nrows - ti * kSgRows), rb = min(kSgRows, nrows - tj * kSgRows);
-    const bool diag_tile = (ti == tj);
-    const bool active = (ty < ra) && (tx < rb) && (!diag_tile || ty >= tx);
-    const bool diag_pair = diag_tile && (ty == tx);
-    float acc[36], bacc[6];
-#pragma unroll
-    for (int k = 0; k < 36; k++) acc[k] = 0.f;
-#pragma unroll
-    for (int k = 0; k < 6; k++) bacc[k] = 0.f;
-
-    for (int p0 = px_begin; p0 < px_end; p0 += kSgK) {
-      const int np = min(kSgK, px_end - p0);
-      __syncthreads();
-      // ---- stage: A tile scaled by Q, B tile raw; one warp per (row, component) line of 64 pixels, transposed into [px][row*6+c]
-      for (int px = tid; px < kSgK; px += kSgThreads) {
-        const bool okp = px < np;
-        const float q = okp ? safe_rcp(__ldg(Cin + (size_t)m * pitch + p0 + px)) : 0.f;
-        sQ[px] = q;
-        sQw[px] = okp ? __ldg(win + (size_t)m * pitch + p0 + px) : 0.f;
-      }
-      __syncthreads();
-      for (int ln = warp; ln < (ra + (diag_tile ? 0 : rb)) * 6; ln += kSgThreads / 32) {
-        const int rowl = ln / 6, c = ln - rowl * 6;
-        const bool second = rowl >= ra;
-        const int row = second ? (tj * kSgRows + rowl - ra) : (ti * kSgRows + rowl);
-        const float* src = s_ptr[row] + (size_t)c * pitch + p0;
-        float* dst = (second ? sB : sA) + (second ? rowl - ra : rowl) * 6 + c;
-#pragma unroll
-        for (int h = 0; h < kSgK / 32; h++) {
-          const int px = h * 32 + lane;
-          float v = (px < np) ? __ldg(src + px) : 0.f;
-          if (!second) {
-            // A operand carries Q = 1/C (reference K9: ei = E*q); diagonal tiles keep the unscaled copy in sB
-            if (diag_tile) sB[px * kSgStride + rowl * 6 + c] = v;
-            v *= sQ[px];
-          }
-          dst[px * kSgStride] = v;
-        }
-      }
-      __syncthreads();
-      if (active) {
-        const float* pa = sA + ty * 6;
-        const float* pb = sB + tx * 6;
-#pragma unroll 4
-        for (int px = 0; px < kSgK; px++) {
-          const float2 a01 = *reinterpret_cast<const float2*>(pa + px * kSgStride);
-          const float2 a23 = *reinterpret_cast<const float2*>(pa + px * kSgStride + 2);
-          const float2 a45 = *reinterpret_cast<const float2*>(pa + px * kSgStride + 4);
-          const float2 b01 = *reinterpret_cast<const float2*>(pb + px * kSgStride);
-          const float2 b23 = *reinterpret_cast<const float2*>(pb + px * kSgStride + 2);
-          const float2 b45 = *reinterpret_cast<const float2*>(pb + px * kSgStride + 4);
-          const float ea[6] = {a01.x, a01.y, a23.x, a23.y, a45.x, a45.y};
-          const float eb[6] = {b01.x, b01.y, b23.x, b23.y, b45.x, b45.y};
-#pragma unroll
-          for (int a = 0; a < 6; a++)
-#pragma unroll
-            for (int c = 0; c < 6; c++) acc[a * 6 + c] += ea[a] * eb[c];
-          if (diag_pair) {
-            const float w = sQw[px];          // (Q E) w = Q w E
-#pragma unroll
-            for (int c = 0; c < 6; c++) bacc[c] += w * ea[c];
-          }
-        }
-      }
-    }
-    // ---- flush this thread's block pair into the lower triangle
-    if (active) {
-      const int pa_ = s_pose[ti * kSgRows + ty], pb_ = s_pose[tj * kSgRows + tx];
-#pragma unroll
-      for (int a = 0; a < 6; a++) {
-#pragma unroll
-        for (int c = 0; c < 6; c++) {
-          const double v = -(double)acc[a * 6 + c];
-          const int gr = pa_ * 6 + a, gc = pb_ * 6 + c;
-          if (diag_pair) {
-            if (gr >= gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
-          } else {
-            if (gr >= gc) atomicAdd(&Hsys[(size_t)gr * n + gc], v);
-            if (gc >= gr) atomicAdd(&Hsys[(size_t)gc * n + gr], v);
-          }
-        }
-      }
-      if (diag_pair) {
-#pragma unroll
-        for (int a = 0; a < 6; a++) atomicAdd(&bsys[pa_ * 6 + a], -(double)bacc[a]);
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Schur complement on the tensor cores (frames with at most kTcRowsMax rows; PAIR mode below: up to kPairRowsMax rows):
+// Schur complement on the tensor cores (frames with at most kTcRowsMax rows; PAIR mode below: up to kSchurMaxRows rows):
 //   S = X X^T  with  X = [ E_r / sqrt(C) ; w / sqrt(C) ]  (6R + 1 rows x pixels),  so that S[:6R,:6R] = sum E q E^T and
 //   S[:6R, 6R] = sum E q w  -- one symmetric rank-K update per frame, K = pixels.
 // fp32 accuracy on the tf32 pipe by operand splitting (3xTF32): x = hi + lo with hi = tf32(x), lo = x - hi (exact), and
@@ -649,8 +476,7 @@ __global__ void __launch_bounds__(kSgThreads) ba_schur_gemm_kernel(
 // and C, and rsqrt(C) is taken as 0 there, so they add nothing.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int kPairTileRows = 10;               // pair mode: row tiles of 10 frame rows (60 lines + the w line <= 64 operand rows)
-constexpr int kPairGridZ = 45;                  // tile pairs of a kPairRowsMax-row frame (10 tiles)
-constexpr int kTcThreads = 256;
+constexpr int kPairGridZ = 45;                  // CTAs per frame in pair mode: the tile pairs of a 100-row frame (10 tiles)
 constexpr int kTcRawStages = 4;
 constexpr int kTcRawBytes = 128 * 128;          // up to 128 lines (6R rows, w, C; two halves when packed) x 128 bytes
 constexpr int kTcOpBytes = 128 * 128;           // one operand tile (hi or lo)
@@ -669,63 +495,20 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
 }
 __device__ __forceinline__ void sts_f32(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
 
-// PAIR mode (frames with 22..100 rows: dense graphs, edge-sharded ranks): the rows are cut into tiles of 10; CTA (frame, pair z) stacks
-// tile a in operand rows 0..63 and tile b in rows 64..127 over the SAME 32 pixels (the packed layout with a zero pixel offset for the
-// second half), so the one M = N = 128 product holds S_ba in its lower-left block and S_aa / S_bb on the diagonal (emitted only by
-// the designated pair (t, t+1)); G + G^T symmetrisation unchanged.  Off-diagonal-block entries go to (max, min) of the global
-// indices and count twice where two different rows share a pose.
+// One pass of the Schur complement over pixels [px_begin, px_end) of depth frame m (rows in s_pose / s_ptr): the whole frame, or in
+// PAIR mode the row tiles ta < tb, whose diagonal blocks S_aa / S_bb are added only where emit_a / emit_b.  A caller that runs
+// another pass must put a CTA barrier in between: the epilogue reads s_gidx and the operand ring, which the next pass rewrites.
+// lane and warp come from the caller, which in PAIR mode makes warp opaque per pass (see the pair loop).
 template <bool PAIR>
-__global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
-    const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
-    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta,
-    const float* __restrict__ Eij, const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
-    double* __restrict__ Hsys, double* __restrict__ bsys, const int* __restrict__ big) {
-  if (PAIR && (int)blockIdx.y >= hdr[HDR_NBIG]) return;          // PAIR: blockIdx.y runs over the list of high-degree depth frames
-  const int m = PAIR ? big[blockIdx.y] : blockIdx.y;
-  if (m >= hdr[HDR_M]) return;
-  const int ix = kx[m];
-  const int e_begin = rowptr[m];
-  const int deg = rowptr[m + 1] - e_begin;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = 6 * P;
-  const int pitch = ba_pitch(HW);
-
-  __shared__ int s_pose[kSchurMaxRows + 1];
-  __shared__ const float* s_ptr[kSchurMaxRows + 1];
-  __shared__ int s_nrows;
-  __shared__ int s_wcount[kTcThreads / 32];
-  __shared__ int s_gidx[128];                     // operand row / column -> index in the reduced system (-1: rhs, -2: padding)
+__device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nrows, int ta, int tb, bool emit_a, bool emit_b,
+                                              int px_begin, int px_end, int pitch, int n, const float* __restrict__ Cin,
+                                              const float* __restrict__ win, double* __restrict__ Hsys, double* __restrict__ bsys,
+                                              const int* s_pose, const float* const* s_ptr, int* s_gidx) {
+  const int tid = threadIdx.x;
   extern __shared__ uint8_t tc_smem_raw[];
-
-  if (deg == 0) return;                           // no out-edge (e.g. a frame another rank owns): E_k = 0, nothing to subtract
-  if (PAIR) {                                     // cheap exits before the row-list build: at most deg + 1 rows
-    if (deg + 1 <= kTcRowsMax) return;
-    const int tmax = (min(deg + 1, kPairRowsMax) + kPairTileRows - 1) / kPairTileRows;
-    if ((int)blockIdx.z >= tmax * (tmax - 1) / 2) return;
-  }
-  build_row_list<kTcThreads>(jj, hdr, edgeidx, e_begin, deg, ix, m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
-  const int nrows = s_nrows;
-  if (!PAIR && (nrows == 0 || nrows > kTcRowsMax)) return;            // larger frames belong to the pair-mode launch / ba_schur_gemm_kernel
-  if (PAIR && (nrows <= kTcRowsMax || nrows > kPairRowsMax)) return;
-  int ta = 0, tb = 0;                                    // PAIR: the two row tiles of this CTA (ta < tb)
-  bool emit_a = true, emit_b = true;
-  if (PAIR) {
-    const int T = (nrows + kPairTileRows - 1) / kPairTileRows;         // >= 3
-    const int pr = blockIdx.z;
-    if (pr >= T * (T - 1) / 2) return;
-    tb = (int)((sqrtf(8.f * (float)pr + 1.f) + 1.f) * 0.5f);
-    while (tb * (tb - 1) / 2 > pr) tb--;
-    while ((tb + 1) * tb / 2 <= pr) tb++;
-    ta = pr - tb * (tb - 1) / 2;
-    emit_a = (tb == ta + 1);                             // S_tt of tile t < T-1 comes from pair (t, t+1), of tile T-1 from pair (T-2, T-1)
-    emit_b = (tb == T - 1 && ta == T - 2);
-  }
-  const int px_begin = blockIdx.x * px_per_cta;
-  const int px_end = min(HW, px_begin + px_per_cta);
-  if (px_begin >= px_end) return;
   const int R6a = PAIR ? 6 * min(kPairTileRows, nrows - kPairTileRows * ta) : 6 * nrows;
   const int R6b = PAIR ? 6 * min(kPairTileRows, nrows - kPairTileRows * tb) : 6 * nrows;
-  const int R6 = R6a;                                    // operand rows 0..R6-1: E rows, row R6: w  (PAIR: of the half, see R6h)
+  const int R6 = R6a;                                    // operand rows 0..R6-1: E rows, row R6: w  (PAIR: of tile a, R6b of tile b)
   const bool packed = !PAIR && (R6 + 2 <= 64);          // two PIXEL halves of a 64-pixel chunk in operand rows 0..63 / 64..127
   const bool two_halves = PAIR || packed;                // operand rows 64..127 carry a second set of lines
   const int nhalf = packed ? 2 : 1;
@@ -743,7 +526,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
     } else s_gidx[tid] = (tid < R6) ? s_pose[tid / 6] * 6 + (tid % 6) : (tid == R6 ? -1 : -2);
   }
   {
-    // operand tiles start as zeros: rows that carry no line are never written again
+    // operand tiles start each pass as zeros (the previous pass's G staging overwrote them): rows that carry no line are never written
     uint4* z = reinterpret_cast<uint4*>(smem);
     for (int k = tid; k < kTcOpStages * 2 * kTcOpBytes / 16; k += kTcThreads) z[k] = make_uint4(0u, 0u, 0u, 0u);
   }
@@ -924,6 +707,68 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   }
 }
 
+// PAIR mode (frames with 22..kSchurMaxRows rows: dense graphs, edge-sharded ranks): the rows are cut into T <= 26 tiles of 10, and a pass
+// stacks tile a in operand rows 0..63 and tile b in rows 64..127 over the SAME 32 pixels (the packed layout with a zero pixel offset
+// for the second half), so the one M = N = 128 product holds S_ba in its lower-left block and S_aa / S_bb on the diagonal (emitted
+// only by the designated pair (t, t+1)); G + G^T symmetrisation unchanged.  Off-diagonal-block entries go to (max, min) of the global
+// indices and count twice where two different rows share a pose.  CTA (frame, z) runs the tile pairs z, z + gridDim.z, ... of the
+// T (T - 1) / 2, each over the whole pixel range: one pair per CTA up to 100 rows (45 pairs), at most 8 at 255 rows (325 pairs).
+template <bool PAIR>
+__global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
+    const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
+    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta,
+    const float* __restrict__ Eij, const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
+    double* __restrict__ Hsys, double* __restrict__ bsys, const int* __restrict__ big) {
+  if (PAIR && (int)blockIdx.y >= hdr[HDR_NBIG]) return;          // PAIR: blockIdx.y runs over the list of high-degree depth frames
+  const int m = PAIR ? big[blockIdx.y] : blockIdx.y;
+  if (m >= hdr[HDR_M]) return;
+  const int ix = kx[m];
+  const int e_begin = rowptr[m];
+  const int deg = rowptr[m + 1] - e_begin;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int n = 6 * P;
+  const int pitch = ba_pitch(HW);
+
+  __shared__ int s_pose[kSchurMaxRows + 1];
+  __shared__ const float* s_ptr[kSchurMaxRows + 1];
+  __shared__ int s_nrows;
+  __shared__ int s_wcount[kTcThreads / 32];
+  __shared__ int s_gidx[128];                     // operand row / column -> index in the reduced system (-1: rhs, -2: padding)
+
+  if (deg == 0) return;                           // no out-edge (e.g. a frame another rank owns): E_k = 0, nothing to subtract
+  if (PAIR) {                                     // cheap exits before the row-list build: at most deg + 1 rows
+    if (deg + 1 <= kTcRowsMax) return;
+    const int tmax = (min(deg + 1, kSchurMaxRows) + kPairTileRows - 1) / kPairTileRows;
+    if ((int)blockIdx.z >= tmax * (tmax - 1) / 2) return;
+  }
+  build_row_list(jj, hdr, edgeidx, e_begin, deg, ix, m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
+  const int nrows = s_nrows;
+  if (!PAIR && (nrows == 0 || nrows > kTcRowsMax)) return;            // larger frames belong to the pair-mode launch
+  if (PAIR && nrows <= kTcRowsMax) return;
+  const int px_begin = blockIdx.x * px_per_cta;
+  const int px_end = min(HW, px_begin + px_per_cta);
+  if (px_begin >= px_end) return;
+  if (!PAIR) {
+    schur_tc_pass<false>(lane, warp, m, nrows, 0, 0, true, true, px_begin, px_end, pitch, n, Cin, win, Hsys, bsys, s_pose, s_ptr, s_gidx);
+    return;
+  }
+  const int T = (nrows + kPairTileRows - 1) / kPairTileRows;         // 3 .. 26
+  for (int pr = blockIdx.z; pr < T * (T - 1) / 2; pr += gridDim.z) {
+    int tb = (int)((sqrtf(8.f * (float)pr + 1.f) + 1.f) * 0.5f);       // the two row tiles of this pass (ta < tb)
+    while (tb * (tb - 1) / 2 > pr) tb--;
+    while ((tb + 1) * tb / 2 <= pr) tb++;
+    const int ta = pr - tb * (tb - 1) / 2;
+    // warp made opaque per pass: the copy slots and swizzled offsets derived from it are then computed inside the loop.  Hoisted out
+    // of it, they would stay live across every pass and the kernel would spill.
+    int warp_p = warp;
+    asm volatile("" : "+r"(warp_p));
+    // S_tt of tile t < T-1 comes from pair (t, t+1), of tile T-1 from pair (T-2, T-1)
+    schur_tc_pass<true>(lane, warp_p, m, nrows, ta, tb, tb == ta + 1, tb == T - 1 && ta == T - 2, px_begin, px_end, pitch, n, Cin,
+                        win, Hsys, bsys, s_pose, s_ptr, s_gidx);
+    __syncthreads();                                     // the next pass rewrites s_gidx and the operand ring
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // back substitution + retractions
 // ---------------------------------------------------------------------------------------------------------
@@ -1062,20 +907,14 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
 #undef LAUNCH_BUILD
   DBA_CHECK_LAUNCH("ba_build");
   if (!a->motion_only && L.P > 0) {
-    const size_t smem2 = (size_t)2 * kSgK * kSgStride * sizeof(float);
-    // the SGEMM-style kernel keeps its accumulators in registers over the whole pixel chunk: few long chunks, tile pairs over z
-    const int px_per_cta2 = ((HW + 2) / 3 + kSgK - 1) / kSgK * kSgK;
-    const int gx2 = (HW + px_per_cta2 - 1) / px_per_cta2;
-    const int zsplit2 = std::max(1, std::min(32, (6 * sms + eff_frames * gx2 - 1) / (eff_frames * gx2)));
     static bool attr_set = false;
     if (!attr_set) {
-      DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2), "schur gemm smem attr");
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc smem attr");
       DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc pair smem attr");
       attr_set = true;
     }
-    // one launch per routing-table entry (see the Schur section): frames with at most kTcRowsMax rows on the packed / single
-    // tensor-core kernel, up to kPairRowsMax rows on the pair kernel, more on ba_schur_gemm_kernel.  Each kernel exits on other frames.
+    // one launch per routing-table entry (see the Schur section): frames with at most kTcRowsMax rows on the packed / single-tile
+    // kernel, more on the pair kernel.  Each exits on the other's frames.
     const int tiles64 = (HW + 63) / 64;
     const int chunks_tc = std::max(1, std::min(tiles64, (sms + eff_frames / 2) / eff_frames));     // one CTA per SM
     const int px_per_cta_tc = ((tiles64 + chunks_tc - 1) / chunks_tc) * 64;
@@ -1083,18 +922,14 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
     ba_schur_tc_kernel<false><<<dim3(gx_tc, a->n_frames, 1), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
                                                          WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta_tc, WS(float, L.off_Eij),
                                                          WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
-    // pair mode: tile pairs over gridDim.z, whole pixel range per CTA; CTAs of frames outside its row range (and pair indices beyond
-    // a frame's count) exit after the row-list build.
+    // pair mode: kPairGridZ CTAs per listed frame share its tile pairs, whole pixel range per CTA; CTAs beyond a frame's pair count
+    // and CTAs of frames with at most kTcRowsMax rows (targets outside the window) exit before any Schur work.
     const int max_big = std::min(a->n_frames, a->n_edges / kTcRowsMax);     // a frame with 22+ rows has 21+ out-edges
     if (max_big > 0)
       ba_schur_tc_kernel<true><<<dim3(1, max_big, kPairGridZ), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
                                                          WS(int, L.off_edgeidx), HW, a->t0, L.P, ((HW + 31) / 32) * 32, WS(float, L.off_Eij),
                                                          WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
-    DBA_CHECK_LAUNCH("ba_schur<single>");
-    ba_schur_gemm_kernel<<<dim3(gx2, a->n_frames, zsplit2), kSgThreads, smem2, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta2, WS(float, L.off_Eij),
-                                                                         WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys);
-    DBA_CHECK_LAUNCH("ba_schur<multi>");
+    DBA_CHECK_LAUNCH("ba_schur");
   }
   return DBA_OK;
 }

@@ -5,9 +5,10 @@ Each Gauss-Newton iteration of the native `ba` is four stages: build the reduced
 of the inverse-depth blocks), solve it, back-substitute the inverse-depth updates, retract the poses.  The references below evaluate
 each stage in fp64 from the native state at the start of that iteration, so a failing check names its stage.
 
-The Schur complement of a depth frame runs on one of four kernels, chosen by its row count (its own pose if it is in [t0, t1), plus one
-row per out-edge whose target is in [t0, t1)): packed 3xTF32 tensor-core tiles up to 10 rows, one tile up to 21, pairs of row tiles up
-to 100, the SIMT block-pair kernel above that.  The build kernel runs at 1, 2 or 4 pixels per thread (`ppt` below)."""
+The Schur complement of a depth frame runs on one of three 3xTF32 tensor-core routes, chosen by its row count (its own pose if it is
+in [t0, t1), plus one row per out-edge whose target is in [t0, t1)): packed tiles up to 10 rows, one tile up to 21, pairs of 10-row
+tiles above that, up to 255 rows (45 CTAs per frame, each running every 45th pair: one pair per CTA up to 100 rows, several above).
+The build kernel runs at 1, 2 or 4 pixels per thread (`ppt` below)."""
 import torch
 
 import oracle
@@ -31,7 +32,7 @@ def route(rows, deg):
     """Schur kernel of a depth frame with `rows` rows and `deg` out-edges (dba_ba_build's routing table); None: nothing to subtract"""
     if deg == 0 or rows == 0:
         return None
-    return "packed" if rows <= 10 else "single" if rows <= 21 else "pair" if rows <= 100 else "gemm"
+    return "packed" if rows <= 10 else "single" if rows <= 21 else "pair"
 
 
 def ppt(N, HW, sms=SMS_H100):
@@ -56,11 +57,13 @@ def _targets(f, n, lo, hi):
 
 
 def boundary_graph(N=40):
-    """frames whose row count sits on each side of every route switch, t0 = 1.  Frames 12 and 20 have out-edges into frame 0, which is
-    outside the window, so their degree exceeds their row count: frame 12 has 21 rows but 23 out-edges (it is in the pair kernel's
-    frame list and is left to the single-tile kernel), frame 20 has 100 rows and 101 out-edges (the SIMT kernel builds its row list and
-    leaves it to the pair kernel).  Frame 28 has 254 out-edges: 255 rows, the most a frame may have."""
-    want = {5: 10, 8: 11, 12: 21, 16: 22, 20: 100, 24: 101, 28: 255}
+    """frames whose row count sits on each side of every route switch, t0 = 1, and on each side of the pair kernel's one pair per CTA.
+    Frames 12 and 20 have out-edges into frame 0, which is outside the window, so their degree exceeds their row count - 1: frame 12
+    has 21 rows but 22 out-edges (it is in the pair kernel's frame list and is left to the single-tile kernel), frame 20 has 100 rows
+    and 100 out-edges (45 tile pairs, one per CTA).  Frame 24 has 101 rows (55 pairs: a second pair for 10 CTAs), frame 32 has 136 rows
+    (14 tiles, 91 pairs = 2 x 45 + 1: a partial last round), frame 28 has 254 out-edges: 255 rows, the most a frame may have
+    (325 pairs, up to 8 per CTA)."""
+    want = {5: 10, 8: 11, 12: 21, 16: 22, 20: 100, 24: 101, 28: 255, 32: 136}
     extra_out = {12: 2, 20: 1}
     e = _sliding(N, skip=want)
     for f, r in want.items():
@@ -228,10 +231,12 @@ def test_boundary_case_has_every_row_count_switch():
     _, _, want = boundary_graph()
     assert {f: int(rows[f]) for f in want} == want
     assert int(deg[12]) == 22 and int(deg[20]) == 100 and int(deg[28]) == 254       # degree + 1 != rows where targets leave the window
-    assert [route(int(rows[f]), int(deg[f])) for f in sorted(want)] == ["packed", "single", "single", "pair", "pair", "gemm", "gemm"]
-    assert routes == {"packed", "single", "pair", "gemm"} and p == 2
+    assert [route(int(rows[f]), int(deg[f])) for f in sorted(want)] == ["packed", "single", "single", "pair", "pair", "pair", "pair", "pair"]
+    assert routes == {"packed", "single", "pair"} and p == 2
+    tiles = {f: (r + 9) // 10 for f, r in want.items() if r > 21}
+    assert {f: t * (t - 1) // 2 for f, t in tiles.items()} == {16: 3, 20: 45, 24: 55, 28: 325, 32: 91}
     ii, jj, *_ = case_graph("boundary_48x64")
-    for f in (8, 16, 24, 28):       # a target repeated inside the frame's first row tile and again in a later position
+    for f in (8, 16, 24, 28, 32):   # a target repeated inside the frame's first row tile and again in a later position
         t = jj[ii == f].tolist()
         assert t[0] == t[1] == t[-1]
 

@@ -19,8 +19,9 @@ Bounds, each a normalised error:
   retract window poses against the fp64 retraction of dx_native: <= 1e-6 (1 + |t|); poses outside [t0, t1) are untouched.
 
 Worst observed on one H100 80GB HBM3 at a 400 W power limit (system / motion-only A / solve / backsub / retract), per case, with
-the Schur routes and the pixels per thread (ppt) of the build that the case takes:
-  boundary_48x64             7.1e-07 / 7.5e-07 / 3.7e-08 / 2.2e-06 / 7.0e-08  (packed, single, pair, gemm; ppt 2)
+the Schur routes and the pixels per thread (ppt) of the build that the case takes; boundary_48x64 and degree_254_8x12 (* below) were
+taken again on one H100 80GB HBM3 at a 700 W power limit once their frames above 100 rows ran in pair mode:
+  boundary_48x64 *           5.8e-07 / 5.5e-07 / 3.0e-08 / 3.1e-06 / 1.0e-07  (packed, single, pair up to 255 rows; ppt 2)
   mixed_47x63_nan_ws         5.2e-07 / 6.0e-07 / 5.2e-08 / 3.6e-06 / 6.2e-08  (packed, single, pair; ppt 2)
   mixed_7x9                  1.6e-07 / 1.7e-07 / 3.0e-08 / 1.1e-06 / 7.4e-08  (packed, single, pair; ppt 1)
   mixed_3x5                  1.7e-07 / 1.7e-07 / 3.7e-08 / 6.7e-07 / 5.0e-08  (packed, single, pair; ppt 1)
@@ -32,7 +33,7 @@ the Schur routes and the pixels per thread (ppt) of the build that the case take
   empty_window               0 / 0 / 0 / 2.1e-06 / 0                       (no pose system; ppt 1)
   metric                     2.1e-07 / 6.7e-07 / 4.4e-08 / 6.6e-07 / 8.0e-08  (packed; ppt 4)
   c3_global                  9.7e-07 / 3.9e-06 / 3.0e-08 / 3.4e-06 / 1.2e-07  (packed; ppt 4)
-  degree_254_8x12            1.1e-07 / 1.9e-07 / 3.7e-08 / 3.8e-07 / 6.3e-08  (packed, gemm (255 rows); ppt 1)
+  degree_254_8x12 *          1.1e-07 / 1.9e-07 / 3.7e-08 / 3.5e-07 / 6.3e-08  (packed, pair (255 rows); ppt 1)
 """
 import ctypes
 import json

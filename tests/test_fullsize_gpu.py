@@ -167,15 +167,16 @@ def test_ba_every_schur_kernel_on_padded_rows_matches_oracle(backends):
 
 def _high_degree_graph():
     """_mixed_degree_graph plus frame 12 with its 24 targets within 12 frames repeated 5 times: 124 out-edges -> 125 rows (120 after
-    dropping the 5 rows of frame 0, which is outside the window).  That frame takes ba_schur_gemm_kernel (more than 100 rows), where
-    repeated targets put rows with one pose into different tiles (the duplicate-pose rule)."""
+    dropping the 5 rows of frame 0, which is outside the window).  That frame takes the tensor-core pair mode with more than 100 rows
+    (12 tiles, 66 tile pairs: a second pair for some CTAs), where repeated targets put rows with one pose into different tiles (the
+    duplicate-pose rule)."""
     ii, jj = _mixed_degree_graph()
     extra = [j for _ in range(5) for j in range(0, 25) if j != 12]
     return ii + [12] * len(extra), jj + extra
 
 
 @pytest.mark.parametrize("ht,wd", [(48, 64), (47, 63)])
-def test_ba_schur_gemm_frame_over_100_rows_matches_oracle(capi, ht, wd):
+def test_ba_schur_pair_frame_over_100_rows_matches_oracle(capi, ht, wd):
     """every Schur kernel in one graph, with a workspace that starts as NaN: a pad pixel that the Schur kernels read but nothing
     zeroed would turn the result into NaN"""
     ii, jj = _high_degree_graph()
