@@ -14,7 +14,7 @@ SYMBOLS = [
     "dba_ba_prepare", "dba_ba_build", "dba_ba_solve", "dba_ba", "dba_ba_read_info", "dba_ba_p2p_signal",
     "dba_solve_workspace_bytes", "dba_solve_spd", "dba_solve_tile_placement",
     "dba_update_workspace_bytes", "dba_update_workspace_layout", "dba_update_forward", "dba_conv_nhwc", "dba_conv_nhwc_plan", "dba_encoder_workspace_bytes", "dba_encoder_forward",
-    "dba_encoder_workspace_layout", "dba_encoder_forward_prefix", "dba_proximity_workspace_bytes", "dba_proximity_edges",
+    "dba_encoder_forward_frames", "dba_encoder_workspace_layout", "dba_encoder_forward_prefix", "dba_proximity_workspace_bytes", "dba_proximity_edges",
     "dba_fill_interpolate", "dba_pose_only_ba",
 ]
 
@@ -91,6 +91,7 @@ def load():
     L.dba_encoder_workspace_bytes.argtypes = [ci] * 4
     L.dba_encoder_workspace_layout.argtypes = [ci] * 4 + [vp] * 4
     L.dba_encoder_forward_prefix.argtypes = [vp, ci]
+    L.dba_encoder_forward_frames.argtypes = [vp, vp]
     L.dba_proximity_workspace_bytes.restype = ctypes.c_size_t
     L.dba_proximity_workspace_bytes.argtypes = [ci, ci, ci]
     L.dba_proximity_edges.argtypes = [vp, ci, ci, ci, vp, vp, ci, ci, ci, cf, ci, ci, vp, ci, vp, vp, ctypes.c_size_t, vp]

@@ -647,14 +647,17 @@ std::vector<torch::Tensor> update_forward(torch::Tensor net, torch::Tensor inp, 
 // BasicEncoder.forward (reference droid_slam/modules/extractor.py:183-198) for DroidNet's fnet (norm 1 = instance, output_dim
 // 128) and cnet (norm 0 = none, output_dim 256).  images [n,3,H,W] f32/f16, H and W multiples of 8; packed = the 28 tensors of
 // droid_slam_b200.encoder.pack_encoder_weights (w[0..13] f16, then b[0..13] f32, include/droid_b200.h).  Returns [n,output_dim,H/8,W/8] f16.
-torch::Tensor encoder_forward(torch::Tensor images, std::vector<torch::Tensor> packed, int64_t norm, int64_t output_dim) {
-  const Expect expect("encoder_forward", images, "images");
-  expect(images, "images", {F32, F16}, dims({kAny, 3, kAny, kAny}));
-  TORCH_CHECK(norm == 0 || norm == 1, "encoder_forward: norm must be 0 (none) or 1 (instance)");
-  TORCH_CHECK(output_dim == 128 || output_dim == 256, "encoder_forward: output_dim must be 128 or 256");
-  TORCH_CHECK(packed.size() == 2 * DBA_ENCODER_CONVS, "encoder_forward: 28 packed tensors expected");
+// frames: null for f32 / f16 images (dba_encoder_forward), else uint8 camera frames in that format (dba_encoder_forward_frames)
+static torch::Tensor run_encoder(const char* fn, torch::Tensor images, const std::vector<torch::Tensor>& packed, int64_t norm, int64_t output_dim,
+                                 const dba_frame_format* frames) {
+  const Expect expect(fn, images, frames ? "frames" : "images");
+  if (frames) expect(images, "frames", torch::kUInt8, dims({kAny, 3, kAny, kAny}));
+  else expect(images, "images", {F32, F16}, dims({kAny, 3, kAny, kAny}));
+  TORCH_CHECK(norm == 0 || norm == 1, fn, ": norm must be 0 (none) or 1 (instance)");
+  TORCH_CHECK(output_dim == 128 || output_dim == 256, fn, ": output_dim must be 128 or 256");
+  TORCH_CHECK(packed.size() == 2 * DBA_ENCODER_CONVS, fn, ": 28 packed tensors expected");
   const int n = (int)images.size(0), H = (int)images.size(2), W = (int)images.size(3);
-  TORCH_CHECK(n > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, "encoder_forward: H and W must be positive multiples of 8, got ", H, "x", W);
+  TORCH_CHECK(n > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, fn, ": H and W must be positive multiples of 8, got ", H, "x", W);
   // [taps, N, Kpad] of each packed weight
   const int64_t shapes[DBA_ENCODER_CONVS][3] = {{1, 32, 192}, {9, 32, 64}, {9, 32, 64}, {9, 32, 64}, {9, 32, 64}, {1, 128, 320}, {9, 64, 64},
                                                 {9, 64, 64}, {9, 64, 64}, {1, 256, 576}, {9, 128, 128}, {9, 128, 128}, {9, 128, 128}, {1, output_dim, 128}};
@@ -671,13 +674,30 @@ torch::Tensor encoder_forward(torch::Tensor images, std::vector<torch::Tensor> p
   torch::Tensor ws;
   dba_encoder_args a;
   memset(&a, 0, sizeof(a));
-  a.images = images.data_ptr(); a.images_dtype = dtype_code(images, "encoder_forward");
+  a.images = images.data_ptr(); a.images_dtype = frames ? DBA_F32 : dtype_code(images, fn);
   a.n_images = n; a.H = H; a.W = W;
   a.weights = &Wt; a.norm = (int)norm; a.output_dim = (int)output_dim;
   a.out = out.data_ptr();
   a.workspace = workspace(ws_bytes, expect.dev, ws); a.workspace_bytes = ws_bytes; a.stream = cur_stream();
-  check_status(dba_encoder_forward(&a), "encoder_forward");
+  check_status(frames ? dba_encoder_forward_frames(&a, frames) : dba_encoder_forward(&a), fn);
   return out;
+}
+
+torch::Tensor encoder_forward(torch::Tensor images, std::vector<torch::Tensor> packed, int64_t norm, int64_t output_dim) {
+  return run_encoder("encoder_forward", images, packed, norm, output_dim, nullptr);
+}
+
+// encoder_forward on uint8 camera frames [n,3,H,W] (BGR when bgr, else RGB), normalised on load as the reference does in fp32:
+// x / 255 - mean[c], / std[c] per RGB channel (dba_encoder_forward_frames).  The same bits as encoder_forward on the normalised frames.
+torch::Tensor encoder_forward_frames(torch::Tensor frames, std::vector<torch::Tensor> packed, int64_t norm, int64_t output_dim, bool bgr,
+                                     std::vector<double> mean, std::vector<double> std) {
+  TORCH_CHECK(mean.size() == 3 && std.size() == 3, "droid_backends.encoder_forward_frames: mean and std must hold 3 values (one per RGB channel), got ",
+              mean.size(), " and ", std.size());
+  dba_frame_format f;
+  memset(&f, 0, sizeof(f));
+  f.channel_order = bgr ? DBA_FRAME_BGR : DBA_FRAME_RGB;
+  for (int c = 0; c < 3; c++) { f.mean[c] = (float)mean[c]; f.std[c] = (float)std[c]; }
+  return run_encoder("encoder_forward_frames", frames, packed, norm, output_dim, &f);
 }
 
 // channels-last tensor-core convolution (building block of update_forward).  src0 [E,ht,wd,C0] f16 (+ src1 [E,ht,wd,C1]),
@@ -777,6 +797,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("update_forward", &update_forward, "update operator (ConvGRU + heads + GraphAgg) on wgmma, native extension");
   m.def("encoder_forward", &encoder_forward, "feature / context encoder (BasicEncoder: fnet norm=1, cnet norm=0) on wgmma -> [n,output_dim,H/8,W/8] f16, native extension",
         pybind11::arg("images"), pybind11::arg("packed_weights"), pybind11::arg("norm"), pybind11::arg("output_dim"));
+  m.def("encoder_forward_frames", &encoder_forward_frames,
+        "encoder_forward on uint8 camera frames [n,3,H,W], channel reorder and normalisation on load -> [n,output_dim,H/8,W/8] f16, native extension",
+        pybind11::arg("frames"), pybind11::arg("packed_weights"), pybind11::arg("norm"), pybind11::arg("output_dim"), pybind11::arg("bgr"),
+        pybind11::arg("mean"), pybind11::arg("std"));
   m.def("conv_nhwc", &conv_nhwc,"channels-last 1x1/3x3 convolution on wgmma, native extension");
   m.def("cvx_upsample", &cvx_upsample, "convex upsampling of inverse depth maps (droid_net.cvx_upsample, dim = 1), native extension");
   m.def("proximity_edges", &proximity_edges, "edge selection of FactorGraph.add_proximity_factors (factor_graph.py:357-411), native extension");

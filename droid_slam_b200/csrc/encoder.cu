@@ -20,22 +20,39 @@ namespace dba {
 constexpr int kStemTaps = 147;    // 7 x 7 taps x 3 channels
 constexpr int kStemPitch = 152;   // im2col row pitch (16-byte rows)
 
-__device__ __forceinline__ float to_f32(float v) { return v; }
-__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+// How uint8 camera frames are normalised on load (dba_encoder_forward_frames); unused for f32 / f16 images.
+struct FrameNorm {
+  int bgr;                  // source channel of RGB channel c: 2 - c (BGR frames) or c
+  float inv255;             // 1.0f / 255.0f, rounded once in fp32 as ATen does for a division by a Python scalar
+  float mean[3], stdv[3];   // per RGB channel
+};
+
+// tap (channel c, pixel off) of image e: f32 / f16 images as stored; uint8 frames normalised exactly like the reference's ATen
+// sequence x / 255.0, .sub_(MEAN), .div_(STDV) on CUDA: a multiply by the fp32 reciprocal, a subtraction and an IEEE division, each
+// rounded on its own (the _rn intrinsics keep the compiler from contracting the first two into an fma)
+__device__ __forceinline__ float image_tap(const float* img, size_t plane, int c, size_t off, const FrameNorm&) { return img[c * plane + off]; }
+__device__ __forceinline__ float image_tap(const __half* img, size_t plane, int c, size_t off, const FrameNorm&) {
+  return __half2float(img[c * plane + off]);
+}
+__device__ __forceinline__ float image_tap(const uint8_t* img, size_t plane, int c, size_t off, const FrameNorm& f) {
+  const float x = (float)img[(f.bgr ? 2 - c : c) * plane + off];
+  return __fdiv_rn(__fsub_rn(__fmul_rn(x, f.inv255), f.mean[c]), f.stdv[c]);
+}
 
 // conv1's im2col: dst[(e*Ho*Wo + p) * 152 + (dy*7 + dx)*3 + c] = f16(img[e][c][2y+dy-3][2x+dx-3]) (0 outside; K 147..151 = 0).
 // CTA = 64 output pixels of one output row; the 3 x 7 x 133 input halo goes through shared memory.
 template <typename T>
-__global__ void __launch_bounds__(256) image_im2col_kernel(const T* __restrict__ img, __half* __restrict__ dst, int H, int W) {
+__global__ void __launch_bounds__(256) image_im2col_kernel(const T* __restrict__ img, __half* __restrict__ dst, int H, int W, FrameNorm fn) {
   constexpr int kCols = 2 * 64 + 5;
   __shared__ float halo[3][7][kCols];
   const int e = blockIdx.z, y = blockIdx.y, x0 = blockIdx.x * 64;
   const int Ho = H >> 1, Wo = W >> 1;
+  const size_t plane = (size_t)H * W;
   for (int i = threadIdx.x; i < 3 * 7 * kCols; i += 256) {
     const int c = i / (7 * kCols), r = (i - c * 7 * kCols) / kCols, col = i - c * 7 * kCols - r * kCols;
     const int yy = 2 * y + r - 3, xx = 2 * x0 + col - 3;
     float v = 0.f;
-    if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = to_f32(img[((size_t)e * 3 + c) * H * W + (size_t)yy * W + xx]);
+    if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = image_tap(img + (size_t)e * 3 * plane, plane, c, (size_t)yy * W + xx, fn);
     halo[c][r][col] = v;
   }
   __syncthreads();
@@ -284,8 +301,9 @@ static int enc_block_s2(Enc& c, bool inorm, int ht, int wd, int Cin, int P, __ha
 }
 
 // the schedule of both encoders: launches its first `limit` kernels (limit 0: none, the tilings and the launch count only, with a
-// null workspace) and reports how many it has in all and, in plans, each convolution's tiling
-static int enc_forward(const dba_encoder_args* a, int limit, int* n_launches, int* plans) {
+// null workspace) and reports how many it has in all and, in plans, each convolution's tiling.  frames set: a->images are uint8
+// camera frames normalised on load by that format.
+static int enc_forward(const dba_encoder_args* a, int limit, int* n_launches, int* plans, const dba_frame_format* frames = nullptr) {
   const int E = a->n_images, H = a->H, W = a->W;
   const dba_encoder_weights* Wt = a->weights;
   const EncWs L = enc_layout(E, H, W);
@@ -304,8 +322,18 @@ static int enc_forward(const dba_encoder_args* a, int limit, int* n_launches, in
   // conv1 7x7/2 3->32, norm1, relu1 (extractor.py:187-189)
   if (enc_next(c)) {
     const dim3 g((w1 + 63) / 64, h1, E);
-    if (a->images_dtype == DBA_F32) image_im2col_kernel<float><<<g, 256, 0, st>>>((const float*)a->images, big, H, W);
-    else image_im2col_kernel<__half><<<g, 256, 0, st>>>((const __half*)a->images, big, H, W);
+    FrameNorm fn;
+    memset(&fn, 0, sizeof(fn));
+    if (frames) {
+      fn.bgr = frames->channel_order == DBA_FRAME_BGR;
+      fn.inv255 = 1.0f / 255.0f;
+      for (int c = 0; c < 3; c++) { fn.mean[c] = frames->mean[c]; fn.stdv[c] = frames->std[c]; }
+      image_im2col_kernel<uint8_t><<<g, 256, 0, st>>>((const uint8_t*)a->images, big, H, W, fn);
+    } else if (a->images_dtype == DBA_F32) {
+      image_im2col_kernel<float><<<g, 256, 0, st>>>((const float*)a->images, big, H, W, fn);
+    } else {
+      image_im2col_kernel<__half><<<g, 256, 0, st>>>((const __half*)a->images, big, H, W, fn);
+    }
     DBA_CHECK_LAUNCH("image_im2col_kernel");
   }
   const ConvSrc stem{big, kStemTaps, kStemPitch};
@@ -353,21 +381,31 @@ extern "C" int dba_encoder_workspace_layout(int n_images, int H, int W, int norm
   return enc_forward(&a, 0, n_launches, plans);
 }
 
-extern "C" int dba_encoder_forward_prefix(const dba_encoder_args* a, int n_launches) {
+static int enc_checked(const dba_encoder_args* a, int n_launches, const dba_frame_format* frames) {
   DBA_CHECK_ARG(a, "null args");
   const int E = a->n_images, H = a->H, W = a->W;
   DBA_CHECK_ARG(n_launches >= 0, "encoder: negative launch count");
   DBA_CHECK_ARG(E > 0 && H > 0 && W > 0 && H % 8 == 0 && W % 8 == 0, "encoder: n_images must be positive and H, W positive multiples of 8");
   DBA_CHECK_ARG(a->norm == 0 || a->norm == 1, "encoder: norm must be 0 (none) or 1 (instance)");
   DBA_CHECK_ARG(a->output_dim == 128 || a->output_dim == 256, "encoder: output_dim must be 128 or 256");
-  DBA_CHECK_ARG(a->images_dtype == DBA_F32 || a->images_dtype == DBA_F16, "encoder: images must be DBA_F32 or DBA_F16");
+  if (frames)
+    DBA_CHECK_ARG(frames->channel_order == DBA_FRAME_RGB || frames->channel_order == DBA_FRAME_BGR, "encoder: channel_order must be DBA_FRAME_RGB or DBA_FRAME_BGR");
+  else
+    DBA_CHECK_ARG(a->images_dtype == DBA_F32 || a->images_dtype == DBA_F16, "encoder: images must be DBA_F32 or DBA_F16");
   DBA_CHECK_ARG(a->images && a->weights && a->out && a->workspace, "null pointer");
   const dba_encoder_weights* Wt = a->weights;
   for (int k = 0; k < DBA_ENCODER_CONVS; k++)
     DBA_CHECK_ARG(Wt->w[k] && Wt->b[k] && ((uintptr_t)Wt->w[k] & 15) == 0, "encoder: packed weights must be non-null, w[k] 16-byte aligned");
   if (a->workspace_bytes < enc_layout(E, H, W).total) { set_error("invalid argument: workspace too small (dba_encoder_workspace_bytes)"); return DBA_ERR_WORKSPACE; }
   DBA_CHECK_ARG(((uintptr_t)a->workspace & 255) == 0, "encoder: workspace must be 256-byte aligned");
-  return enc_forward(a, n_launches, nullptr, nullptr);
+  return enc_forward(a, n_launches, nullptr, nullptr, frames);
 }
 
-extern "C" int dba_encoder_forward(const dba_encoder_args* a) { return dba_encoder_forward_prefix(a, INT_MAX); }
+extern "C" int dba_encoder_forward_prefix(const dba_encoder_args* a, int n_launches) { return enc_checked(a, n_launches, nullptr); }
+
+extern "C" int dba_encoder_forward(const dba_encoder_args* a) { return enc_checked(a, INT_MAX, nullptr); }
+
+extern "C" int dba_encoder_forward_frames(const dba_encoder_args* a, const dba_frame_format* f) {
+  DBA_CHECK_ARG(f, "encoder: null frame format");
+  return enc_checked(a, INT_MAX, f);
+}

@@ -25,6 +25,9 @@ kernel for is offered as a hook:
   * `fill_trajectory(filler, stream)` / `install_trajectory_filler_hook(trajectory_filler)`: `PoseTrajectoryFiller.__call__`
     (trajectory_filler.py:42-110) with on-device pose interpolation (`droid_backends.fill_interpolate`), batches sized by free device
     memory and a one-launch motion-only BA per update (`droid_backends.pose_only_ba`).
+  * `track(filter, ...)` / `install_motion_filter_hook(motion_filter)`: `MotionFilter.track` (motion_filter.py:50-91) with camera frames
+    fed straight into the encoders (`droid_backends.encoder_forward_frames`), the motion probe on the correlation kernels and one host
+    read per frame (row F6).
 """
 import sys
 
@@ -34,7 +37,7 @@ from . import install
 
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
-           "install_trajectory_filler_hook"]
+           "install_trajectory_filler_hook", "track", "install_motion_filter_hook"]
 
 
 def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
@@ -189,16 +192,8 @@ def install_encoder_hook(extractor_module, strict=True):
     output_dim other than 128 / 256, inputs not f16/f32 on CUDA, H or W not a multiple of 8) raise; with strict=False the reference's own
     forward runs for them.  Forward only: an input that requires grad under grad mode raises, and the parameters get no gradient."""
     be = install()
-    from .encoder import pack_encoder_weights
     cls = extractor_module.BasicEncoder
     ref_forward = cls.forward
-
-    def packed(self, device):
-        key = (str(device),) + tuple((p.data_ptr(), p._version) for p in self.parameters())
-        if getattr(self, "_b200_packed_key", None) != key:
-            self._b200_packed = pack_encoder_weights(self.state_dict(), self.norm_fn, self.conv2.out_channels, device)
-            self._b200_packed_key = key
-        return self._b200_packed
 
     def forward(self, x):
         why = _encoder_unsupported(self, x)
@@ -209,7 +204,7 @@ def install_encoder_hook(extractor_module, strict=True):
         if torch.is_grad_enabled() and x.requires_grad:
             raise RuntimeError("the native BasicEncoder is forward only: the input requires grad")
         b, n, c, h, w = x.shape
-        out = be.encoder_forward(x.reshape(b * n, c, h, w).contiguous(), packed(self, x.device), 1 if self.norm_fn == "instance" else 0,
+        out = be.encoder_forward(x.reshape(b * n, c, h, w).contiguous(), _packed_encoder(self, x.device), 1 if self.norm_fn == "instance" else 0,
                                  self.conv2.out_channels)
         if not torch.is_autocast_enabled("cuda"):
             out = out.to(x.dtype)
@@ -218,6 +213,35 @@ def install_encoder_hook(extractor_module, strict=True):
     forward._b200_native = True
     cls.forward = forward
     return extractor_module
+
+
+def _packed_encoder(enc, device):
+    """the BasicEncoder's parameters in the kernels' layout, packed once and re-packed when a parameter's storage or version changes"""
+    from .encoder import pack_encoder_weights
+    key = (str(device),) + tuple((p.data_ptr(), p._version) for p in enc.parameters())
+    if getattr(enc, "_b200_packed_key", None) != key:
+        enc._b200_packed = pack_encoder_weights(enc.state_dict(), enc.norm_fn, enc.conv2.out_channels, device)
+        enc._b200_packed_key = key
+    return enc._b200_packed
+
+
+def _frame_norm(owner):
+    """owner.MEAN / owner.STDV (the reference's [3,1,1] normalisation constants, possibly on the device) as two lists of 3 floats; read
+    from the device once and again only when either tensor is replaced or modified"""
+    key = tuple((t.data_ptr(), t._version) for t in (owner.MEAN, owner.STDV))
+    cached = getattr(owner, "_b200_frame_norm", None)
+    if cached is None or cached[0] != key:
+        cached = (key, owner.MEAN.reshape(-1).tolist(), owner.STDV.reshape(-1).tolist())
+        owner._b200_frame_norm = cached
+    return cached[1], cached[2]
+
+
+def _encode_frames(be, enc, frames, norm):
+    """a BasicEncoder under install_encoder_hook on uint8 BGR camera frames [n,3,H,W] on the device -> [n,output_dim,H/8,W/8] f16, with the
+    reference's channel flip and normalisation (norm = _frame_norm(...)) done on load by the encoder's first kernel: the bits of the
+    hooked forward under autocast on `(frames[:, [2, 1, 0]] / 255.0).sub_(MEAN).div_(STDV)`, without that fp32 copy"""
+    return be.encoder_forward_frames(frames.contiguous(), _packed_encoder(enc, frames.device), 1 if enc.norm_fn == "instance" else 0,
+                                     enc.conv2.out_channels, True, norm[0], norm[1])
 
 
 def reproject(poses, disps, intrinsics, ii, jj):
@@ -549,12 +573,12 @@ def _filler_unsupported(filler):
 def _filler_frame_budget(be, ht, wd, device):
     """the most frames one fill_trajectory batch takes: a quarter of the free device memory over what one frame needs -- two edges, each
     with its volume pyramid (f16, four levels), its share of the update operator's workspace, its corr features, hidden state and outputs;
-    and the frame's image (64 hw pixels x 3 channels) as uint8 on the device, its normalised fp32 copy and the fp32 temporary made on the
-    way, its feature map (f16, 128 channels) and its pose / intrinsics rows"""
+    and the frame's image (64 hw pixels x 3 channels) as uint8 on the device (fnet normalises it on load), its feature map (f16, 128
+    channels) and its pose / intrinsics rows"""
     hw = ht * wd
     volume = 2 * sum(hw * (ht >> l) * (wd >> l) for l in range(4))
     per_edge = volume + -(-be.update_workspace_bytes(64, 64, ht, wd) // 64) + hw * (196 * 2 + 128 * 2 * 3 + 2 * 2 * 4 * 4 + 4 * 4)
-    per_image = 64 * hw * 3 * (1 + 4 + 4) + hw * 128 * 2 + 4 * (7 + 4)
+    per_image = 64 * hw * 3 + hw * 128 * 2 + 4 * (7 + 4)
     free, _ = torch.cuda.mem_get_info(device)
     return max(1, (free // 4) // (2 * per_edge + per_image))
 
@@ -575,9 +599,10 @@ def _fill_batch(be, filler, tstamps, images, intrinsics):
     tt = _pinned_to(dev, torch.as_tensor(tstamps))
     images = _pinned_to(dev, torch.stack(images, 0))
     intr = _pinned_to(dev, torch.stack(intrinsics, 0)) / 8.0
-    inputs = (images.flip(2) / 255.0).sub_(filler.MEAN).div_(filler.STDV)        # images[:, :, [2, 1, 0]] without an index upload
-    with torch.autocast("cuda", enabled=True):
-        fmap = torch.cat([filler.fnet(inputs[a:a + _FNET_IMAGES]) for a in range(0, M, _FNET_IMAGES)])
+    norm = _frame_norm(filler)
+    cams, H, W = images.shape[1], images.shape[-2], images.shape[-1]
+    fmap = torch.cat([_encode_frames(be, filler.fnet, images[a:a + _FNET_IMAGES].reshape(-1, 3, H, W), norm).view(-1, cams, ch, ht, wd)
+                      for a in range(0, M, _FNET_IMAGES)])
     t0, t1, G = be.fill_interpolate(video.poses[:N].contiguous(), video.tstamp[:N].contiguous(), tt.float().contiguous())
 
     host = torch.stack([t0, t1]).cpu()                                   # the one host read: the edge list
@@ -661,3 +686,119 @@ def install_trajectory_filler_hook(trajectory_filler_module, strict=True):
 
     cls.__call__ = __call__
     return trajectory_filler_module
+
+
+# ---- MotionFilter ----------------------------------------------------------------------------------------------------------------------
+
+def _motion_filter_unsupported(be, filt, image):
+    """why track cannot run this MotionFilter on this frame natively (None: it can)"""
+    from .update import UpdateModule
+    if not isinstance(filt.update, UpdateModule):
+        return "filter.update is %s, not droid_slam_b200.update.UpdateModule" % type(filt.update).__name__
+    for name in ("fnet", "cnet"):
+        enc = getattr(filt, name)
+        if not getattr(type(enc).forward, "_b200_native", False):
+            return "filter.%s (%s) is not a BasicEncoder under install_encoder_hook" % (name, type(enc).__name__)
+    video = filt.video
+    for name in ("tstamp", "images", "poses", "disps", "disps_sens", "intrinsics", "fmaps", "nets", "inps"):
+        t = getattr(video, name, None)
+        if not (isinstance(t, torch.Tensor) and t.is_cuda):
+            return "video.%s is not a CUDA tensor" % name
+    if not (isinstance(image, torch.Tensor) and image.dim() == 4 and image.shape[1] == 3 and image.dtype == torch.uint8):
+        return "the image must be a uint8 tensor [cameras,3,H,W]"
+    H, W = image.shape[-2:]
+    if H % 8 or W % 8:
+        return "%dx%d images (H and W must be multiples of 8)" % (H, W)
+    if H < 64 or W < 64 or not be.corr_volume_supported(128, H // 8, W // 8):
+        return "no correlation volume kernel for %dx%d feature maps" % (H // 8, W // 8)
+    return None
+
+
+def _probe_grid(filt, ht, wd, dev):
+    """the identity grid pops.coords_grid(ht, wd) as [1,2,ht,wd] (x, y) and the one-entry index of the probe's volume, cached per size"""
+    key = (ht, wd, str(dev))
+    cached = getattr(filt, "_b200_probe_grid", None)
+    if cached is None or cached[0] != key:
+        y, x = torch.meshgrid(torch.arange(ht, device=dev).float(), torch.arange(wd, device=dev).float(), indexing="ij")
+        cached = (key, torch.stack([x, y])[None].contiguous(), torch.zeros(1, dtype=torch.long, device=dev))
+        filt._b200_probe_grid = cached
+    return cached[1], cached[2]
+
+
+def _context(be, filt, frames, norm):
+    """MotionFilter.__context_encoder (motion_filter.py:39-43) on camera 0 of the frames: net, inp [1,128,ht,wd] f16"""
+    out = _encode_frames(be, filt.cnet, frames[:1], norm)
+    net, inp = out[None].split([128, 128], dim=2)
+    return net.tanh().squeeze(0), inp.relu().squeeze(0)
+
+
+def track(filt, tstamp, image, depth=None, intrinsics=None):
+    """MotionFilter.track (reference motion_filter.py:50-91) with the same signature and effects, `filt` being the reference's MotionFilter
+    (or an object with its attributes: fnet, cnet, update, video, thresh, count, MEAN, STDV) -- the filter's net, inp, fmap and count and
+    the video's buffers and counter, bit for bit as the reference method on the same operators.
+
+    Per frame: the frame goes up through pinned staging without blocking; fnet takes the uint8 frames as stored (the BGR -> RGB flip and
+    the normalisation happen in its first kernel, droid_backends.encoder_forward_frames); the motion probe builds the correlation volume
+    of the last keyframe's and this frame's camera-0 features (corr_volume_pyramid) and looks it up on the identity grid
+    (corr_lookup_pyramid), as CorrBlock under install_corr_volume_hook does; the update operator runs once without aggregation; the
+    statistic is the reference's own `delta.norm(dim=-1).mean()`, and reading it is the one host read of the frame.  A keyframe (the
+    statistic strictly above thresh, or the video's first frame) runs cnet on camera 0 and goes through `video.append`, so the video's lock
+    and counter logic stay the video's.  Kept from the reference: the first frame writes net[0,0] / inp[0,0] (channel 0, broadcast over
+    the video's 128 channels) and the identity pose and disparity 1.0; later keyframes write neither pose nor disparity; the depth
+    (RGB-D) goes to the video as given, whose setter samples and inverts it; intrinsics are divided by 8.  Raises when the filter or the
+    frame cannot run natively (see install_motion_filter_hook)."""
+    be = install()
+    why = _motion_filter_unsupported(be, filt, image)
+    if why is not None:
+        raise RuntimeError("the native motion filter cannot run this frame: %s" % why)
+    video = filt.video
+    dev = video.poses.device
+    ht, wd = image.shape[-2] // 8, image.shape[-1] // 8
+    norm = _frame_norm(filt)
+    with torch.no_grad():
+        frames = _pinned_to(dev, image)
+        gmap = _encode_frames(be, filt.fnet, frames, norm)                     # [cameras,128,ht,wd]
+        if video.counter.value == 0:
+            keyframe, pose, disp = True, video.poses.new_zeros(7), 1.0
+            pose[6] = 1                                                         # lietorch.SE3.Identity(1).data
+        else:
+            coords_t, idx = _probe_grid(filt, ht, wd, dev)
+            tiled = be.corr_volume_supported(128, ht, wd, True)
+            pyr = be.corr_volume_pyramid(filt.fmap[:1].contiguous(), gmap[:1].contiguous(), idx, idx, tiled)
+            corr = be.corr_lookup_pyramid(pyr, coords_t, tiled).view(1, 1, -1, ht, wd)
+            _, delta, _ = filt.update.forward_segments(filt.net[None], filt.inp[None], corr, None, None, 0)
+            with torch.autocast("cuda", enabled=True):
+                stat = delta.norm(dim=-1).mean()
+            keyframe, pose, disp = stat.item() > filt.thresh, None, None         # the one host read
+        if not keyframe:
+            filt.count += 1
+            return
+        with torch.autocast("cuda", enabled=True):
+            net, inp = _context(be, filt, frames, norm)
+        first = pose is not None
+        if not first:
+            filt.count = 0
+        filt.net, filt.inp, filt.fmap = net, inp, gmap
+        if depth is not None:
+            depth = _pinned_to(dev, depth)
+        intr = _pinned_to(dev, intrinsics) / 8.0
+        # the stamp as a device scalar: the video's `tstamp[i] = stamp` then copies on the device instead of synchronising the host
+        ts = _pinned_to(dev, torch.as_tensor(tstamp, dtype=video.tstamp.dtype))
+        video.append(ts, frames[0], pose, disp, depth, intr, gmap, net[0, 0] if first else net[0], inp[0, 0] if first else inp[0])
+
+
+def install_motion_filter_hook(motion_filter_module, strict=True):
+    """motion_filter_module = the imported reference module `motion_filter`.  Replaces `MotionFilter.track` (motion_filter.py:50-91) by
+    track above.  strict: a filter or frame the native path cannot run (update not droid_slam_b200.update.UpdateModule, fnet or cnet not a
+    BasicEncoder under install_encoder_hook, video tensors not on CUDA, a frame size without a kernel) raises, naming the reason; with
+    strict=False the reference's own method runs for it."""
+    cls = motion_filter_module.MotionFilter
+    ref_track = cls.track
+
+    def _track(self, tstamp, image, depth=None, intrinsics=None):
+        if not strict and _motion_filter_unsupported(install(), self, image) is not None:
+            return ref_track(self, tstamp, image, depth, intrinsics)
+        return track(self, tstamp, image, depth, intrinsics)
+
+    cls.track = _track
+    return motion_filter_module

@@ -297,3 +297,25 @@ def make_update_inputs(E=5, ht=6, wd=8, seed=0, n_src=3):
     flow = 4.0 * torch.randn(1, E, 4, ht, wd, generator=g)
     ii = torch.randint(0, n_src, (E,), generator=g) * 3 + 2          # unsorted, non-contiguous frame numbers
     return net, inp, corr, flow, ii
+
+
+def make_frames(n, H, W, cams=1, seed=0, still=0.5, move=6.0, margin=32):
+    """n synthetic camera frames, uint8 [n,cams,3,H,W]: one smooth random texture seen through a camera that pans by a bounded random
+    walk, each frame's step either small (up to `still` pixels) or large (up to `move` pixels) at random; camera k of a rig looks 8k
+    pixels to the right of camera 0.  Inputs for MotionFilter.track with frames on both sides of its motion threshold."""
+    g = torch.Generator().manual_seed(9137 + seed)
+    hh, ww = H + 2 * margin, W + 2 * margin + 8 * (cams - 1)
+    coarse = torch.rand(1, 3, hh // 16 + 2, ww // 16 + 2, generator=g)
+    fine = torch.rand(1, 3, hh // 4 + 2, ww // 4 + 2, generator=g)
+    tex = 0.7 * F.interpolate(coarse, size=(hh, ww), mode="bilinear", align_corners=False)[0] \
+        + 0.3 * F.interpolate(fine, size=(hh, ww), mode="bilinear", align_corners=False)[0]
+    tex = (255 * tex).round().clamp(0, 255).to(torch.uint8)
+    out = torch.empty(n, cams, 3, H, W, dtype=torch.uint8)
+    pos = torch.zeros(2)
+    for k in range(n):
+        size = still if float(torch.rand(1, generator=g)) < 0.5 else move
+        pos = (pos + size * (2 * torch.rand(2, generator=g) - 1)).clamp(-margin, margin)
+        y, x = margin + int(round(float(pos[0]))), margin + int(round(float(pos[1])))
+        for c in range(cams):
+            out[k, c] = tex[:, y:y + H, x + 8 * c:x + 8 * c + W]
+    return out

@@ -366,6 +366,18 @@ typedef struct {
 size_t dba_encoder_workspace_bytes(int n_images, int H, int W, int output_dim);
 int dba_encoder_forward(const dba_encoder_args* a);
 
+/* camera frames straight into the encoders: dba_encoder_forward on a->images = uint8 frames [n_images,3,H,W] in the format's channel
+ * order (a->images_dtype is ignored).  Each tap is reordered to RGB and normalised in fp32 as the reference's ATen sequence on CUDA does
+ * it (motion_filter.py:62-63: x / 255.0, .sub_(MEAN), .div_(STDV)): x * (1.0f / 255.0f), then - mean[c], then an IEEE division by
+ * std[c], each step rounded to fp32, c the RGB channel; then rounded to f16 like the DBA_F32 path.  The output equals
+ * dba_encoder_forward on the normalised fp32 frames bit for bit; the fp32 frames are never stored.  Same workspace. */
+enum { DBA_FRAME_RGB = 0, DBA_FRAME_BGR = 1 };
+typedef struct {
+  int channel_order;                                   /* DBA_FRAME_RGB, or DBA_FRAME_BGR (reversed to RGB on load) */
+  float mean[3], std[3];                               /* per RGB channel */
+} dba_frame_format;
+int dba_encoder_forward_frames(const dba_encoder_args* a, const dba_frame_format* f);
+
 /* host only: where dba_encoder_forward keeps its intermediates, from the layout and the schedule it uses itself (for tests that check
  * each launch on what the previous one wrote).  offsets / sizes [DBA_ENCWS_COUNT]: byte offset from the workspace start and size of
  *   BIG  f16  the im2col rows [n,H/2,W/2,152] (147 used), then the gathered 3x3/2 taps [n,h/2,w/2,9C] of layer2.0 and layer3.0
