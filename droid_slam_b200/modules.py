@@ -28,6 +28,10 @@ kernel for is offered as a hook:
   * `track(filter, ...)` / `install_motion_filter_hook(motion_filter)`: `MotionFilter.track` (motion_filter.py:50-91) with camera frames
     fed straight into the encoders (`droid_backends.encoder_forward_frames`), the motion probe on the correlation kernels and one host
     read per frame (row F6).
+
+The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
+it.  If not, strict=True (the default) raises RuntimeError naming the replaced method and the reason; strict=False runs the reference's
+own method.  `update`, `update_lowmem`, `fill_trajectory` and `track` called directly raise in the same words.
 """
 import sys
 
@@ -38,6 +42,82 @@ from . import install
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
            "install_trajectory_filler_hook", "track", "install_motion_filter_hook"]
+
+
+def _require(entry, why):
+    """raise for a call of `entry` the native path cannot run (why: the reason; None: it can run it)"""
+    if why is not None:
+        raise RuntimeError("%s has no kernel for this call: %s" % (entry, why))
+
+
+def _replace(cls, name, native, unsupported, strict):
+    """replace the method `name` of the reference's class `cls` by native(self, ...) under the strict policy; unsupported(self, ...)
+    takes the same arguments and gives why the native path cannot run the call (None: it can)"""
+    ref = getattr(cls, name)
+
+    def method(self, *args, **kwargs):
+        why = unsupported(self, *args, **kwargs)
+        if why is not None and not strict:
+            return ref(self, *args, **kwargs)
+        _require("%s.%s" % (cls.__name__, name), why)
+        return native(self, *args, **kwargs)
+
+    setattr(cls, name, method)
+
+
+def _graph_unsupported(who, obj, update, encoders=(), own=(), video=()):
+    """why `obj` (`who` in the reason) cannot run natively for its operators and buffers (None: it can): obj.<update> must be
+    droid_slam_b200.update.UpdateModule, obj.<encoders> under install_encoder_hook, obj.<own> and obj.video.<video> CUDA tensors"""
+    from .update import UpdateModule
+    if not isinstance(getattr(obj, update), UpdateModule):
+        return "%s.%s is %s, not droid_slam_b200.update.UpdateModule" % (who, update, type(getattr(obj, update)).__name__)
+    for name in encoders:
+        if not getattr(type(getattr(obj, name)).forward, "_b200_encoder_hook", False):
+            return "%s.%s (%s) is not a BasicEncoder under install_encoder_hook" % (who, name, type(getattr(obj, name)).__name__)
+    for prefix, owner, names in ((who, obj, own), ("video", obj.video, video)):
+        for name in names:
+            t = getattr(owner, name, None)
+            if not (isinstance(t, torch.Tensor) and t.is_cuda):
+                return "%s.%s is not a CUDA tensor" % (prefix, name)
+    return None
+
+
+def _repack_key(tensors):
+    """(data_ptr, version) of each tensor: a cache built from them is stale once this changes (a tensor replaced or modified in place)"""
+    return tuple((t.data_ptr(), t._version) for t in tensors)
+
+
+def _stage(dev, *tensors):
+    """tensors to the device without a host synchronisation, shapes kept.  One tensor: by pinned staging and a non-blocking copy, or
+    passed through when already on the device.  Several CPU tensors of one dtype: in one such copy, as views of one buffer."""
+    if len(tensors) > 1:
+        flat = _stage(dev, torch.cat([t.reshape(-1) for t in tensors]))
+        return [v.view(t.shape) for v, t in zip(torch.split(flat, [t.numel() for t in tensors]), tensors)]
+    return tensors[0].to(dev) if tensors[0].is_cuda else tensors[0].pin_memory().to(dev, non_blocking=True)
+
+
+def _update_edge_bytes(be, ht, wd):
+    """one edge's share of the update operator's workspace, every edge its own source frame"""
+    return -(-be.update_workspace_bytes(64, 64, ht, wd) // 64)
+
+
+def _quarter_free(device, unit_bytes):
+    """how many units of unit_bytes a quarter of the free device memory holds, at least 1"""
+    free, _ = torch.cuda.mem_get_info(device)
+    return max(1, (free // 4) // unit_bytes)
+
+
+def _volumes(be, fmap1, fmap2, ii, jj, tiled=True):
+    """the 4-level correlation volumes of fmap1[ii] with fmap2[jj] (f16 [.,C,ht,wd]) -> (pyramid, tiled).  tiled: take the tiled private
+    layout (64-byte DRAM atoms) wherever corr_volume_pyramid has a tiled builder; otherwise, and with tiled=False, the reference layout"""
+    tiled = bool(tiled) and be.corr_volume_supported(*fmap1.shape[-3:], tiled=True)
+    return be.corr_volume_pyramid(fmap1, fmap2, ii, jj, tiled), tiled
+
+
+def _lookup(be, pyramid, tiled, coords_t):
+    """the one-launch 4-level lookup of volumes from _volumes (or CorrBlock's) at coords_t [n,2,ht,wd] -> [1,n,196,ht,wd]"""
+    n, _, ht, wd = coords_t.shape
+    return be.corr_lookup_pyramid([v.contiguous() for v in pyramid], coords_t, tiled).view(1, n, -1, ht, wd)
 
 
 def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
@@ -62,40 +142,34 @@ def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
 
 def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
     """corr_module = the imported reference module `modules.corr`.  `CorrBlock.__init__` builds its pyramid with corr_volume_pyramid for
-    f16 feature maps with 128 channels, 4 levels and ht, wd >= 8.  strict: anything else raises (naming the reason) instead of silently
-    taking the reference's library path; with strict=False the reference's own methods run for it.
+    f16 feature maps with 128 channels, 4 levels and ht, wd >= 8; anything else follows the strict policy (module docstring).
     fused_lookup: additionally replace `CorrBlock.__call__` by the one-launch 4-level lookup `corr_lookup_pyramid`.  Where
     corr_volume_pyramid has a tiled builder (wd = 64, ht % 8 == 0) the volumes of levels 0 and 1 are kept in the tiled private layout
     (64-byte DRAM atoms, about a third less HBM traffic per lookup); elsewhere the reference layout.  Same tensor shapes, `cat` /
     `__getitem__` over edges keep working, results bit-identical to the reference-layout path."""
     be = install()
-    ref_init, ref_call = corr_module.CorrBlock.__init__, corr_module.CorrBlock.__call__
+    cls = corr_module.CorrBlock
+    ref_call = cls.__call__
 
     def __init__(self, fmap1, fmap2, num_levels=4, radius=3):
-        why = _corr_volume_unsupported(be, fmap1, fmap2, num_levels)
-        self._b200_native = why is None
-        if why is not None:
-            if strict:
-                raise RuntimeError("corr_volume_pyramid has no kernel for CorrBlock(%s %s, num_levels=%d): %s"
-                                   % (tuple(fmap1.shape), fmap1.dtype, num_levels, why))
-            return ref_init(self, fmap1, fmap2, num_levels, radius)
         batch, num, dim, ht, wd = fmap1.shape
-        tiled = bool(fused_lookup) and be.corr_volume_supported(dim, ht, wd, tiled=True)
         self.num_levels, self.radius = num_levels, radius
         idx = torch.arange(batch * num, device=fmap1.device)
-        self.corr_pyramid = be.corr_volume_pyramid(fmap1.reshape(batch * num, dim, ht, wd).contiguous(), fmap2.reshape(batch * num, dim, ht, wd).contiguous(), idx, idx, tiled)
-        self._b200_tiled = tiled
+        self.corr_pyramid, self._b200_tiled = _volumes(be, fmap1.reshape(batch * num, dim, ht, wd).contiguous(),
+                                                       fmap2.reshape(batch * num, dim, ht, wd).contiguous(), idx, idx, fused_lookup)
 
     def __call__(self, coords):
-        if not getattr(self, "_b200_native", False):
+        if self._b200_tiled is None:
             return ref_call(self, coords)
         batch, num, ht, wd, _ = coords.shape
         c = coords.permute(0, 1, 4, 2, 3).contiguous().view(batch * num, 2, ht, wd)
-        return be.corr_lookup_pyramid([v.contiguous() for v in self.corr_pyramid], c, self._b200_tiled).view(batch, num, -1, ht, wd)
+        return _lookup(be, self.corr_pyramid, self._b200_tiled, c).view(batch, num, -1, ht, wd)
 
-    corr_module.CorrBlock.__init__ = __init__
+    cls._b200_tiled = None                      # a block's volume layout (True: tiled); None where the reference's constructor ran
+    _replace(cls, "__init__", __init__, lambda blk, fmap1, fmap2, num_levels=4, radius=3: _corr_volume_unsupported(be, fmap1, fmap2, num_levels),
+             strict)
     if fused_lookup:
-        corr_module.CorrBlock.__call__ = __call__
+        cls.__call__ = __call__
     return corr_module
 
 
@@ -123,41 +197,37 @@ def install_alt_corr_hook(corr_module, strict=True):
     """corr_module = the imported reference module `modules.corr`.  Replaces `AltCorrBlock.__init__(fmaps, num_levels=4, radius=3)` and
     `__call__(coords [B,M,H,W,2], ii, jj)` in place on the class (so `from modules.corr import AltCorrBlock` elsewhere picks it up) by
     the one-launch pyramid build and the one-launch all-level lookup on a private channels-last pyramid; the output equals the reference's
-    bit for bit.  strict: fmaps / radii without a kernel (not f16/f32 on CUDA, C % 8 != 0, radius != 3, more than 4 levels) raise; with
-    strict=False the reference's own methods run for them.  Forward only: inputs that require grad under grad mode raise (the hook would
-    otherwise drop their gradients)."""
+    bit for bit.  Kernels exist for f16/f32 fmaps on CUDA with C % 8 == 0, radius 3 and 1-4 levels; anything else follows the strict
+    policy (module docstring).  Forward only: inputs that require grad under grad mode raise, whichever constructor would run (the hook
+    would otherwise drop their gradients)."""
     be = install()
     cls = corr_module.AltCorrBlock
-    ref_init, ref_call = cls.__init__, cls.__call__
+    ref_call = cls.__call__
 
     def _no_grad_inputs(*ts):
         if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts):
             raise RuntimeError("the native AltCorrBlock is forward only: an input requires grad")
 
     def __init__(self, fmaps, num_levels=4, radius=3):
-        _no_grad_inputs(fmaps)
-        why = _alt_unsupported(fmaps, num_levels, radius)
-        if why is not None:
-            if strict:
-                raise RuntimeError("altcorr_pyramid has no kernel for AltCorrBlock(%s %s, num_levels=%d, radius=%d): %s"
-                                   % (tuple(fmaps.shape), fmaps.dtype, num_levels, radius, why))
-            self._b200_pyramid = None
-            return ref_init(self, fmaps, num_levels, radius)
         self.num_levels, self.radius = num_levels, radius
         self._b200_pyramid = be.altcorr_pyramid(fmaps.contiguous(), num_levels)
 
+    def unsupported(self, fmaps, num_levels=4, radius=3):
+        _no_grad_inputs(fmaps)                   # an input check, ahead of the policy
+        return _alt_unsupported(fmaps, num_levels, radius)
+
     def __call__(self, coords, ii, jj):
-        pyramid = getattr(self, "_b200_pyramid", None)
-        if pyramid is None:
+        if self._b200_pyramid is None:
             return ref_call(self, coords, ii, jj)
         _no_grad_inputs(coords)
         if not (coords.is_cuda and coords.dtype == torch.float32 and coords.dim() == 5 and coords.shape[-1] == 2):
             raise RuntimeError("AltCorrBlock: coords must be a float32 CUDA tensor [B,M,H,W,2], got %s %s on %s"
                                % (tuple(coords.shape), coords.dtype, coords.device))
         c = coords.permute(0, 1, 4, 2, 3).contiguous()
-        return be.altcorr_lookup_pyramid(pyramid, c, ii, jj, self.radius)
+        return be.altcorr_lookup_pyramid(self._b200_pyramid, c, ii, jj, self.radius)
 
-    cls.__init__ = __init__
+    cls._b200_pyramid = None                    # a block's private pyramid; None where the reference's constructor ran
+    _replace(cls, "__init__", __init__, unsupported, strict)
     cls.__call__ = __call__
     return corr_module
 
@@ -188,19 +258,12 @@ def install_encoder_hook(extractor_module, strict=True):
     the class (so droid_net.py, motion_filter.py and trajectory_filler.py pick it up unchanged) by one `encoder_forward` call: the
     module keeps the reference's parameters (a DROID checkpoint loads as before); they are packed once and re-packed when a parameter's
     storage or version changes.  Output [b,n,output_dim,H/8,W/8]: f16 under CUDA autocast (as the reference's last convolution gives),
-    otherwise the input's dtype.  strict: encoders and inputs without a kernel (norm_fn other than instance / none, multidim, dropout,
-    output_dim other than 128 / 256, inputs not f16/f32 on CUDA, H or W not a multiple of 8) raise; with strict=False the reference's own
-    forward runs for them.  Forward only: an input that requires grad under grad mode raises, and the parameters get no gradient."""
+    otherwise the input's dtype.  Kernels exist for norm_fn instance / none, no multidim, no dropout, output_dim 128 / 256 and f16/f32
+    inputs on CUDA with H and W multiples of 8; anything else follows the strict policy (module docstring).  Forward only: an input that
+    requires grad under grad mode raises, and the parameters get no gradient."""
     be = install()
-    cls = extractor_module.BasicEncoder
-    ref_forward = cls.forward
 
     def forward(self, x):
-        why = _encoder_unsupported(self, x)
-        if why is not None:
-            if strict:
-                raise RuntimeError("encoder_forward has no kernel for BasicEncoder(norm_fn=%r) on %s %s: %s" % (self.norm_fn, tuple(x.shape), x.dtype, why))
-            return ref_forward(self, x)
         if torch.is_grad_enabled() and x.requires_grad:
             raise RuntimeError("the native BasicEncoder is forward only: the input requires grad")
         b, n, c, h, w = x.shape
@@ -210,15 +273,15 @@ def install_encoder_hook(extractor_module, strict=True):
             out = out.to(x.dtype)
         return out.view(b, n, -1, h // 8, w // 8)
 
-    forward._b200_native = True
-    cls.forward = forward
+    _replace(extractor_module.BasicEncoder, "forward", forward, lambda enc, x: _encoder_unsupported(enc, x), strict)
+    extractor_module.BasicEncoder.forward._b200_encoder_hook = True          # what the filler and motion-filter checks look for
     return extractor_module
 
 
 def _packed_encoder(enc, device):
     """the BasicEncoder's parameters in the kernels' layout, packed once and re-packed when a parameter's storage or version changes"""
     from .encoder import pack_encoder_weights
-    key = (str(device),) + tuple((p.data_ptr(), p._version) for p in enc.parameters())
+    key = (str(device),) + _repack_key(enc.parameters())
     if getattr(enc, "_b200_packed_key", None) != key:
         enc._b200_packed = pack_encoder_weights(enc.state_dict(), enc.norm_fn, enc.conv2.out_channels, device)
         enc._b200_packed_key = key
@@ -228,7 +291,7 @@ def _packed_encoder(enc, device):
 def _frame_norm(owner):
     """owner.MEAN / owner.STDV (the reference's [3,1,1] normalisation constants, possibly on the device) as two lists of 3 floats; read
     from the device once and again only when either tensor is replaced or modified"""
-    key = tuple((t.data_ptr(), t._version) for t in (owner.MEAN, owner.STDV))
+    key = _repack_key((owner.MEAN, owner.STDV))
     cached = getattr(owner, "_b200_frame_norm", None)
     if cached is None or cached[0] != key:
         cached = (key, owner.MEAN.reshape(-1).tolist(), owner.STDV.reshape(-1).tolist())
@@ -312,30 +375,10 @@ _LOWMEM_CHUNK_FRAMES = 8      # the reference's chunk of source frames (factor_g
 
 def _factor_graph_unsupported(graph):
     """why the update hooks cannot run this graph natively (None: they can)"""
-    from .update import UpdateModule
-    if not isinstance(graph.update_op, UpdateModule):
-        return "graph.update_op is %s, not droid_slam_b200.update.UpdateModule" % type(graph.update_op).__name__
-    video = graph.video
-    for name, t in (("graph.ii", graph.ii), ("graph.net", graph.net), ("graph.target", graph.target), ("graph.damping", graph.damping),
-                    ("video.poses", video.poses), ("video.disps", video.disps), ("video.intrinsics", video.intrinsics)):
-        if not (isinstance(t, torch.Tensor) and t.is_cuda):
-            return "%s is not a CUDA tensor" % name
-    if graph.ii.numel() == 0:
+    why = _graph_unsupported("graph", graph, "update_op", own=("ii", "net", "target", "damping"), video=("poses", "disps", "intrinsics"))
+    if why is None and graph.ii.numel() == 0:
         return "the graph has no edges"
-    return None
-
-
-def _check_native(graph):
-    why = _factor_graph_unsupported(graph)
-    if why is not None:
-        raise RuntimeError("the native FactorGraph update cannot run this graph: %s" % why)
-
-
-def _to_device(dev, arrays):
-    """several CPU int64 tensors -> device views, in one pinned, non-blocking copy (no host synchronisation)"""
-    sizes = [a.numel() for a in arrays]
-    flat = torch.cat([a.reshape(-1).long() for a in arrays]).pin_memory().to(dev, non_blocking=True)
-    return list(torch.split(flat, sizes))
+    return why
 
 
 def _segments(ii):
@@ -347,16 +390,11 @@ def _corr_features(be, corr, coords, coords_t, ii=None, jj=None):
     """the graph's corr block looked up at coords [n,ht,wd,2] (coords_t: the same as [n,2,ht,wd]) -> [1,n,196,ht,wd].  A native block
     (CorrBlock under install_corr_volume_hook, AltCorrBlock under install_alt_corr_hook) goes straight to its one-launch lookup on
     coords_t; any other block is called through its own __call__."""
-    n, ht, wd, _ = coords.shape
     if ii is None:
-        if getattr(corr, "_b200_native", False):
-            pyr = [v.contiguous() for v in corr.corr_pyramid]
-            return be.corr_lookup_pyramid(pyr, coords_t, corr._b200_tiled).view(1, n, -1, ht, wd)
-        return corr(coords[None])
+        tiled = getattr(corr, "_b200_tiled", None)
+        return corr(coords[None]) if tiled is None else _lookup(be, corr.corr_pyramid, tiled, coords_t)
     pyramid = getattr(corr, "_b200_pyramid", None)
-    if pyramid is not None:
-        return be.altcorr_lookup_pyramid(pyramid, coords_t[None], ii, jj, corr.radius)
-    return corr(coords[None], ii, jj)
+    return corr(coords[None], ii, jj) if pyramid is None else be.altcorr_lookup_pyramid(pyramid, coords_t[None], ii, jj, corr.radius)
 
 
 def update(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
@@ -364,7 +402,11 @@ def update(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_
     (or an object with its attributes).  One host read plans the call (t0, the inactive edges BA uses, the source frames, BA's window);
     the motion features are one launch, the update operator one call without torch.unique, the write-back of target / weight / damping
     and BA's inputs one launch; then `video.ba` and `video.upsample` as in the reference.  Raises when the graph cannot run natively."""
-    _check_native(graph)
+    _require("FactorGraph.update", _factor_graph_unsupported(graph))
+    _update(graph, t0, t1, itrs, use_inactive, EP, motion_only)
+
+
+def _update(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
     be = install()
     video = graph.video
     dev = graph.ii.device
@@ -385,7 +427,7 @@ def update(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_
     if t1 is None:                               # what DepthVideo.ba computes with a host read of its own
         t1 = max(int(ii_ba.max()), int(jj_ba.max())) + 1
     src, seg = _segments(ii)
-    seg_d, src_d, ba_frames_d, inac_d, ii_ba_d, jj_ba_d = _to_device(dev, [seg, src, torch.unique(ii_ba), inac, ii_ba, jj_ba])
+    seg_d, src_d, ba_frames_d, inac_d, ii_ba_d, jj_ba_d = _stage(dev, seg, src, torch.unique(ii_ba), inac, ii_ba, jj_ba)
     n_inac = inac.numel()
 
     with torch.autocast("cuda", enabled=False):
@@ -412,10 +454,7 @@ def update(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_
 def _lowmem_edge_budget(be, ht, wd, device):
     """the most edges one update-operator call of update_lowmem takes: a quarter of the free device memory over what one edge needs
     (its share of the operator's workspace with every edge its own source frame, its corr features and the operator's outputs)"""
-    hw = ht * wd
-    per_edge = -(-be.update_workspace_bytes(64, 64, ht, wd) // 64) + hw * (196 * 2 + 128 * 2 + 2 * 2 * 4 + 4 + 576 * 2)
-    free, _ = torch.cuda.mem_get_info(device)
-    return max(1, (free // 4) // per_edge)
+    return _quarter_free(device, _update_edge_bytes(be, ht, wd) + ht * wd * (196 * 2 + 128 * 2 + 2 * 2 * 4 + 4 + 576 * 2))
 
 
 def plan_lowmem_chunks(ii, jj, max_edges):
@@ -468,7 +507,11 @@ def update_lowmem(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, 
     are gathered once per call.  Each step: one motion_features launch, per chunk the corr lookup, the update operator and
     graph_writeback, then video.upsample (when graph.upsample) and video.ba -- no host synchronisation.  graph.net is scattered back into
     graph order at the end of the call.  Raises when the graph cannot run natively."""
-    _check_native(graph)
+    _require("FactorGraph.update_lowmem", _factor_graph_unsupported(graph))
+    _update_lowmem(graph, t0, t1, itrs, use_inactive, EP, steps)
+
+
+def _update_lowmem(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, steps=8):
     be = install()
     video = graph.video
     dev = graph.ii.device
@@ -481,8 +524,8 @@ def update_lowmem(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, 
     ii_ba = torch.cat([host[2 * E:], ii])
     perm, chunks, src, seg = plan_lowmem_chunks(ii, jj, _lowmem_edge_budget(be, ht, wd, dev))
     ip, jp = ii[perm], jj[perm]
-    perm_d, seg_d, src_d, ii_alt_d, jj_alt_d, ba_frames_d = _to_device(
-        dev, [perm, seg, src, rig * ip, rig * jp + (ip == jp).long(), torch.unique(ii_ba)])
+    perm_d, seg_d, src_d, ii_alt_d, jj_alt_d, ba_frames_d = _stage(dev, perm, seg, src, rig * ip, rig * jp + (ip == jp).long(),
+                                                                   torch.unique(ii_ba))
 
     with torch.autocast("cuda", enabled=False):
         corr_op = _alt_corr_class(graph)(video.fmaps.view(1, num * rig, ch, ht, wd))
@@ -528,22 +571,11 @@ def update_lowmem(graph, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, 
 
 def install_factor_graph_hook(factor_graph_class, strict=True):
     """replace `update` and `update_lowmem` of the reference's FactorGraph class (factor_graph.py:214, :266) by the native versions above.
-    strict: a graph they cannot run (update_op not droid_slam_b200.update.UpdateModule, tensors not on CUDA, no edges) raises, naming the
-    reason; with strict=False the reference's own method runs for it."""
-    ref_update, ref_lowmem = factor_graph_class.update, factor_graph_class.update_lowmem
-
-    def _update(self, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, motion_only=False):
-        if not strict and _factor_graph_unsupported(self) is not None:
-            return ref_update(self, t0, t1, itrs, use_inactive, EP, motion_only)
-        return update(self, t0, t1, itrs, use_inactive, EP, motion_only)
-
-    def _update_lowmem(self, t0=None, t1=None, itrs=2, use_inactive=False, EP=1e-7, steps=8):
-        if not strict and _factor_graph_unsupported(self) is not None:
-            return ref_lowmem(self, t0, t1, itrs, use_inactive, EP, steps)
-        return update_lowmem(self, t0, t1, itrs, use_inactive, EP, steps)
-
-    factor_graph_class.update = _update
-    factor_graph_class.update_lowmem = _update_lowmem
+    They run graphs whose update_op is droid_slam_b200.update.UpdateModule, whose tensors are on CUDA and which have edges; any other
+    graph follows the strict policy (module docstring)."""
+    unsupported = lambda graph, *args, **kwargs: _factor_graph_unsupported(graph)          # noqa: E731
+    _replace(factor_graph_class, "update", _update, unsupported, strict)
+    _replace(factor_graph_class, "update_lowmem", _update_lowmem, unsupported, strict)
     return factor_graph_class
 
 
@@ -555,19 +587,10 @@ _FNET_IMAGES = 16     # images per fnet call: the reference's batch
 
 def _filler_unsupported(filler):
     """why fill_trajectory cannot run this PoseTrajectoryFiller natively (None: it can)"""
-    from .update import UpdateModule
-    if not isinstance(filler.update, UpdateModule):
-        return "filler.update is %s, not droid_slam_b200.update.UpdateModule" % type(filler.update).__name__
-    if not getattr(type(filler.fnet).forward, "_b200_native", False):
-        return "filler.fnet (%s) is not a BasicEncoder under install_encoder_hook" % type(filler.fnet).__name__
-    video = filler.video
-    for name in ("poses", "disps", "intrinsics", "tstamp", "fmaps", "nets", "inps"):
-        t = getattr(video, name, None)
-        if not (isinstance(t, torch.Tensor) and t.is_cuda):
-            return "video.%s is not a CUDA tensor" % name
-    if video.counter.value < 1:
+    why = _graph_unsupported("filler", filler, "update", ("fnet",), video=("poses", "disps", "intrinsics", "tstamp", "fmaps", "nets", "inps"))
+    if why is None and filler.video.counter.value < 1:
         return "the video has no keyframe"
-    return None
+    return why
 
 
 def _filler_frame_budget(be, ht, wd, device):
@@ -577,15 +600,9 @@ def _filler_frame_budget(be, ht, wd, device):
     channels) and its pose / intrinsics rows"""
     hw = ht * wd
     volume = 2 * sum(hw * (ht >> l) * (wd >> l) for l in range(4))
-    per_edge = volume + -(-be.update_workspace_bytes(64, 64, ht, wd) // 64) + hw * (196 * 2 + 128 * 2 * 3 + 2 * 2 * 4 * 4 + 4 * 4)
+    per_edge = volume + _update_edge_bytes(be, ht, wd) + hw * (196 * 2 + 128 * 2 * 3 + 2 * 2 * 4 * 4 + 4 * 4)
     per_image = 64 * hw * 3 + hw * 128 * 2 + 4 * (7 + 4)
-    free, _ = torch.cuda.mem_get_info(device)
-    return max(1, (free // 4) // (2 * per_edge + per_image))
-
-
-def _pinned_to(dev, t):
-    """a CPU tensor to the device without a host synchronisation (pinned staging, non-blocking copy); device tensors pass through"""
-    return t.to(dev) if t.is_cuda else t.pin_memory().to(dev, non_blocking=True)
+    return _quarter_free(device, 2 * per_edge + per_image)
 
 
 def _fill_batch(be, filler, tstamps, images, intrinsics):
@@ -596,9 +613,9 @@ def _fill_batch(be, filler, tstamps, images, intrinsics):
     dev = video.poses.device
     N, B, M = video.counter.value, video.poses.shape[0], len(tstamps)
     num, rig, ch, ht, wd = video.fmaps.shape
-    tt = _pinned_to(dev, torch.as_tensor(tstamps))
-    images = _pinned_to(dev, torch.stack(images, 0))
-    intr = _pinned_to(dev, torch.stack(intrinsics, 0)) / 8.0
+    tt = _stage(dev, torch.as_tensor(tstamps))
+    images = _stage(dev, torch.stack(images, 0))
+    intr = _stage(dev, torch.stack(intrinsics, 0)) / 8.0
     norm = _frame_norm(filler)
     cams, H, W = images.shape[1], images.shape[-2], images.shape[-1]
     fmap = torch.cat([_encode_frames(be, filler.fnet, images[a:a + _FNET_IMAGES].reshape(-1, 3, H, W), norm).view(-1, cams, ch, ht, wd)
@@ -612,7 +629,7 @@ def _fill_batch(be, filler, tstamps, images, intrinsics):
     jj = torch.cat([k, k[two]])
     ii = torch.where(ii < 0, ii + B, ii)     # t0 = -1: the reference's graph indexes slot -1 of the video's buffers, the last one
     E = ii.numel()
-    ii_d, jj_d, jloc_d = _to_device(dev, [ii, jj + B, jj])
+    ii_d, jj_d, jloc_d = _stage(dev, ii, jj + B, jj)
 
     with torch.autocast("cuda", enabled=False):
         poses = torch.cat([video.poses, G])
@@ -622,8 +639,7 @@ def _fill_batch(be, filler, tstamps, images, intrinsics):
             vol_i = ii_d
         else:                                # stereo buffers: gather the edges' left images
             f1, vol_i = video.fmaps[ii_d, 0], torch.arange(E, device=dev)
-        tiled = be.corr_volume_supported(ch, ht, wd, True)
-        pyr = be.corr_volume_pyramid(f1, fmap[:, 0].contiguous(), vol_i, jloc_d, tiled)
+        pyr, tiled = _volumes(be, f1, fmap[:, 0].contiguous(), vol_i, jloc_d)
         target = be.reproject(poses, video.disps, intr_all, ii_d, jj_d)[0]
         weight = torch.zeros_like(target)
         net, inp = video.nets[ii_d][None], video.inps[ii_d][None]
@@ -633,7 +649,7 @@ def _fill_batch(be, filler, tstamps, images, intrinsics):
         intr0 = video.intrinsics[0].contiguous()
         for _ in range(_FILL_UPDATES):
             coords, coords_t, motn = be.motion_features(poses, video.disps, intr_all, ii_d, jj_d, target)
-            corr = be.corr_lookup_pyramid(pyr, coords_t, tiled).view(1, E, -1, ht, wd)
+            corr = _lookup(be, pyr, tiled, coords_t)
             net, delta, w = filler.update.forward_segments(net, inp, corr, motn[None], None, 0)
             be.graph_writeback(delta[0], w[0], coords, None, target, weight, ba_target, ba_weight, 0, None, None, damping, None, None, 0.0)
             be.pose_only_ba(poses, video.disps, intr0, ba_target, ba_weight, ii_d, jj_d, B, B + M, 2, 1e-4, 0.1, False)
@@ -652,9 +668,11 @@ def fill_trajectory(filler, image_stream):
     was (the reference leaves the last batch in slots [N, N+16)), and a frame whose damped pose block is not positive definite keeps its
     pose in that iteration on its own (the reference zeroes the update of its whole 16-frame batch).  Raises when the filler cannot run
     natively (see install_trajectory_filler_hook)."""
-    why = _filler_unsupported(filler)
-    if why is not None:
-        raise RuntimeError("the native trajectory filler cannot run this filler: %s" % why)
+    _require("PoseTrajectoryFiller.__call__", _filler_unsupported(filler))
+    return _fill_trajectory(filler, image_stream)
+
+
+def _fill_trajectory(filler, image_stream):
     be = install()
     video = filler.video
     budget = _filler_frame_budget(be, video.fmaps.shape[3], video.fmaps.shape[4], video.poses.device)
@@ -673,18 +691,12 @@ def fill_trajectory(filler, image_stream):
 
 def install_trajectory_filler_hook(trajectory_filler_module, strict=True):
     """trajectory_filler_module = the imported reference module `trajectory_filler`.  Replaces `PoseTrajectoryFiller.__call__` by
-    fill_trajectory; the result is an SE3 of that module's own lietorch, as the reference returns.  strict: a filler the native path
-    cannot run (update operator not droid_slam_b200.update.UpdateModule, fnet not a BasicEncoder under install_encoder_hook, video tensors
-    not on CUDA) raises, naming the reason; with strict=False the reference's own method runs for it."""
-    cls = trajectory_filler_module.PoseTrajectoryFiller
-    ref_call = cls.__call__
-
-    def __call__(self, image_stream):
-        if not strict and _filler_unsupported(self) is not None:
-            return ref_call(self, image_stream)
-        return trajectory_filler_module.SE3(fill_trajectory(self, image_stream))
-
-    cls.__call__ = __call__
+    fill_trajectory; the result is an SE3 of that module's own lietorch, as the reference returns.  It runs fillers whose update operator
+    is droid_slam_b200.update.UpdateModule, whose fnet is a BasicEncoder under install_encoder_hook and whose video tensors are on CUDA,
+    with at least one keyframe; any other filler follows the strict policy (module docstring)."""
+    _replace(trajectory_filler_module.PoseTrajectoryFiller, "__call__",
+             lambda filler, image_stream: trajectory_filler_module.SE3(_fill_trajectory(filler, image_stream)),
+             lambda filler, *args, **kwargs: _filler_unsupported(filler), strict)
     return trajectory_filler_module
 
 
@@ -692,18 +704,10 @@ def install_trajectory_filler_hook(trajectory_filler_module, strict=True):
 
 def _motion_filter_unsupported(be, filt, image):
     """why track cannot run this MotionFilter on this frame natively (None: it can)"""
-    from .update import UpdateModule
-    if not isinstance(filt.update, UpdateModule):
-        return "filter.update is %s, not droid_slam_b200.update.UpdateModule" % type(filt.update).__name__
-    for name in ("fnet", "cnet"):
-        enc = getattr(filt, name)
-        if not getattr(type(enc).forward, "_b200_native", False):
-            return "filter.%s (%s) is not a BasicEncoder under install_encoder_hook" % (name, type(enc).__name__)
-    video = filt.video
-    for name in ("tstamp", "images", "poses", "disps", "disps_sens", "intrinsics", "fmaps", "nets", "inps"):
-        t = getattr(video, name, None)
-        if not (isinstance(t, torch.Tensor) and t.is_cuda):
-            return "video.%s is not a CUDA tensor" % name
+    why = _graph_unsupported("filter", filt, "update", ("fnet", "cnet"), video=("tstamp", "images", "poses", "disps", "disps_sens",
+                                                                              "intrinsics", "fmaps", "nets", "inps"))
+    if why is not None:
+        return why
     if not (isinstance(image, torch.Tensor) and image.dim() == 4 and image.shape[1] == 3 and image.dtype == torch.uint8):
         return "the image must be a uint8 tensor [cameras,3,H,W]"
     H, W = image.shape[-2:]
@@ -747,25 +751,26 @@ def track(filt, tstamp, image, depth=None, intrinsics=None):
     the video's 128 channels) and the identity pose and disparity 1.0; later keyframes write neither pose nor disparity; the depth
     (RGB-D) goes to the video as given, whose setter samples and inverts it; intrinsics are divided by 8.  Raises when the filter or the
     frame cannot run natively (see install_motion_filter_hook)."""
+    _require("MotionFilter.track", _motion_filter_unsupported(install(), filt, image))
+    _track(filt, tstamp, image, depth, intrinsics)
+
+
+def _track(filt, tstamp, image, depth=None, intrinsics=None):
     be = install()
-    why = _motion_filter_unsupported(be, filt, image)
-    if why is not None:
-        raise RuntimeError("the native motion filter cannot run this frame: %s" % why)
     video = filt.video
     dev = video.poses.device
     ht, wd = image.shape[-2] // 8, image.shape[-1] // 8
     norm = _frame_norm(filt)
     with torch.no_grad():
-        frames = _pinned_to(dev, image)
+        frames = _stage(dev, image)
         gmap = _encode_frames(be, filt.fnet, frames, norm)                     # [cameras,128,ht,wd]
         if video.counter.value == 0:
             keyframe, pose, disp = True, video.poses.new_zeros(7), 1.0
             pose[6] = 1                                                         # lietorch.SE3.Identity(1).data
         else:
             coords_t, idx = _probe_grid(filt, ht, wd, dev)
-            tiled = be.corr_volume_supported(128, ht, wd, True)
-            pyr = be.corr_volume_pyramid(filt.fmap[:1].contiguous(), gmap[:1].contiguous(), idx, idx, tiled)
-            corr = be.corr_lookup_pyramid(pyr, coords_t, tiled).view(1, 1, -1, ht, wd)
+            pyr, tiled = _volumes(be, filt.fmap[:1].contiguous(), gmap[:1].contiguous(), idx, idx)
+            corr = _lookup(be, pyr, tiled, coords_t)
             _, delta, _ = filt.update.forward_segments(filt.net[None], filt.inp[None], corr, None, None, 0)
             with torch.autocast("cuda", enabled=True):
                 stat = delta.norm(dim=-1).mean()
@@ -780,25 +785,19 @@ def track(filt, tstamp, image, depth=None, intrinsics=None):
             filt.count = 0
         filt.net, filt.inp, filt.fmap = net, inp, gmap
         if depth is not None:
-            depth = _pinned_to(dev, depth)
-        intr = _pinned_to(dev, intrinsics) / 8.0
+            depth = _stage(dev, depth)
+        intr = _stage(dev, intrinsics) / 8.0
         # the stamp as a device scalar: the video's `tstamp[i] = stamp` then copies on the device instead of synchronising the host
-        ts = _pinned_to(dev, torch.as_tensor(tstamp, dtype=video.tstamp.dtype))
+        ts = _stage(dev, torch.as_tensor(tstamp, dtype=video.tstamp.dtype))
         video.append(ts, frames[0], pose, disp, depth, intr, gmap, net[0, 0] if first else net[0], inp[0, 0] if first else inp[0])
 
 
 def install_motion_filter_hook(motion_filter_module, strict=True):
     """motion_filter_module = the imported reference module `motion_filter`.  Replaces `MotionFilter.track` (motion_filter.py:50-91) by
-    track above.  strict: a filter or frame the native path cannot run (update not droid_slam_b200.update.UpdateModule, fnet or cnet not a
-    BasicEncoder under install_encoder_hook, video tensors not on CUDA, a frame size without a kernel) raises, naming the reason; with
-    strict=False the reference's own method runs for it."""
-    cls = motion_filter_module.MotionFilter
-    ref_track = cls.track
-
-    def _track(self, tstamp, image, depth=None, intrinsics=None):
-        if not strict and _motion_filter_unsupported(install(), self, image) is not None:
-            return ref_track(self, tstamp, image, depth, intrinsics)
-        return track(self, tstamp, image, depth, intrinsics)
-
-    cls.track = _track
+    track above.  It runs filters whose update operator is droid_slam_b200.update.UpdateModule, whose fnet and cnet are BasicEncoders
+    under install_encoder_hook and whose video tensors are on CUDA, on uint8 frames [cameras,3,H,W] whose size the correlation kernels
+    take; any other filter or frame follows the strict policy (module docstring)."""
+    be = install()
+    _replace(motion_filter_module.MotionFilter, "track", _track,
+             lambda filt, tstamp, image, *args, **kwargs: _motion_filter_unsupported(be, filt, image), strict)
     return motion_filter_module

@@ -125,7 +125,8 @@ class UpdateModule(nn.Module):
         self._packed_key = None
 
     def packed_weights(self, device):
-        key = (str(device),) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        from .modules import _repack_key
+        key = (str(device),) + _repack_key(self.parameters())
         if self._packed is None or self._packed_key != key:
             pk = pack_update_weights(self.state_dict(), device)
             self._packed = [pk[k] for k in PACKED_ORDER]

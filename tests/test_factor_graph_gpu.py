@@ -138,7 +138,7 @@ class _FactorGraph:
         self.ran = "reference update_lowmem"
 
 
-def test_strict_mode():
+def test_strict_mode(monkeypatch):
     strict = type("StrictFG", (_FactorGraph,), {})
     lenient = type("LenientFG", (_FactorGraph,), {})
     modules.install_factor_graph_hook(strict, strict=True)
@@ -161,5 +161,8 @@ def test_strict_mode():
             assert g.ran == "reference update_lowmem"
     g = lenient()
     g.__dict__.update(_filler().__dict__)
+    checks, check = [], modules._factor_graph_unsupported
+    monkeypatch.setattr(modules, "_factor_graph_unsupported", lambda *a: checks.append(a) or check(*a))
     g.update(t0=1, t1=10, motion_only=True)                                 # native: the reference method does not run
     assert not hasattr(g, "ran")
+    assert len(checks) == 1                                                 # the readiness check ran once for the call

@@ -203,7 +203,7 @@ def _filter_class():
     return MotionFilter
 
 
-def test_motion_filter_hook_strict_and_fallback(be):
+def test_motion_filter_hook_strict_and_fallback(be, monkeypatch):
     H, W = 384, 512
     stream = _stream(2, H, W, 1, False, seed=9)
     t, image, depth, intr = stream[0]
@@ -229,6 +229,11 @@ def test_motion_filter_hook_strict_and_fallback(be):
         f.track(t, image[..., :56, :], depth, intr)
     mod2 = types.SimpleNamespace(MotionFilter=_filter_class())
     modules.install_motion_filter_hook(mod2, strict=False)
+    g = mod2.MotionFilter(_filter(mmf.Video(False, DEV, H, W, 4), 1.0))
+    checks, check = [], modules._motion_filter_unsupported
+    monkeypatch.setattr(modules, "_motion_filter_unsupported", lambda *a: checks.append(a) or check(*a))
+    assert g.track(t, image, depth, intr) is None and g.video.counter.value == 1
+    assert len(checks) == 1                                  # native: the readiness check ran once for the call
     g = mod2.MotionFilter(_filter(mmf.Video(False, "cpu", H, W, 4), 1.0))
     assert g.track(t, image, depth, intr) == "reference"
 

@@ -375,7 +375,7 @@ def _filler_class():
     return PoseTrajectoryFiller
 
 
-def test_filler_hook_strict_and_fallback(be):
+def test_filler_hook_strict_and_fallback(be, monkeypatch):
     PoseTrajectoryFiller = _filler_class()
     video = FVideo(64, 8, seed=14)
     mod = types.SimpleNamespace(PoseTrajectoryFiller=PoseTrajectoryFiller, SE3=lietorch.SE3)
@@ -393,5 +393,9 @@ def test_filler_hook_strict_and_fallback(be):
     mod2 = types.SimpleNamespace(PoseTrajectoryFiller=_filler_class(), SE3=lietorch.SE3)
     modules.install_trajectory_filler_hook(mod2, strict=False)
     g = mod2.PoseTrajectoryFiller(_filler(video))
+    checks, check = [], modules._filler_unsupported
+    monkeypatch.setattr(modules, "_filler_unsupported", lambda *a: checks.append(a) or check(*a))
+    assert isinstance(g(_stream(video, 5, seed=5)), lietorch.SE3)
+    assert len(checks) == 1                               # native: the readiness check ran once for the call
     g.video = types.SimpleNamespace(**{k: (t.cpu() if isinstance(t, torch.Tensor) else t) for k, t in vars(video).items()})
     assert g([]) == "reference"
