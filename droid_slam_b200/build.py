@@ -20,7 +20,7 @@ INCLUDE = os.path.join(os.path.dirname(PKG), "include")
 
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.environ.get("NVCC", os.path.join(CUDA_HOME, "bin", "nvcc"))
-CUDA_SOURCES = ["common.cu", "corr_index.cu", "corr_lookup_rows.cu", "altcorr.cu", "geom.cu", "ba.cu", "chol.cu", "corr_volume.cu", "update_op.cu", "encoder.cu", "proximity.cu", "filler.cu"]
+CUDA_SOURCES = ["common.cu", "corr_index.cu", "corr_lookup_rows.cu", "altcorr.cu", "geom.cu", "ba.cu", "chol.cu", "corr_volume.cu", "update_op.cu", "encoder.cu", "proximity.cu", "filler.cu", "handover.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-diag-suppress", "177"]
 

@@ -15,7 +15,7 @@ SYMBOLS = [
     "dba_solve_workspace_bytes", "dba_solve_spd", "dba_solve_tile_placement",
     "dba_update_workspace_bytes", "dba_update_workspace_layout", "dba_update_forward", "dba_conv_nhwc", "dba_conv_nhwc_plan", "dba_encoder_workspace_bytes", "dba_encoder_forward",
     "dba_encoder_forward_frames", "dba_encoder_workspace_layout", "dba_encoder_forward_prefix", "dba_proximity_workspace_bytes", "dba_proximity_edges",
-    "dba_fill_interpolate", "dba_pose_only_ba",
+    "dba_fill_interpolate", "dba_pose_only_ba", "dba_fragment_handover",
 ]
 
 DBA_F32, DBA_F16, DBA_F64, DBA_BF16 = 0, 1, 2, 3

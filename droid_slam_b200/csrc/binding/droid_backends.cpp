@@ -759,6 +759,57 @@ torch::Tensor proximity_edges(torch::Tensor d, int64_t t0, int64_t t1, int64_t t
   return es.narrow(0, 0, rows);
 }
 
+// DroidAsync's hand-over of the frontend's keyframes [t0,t1) to the backend (reference droid_slam/droid_async.py:54-119).  front / back:
+// the two DepthVideo's buffers in the order poses, disps, disps_sens, images, tstamp, intrinsics, fmaps, nets, inps; front on one
+// device, back on another or the same one.  On the back device's current stream: the slices [t0,t1) of every buffer go to the back
+// buffers (a peer copy across devices, a device copy otherwise; torch's cross-device copy orders both devices' current streams), the
+// front's poses[t0-10:t0-1] to a staging tensor, then dba_fragment_handover aligns and re-anchors in place.  The front's disps_sens is
+// read where it is on one device and copied whole across devices (the reference's torch.any spans the whole buffer).  No host
+// synchronisation.  Returns [diagnostics [9] f64: s, dG, align_scale] with diagnostics, else [].
+std::vector<torch::Tensor> fragment_handover(std::vector<torch::Tensor> front, std::vector<torch::Tensor> back, int64_t t0, int64_t t1, bool stereo,
+                                             bool diagnostics) {
+  static const char* names[9] = {"poses", "disps", "disps_sens", "images", "tstamp", "intrinsics", "fmaps", "nets", "inps"};
+  TORCH_CHECK(front.size() == 9 && back.size() == 9, "droid_backends.fragment_handover: front and back must each hold the 9 buffers ",
+              "(poses, disps, disps_sens, images, tstamp, intrinsics, fmaps, nets, inps), got ", front.size(), " and ", back.size());
+  const Expect fx("fragment_handover", front[0], "front poses");
+  const Expect bx("fragment_handover", back[0], "back poses");
+  fx(front[0], "front poses", F32, dims({kAny, 7}));
+  const int64_t N = front[0].size(0);
+  fx(front[1], "front disps", F32, dims({N, kAny, kAny}), kAnyLayout);
+  const int64_t ht = front[1].size(1), wd = front[1].size(2);
+  fx(front[2], "front disps_sens", F32, dims({N, ht, wd}));
+  for (int k = 3; k < 9; k++) {
+    const std::string name = std::string("front ") + names[k];
+    fx(front[k], name.c_str(), {}, {}, kAnyLayout);
+    TORCH_CHECK(front[k].dim() >= 1 && front[k].size(0) == N, "droid_backends.fragment_handover: ", name, " must have ", N,
+                " frames (as poses), got shape ", front[k].sizes());
+  }
+  bx(back[0], "back poses", F32, dims({N, 7}));
+  bx(back[1], "back disps", F32, dims({N, ht, wd}));
+  for (int k = 2; k < 9; k++) {
+    const std::string name = std::string("back ") + names[k];
+    bx(back[k], name.c_str(), front[k].scalar_type(), dims(front[k].sizes()), kAnyLayout);
+  }
+  TORCH_CHECK(t0 == 0 || t0 >= 10, "droid_backends.fragment_handover: t0 must be 0 or at least 10 (the frames [t0-10, t0-1) are aligned), got ", t0);
+  TORCH_CHECK(t0 <= N && t1 >= 0 && t1 <= N, "droid_backends.fragment_handover: t0 = ", t0, ", t1 = ", t1, " outside the ", N, "-frame buffers");
+  c10::cuda::CUDAGuard guard(bx.dev);
+  const int64_t n = std::max<int64_t>(t1 - t0, 0);
+  if (n > 0)
+    for (int k = 0; k < 9; k++) back[k].narrow(0, t0, n).copy_(front[k].narrow(0, t0, n), true);
+  torch::Tensor align, sens = front[2];
+  const auto on_back = torch::TensorOptions().device(bx.dev);
+  if (t0 > 0) align = front[0].narrow(0, t0 - 10, 9).to(on_back, true, true);     // a snapshot: the front may move on
+  if (fx.dev != bx.dev) sens = sens.to(on_back, true);
+  torch::Tensor ws, diag;
+  void* ws_p = workspace(DBA_HANDOVER_WORKSPACE_BYTES, bx.dev, ws);
+  if (diagnostics) diag = torch::empty({9}, back[0].options().dtype(torch::kFloat64));
+  check_status(dba_fragment_handover(t0 > 0 ? align.data_ptr<float>() : nullptr, back[0].data_ptr<float>(), back[1].data_ptr<float>(),
+                                     sens.data_ptr<float>(), sens.numel(), (int)t0, (int)t1, (int)(ht * wd), stereo ? 1 : 0, ws_p,
+                                     diagnostics ? diag.data_ptr<double>() : nullptr, cur_stream()), "fragment_handover");
+  if (!diagnostics) return {};
+  return {diag};
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
   // bundle adjustment kernels
@@ -810,6 +861,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("poses"), pybind11::arg("disps"), pybind11::arg("intrinsics"), pybind11::arg("targets"), pybind11::arg("weights"),
         pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("t0"), pybind11::arg("t1"), pybind11::arg("iterations") = 2,
         pybind11::arg("lm") = 1e-4f, pybind11::arg("ep") = 0.1f, pybind11::arg("check") = true,
+        pybind11::arg("diagnostics") = false);
+  m.def("fragment_handover", &fragment_handover,
+        "DroidAsync's frontend -> backend hand-over of frames [t0,t1): slice copies, fragment alignment and re-anchoring on the back device "
+        "-> [diagnostics (s, dG, align_scale)] or [], native extension",
+        pybind11::arg("front"), pybind11::arg("back"), pybind11::arg("t0"), pybind11::arg("t1"), pybind11::arg("stereo"),
         pybind11::arg("diagnostics") = false);
   m.def("_b200_native", []() { return true; });
 }

@@ -29,11 +29,20 @@ kernel for is offered as a hook:
     fed straight into the encoders (`droid_backends.encoder_forward_frames`), the motion probe on the correlation kernels and one host
     read per frame (row F6).
 
+  * `install_update_module_hook(droid_net)`: DroidNet (and both reference `load_network` functions) build the native update operator.
+  * `install_async_hook(droid_async)`: DroidAsync's backend process (droid_async.py:37-130), started with `spawn`, re-installs every hook
+    of the parent (`hook_registry`) and runs the reference's loop with the frontend -> backend hand-over on the device
+    (`handover_round` -> `droid_backends.fragment_handover`, one host sync per round).
+
 The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
 it.  If not, strict=True (the default) raises RuntimeError naming the replaced method and the reason; strict=False runs the reference's
 own method.  `update`, `update_lowmem`, `fill_trajectory` and `track` called directly raise in the same words.
 """
+import copy
+import importlib
 import sys
+import time
+import types
 
 import torch
 
@@ -41,7 +50,8 @@ from . import install
 
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
-           "install_trajectory_filler_hook", "track", "install_motion_filter_hook"]
+           "install_trajectory_filler_hook", "track", "install_motion_filter_hook", "hook_registry", "reinstall_hooks",
+           "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook"]
 
 
 def _require(entry, why):
@@ -170,6 +180,7 @@ def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
              strict)
     if fused_lookup:
         cls.__call__ = __call__
+    _record("install_corr_volume_hook", corr_module, strict=strict, fused_lookup=fused_lookup)
     return corr_module
 
 
@@ -229,6 +240,7 @@ def install_alt_corr_hook(corr_module, strict=True):
     cls._b200_pyramid = None                    # a block's private pyramid; None where the reference's constructor ran
     _replace(cls, "__init__", __init__, unsupported, strict)
     cls.__call__ = __call__
+    _record("install_alt_corr_hook", corr_module, strict=strict)
     return corr_module
 
 
@@ -275,6 +287,7 @@ def install_encoder_hook(extractor_module, strict=True):
 
     _replace(extractor_module.BasicEncoder, "forward", forward, lambda enc, x: _encoder_unsupported(enc, x), strict)
     extractor_module.BasicEncoder.forward._b200_encoder_hook = True          # what the filler and motion-filter checks look for
+    _record("install_encoder_hook", extractor_module, strict=strict)
     return extractor_module
 
 
@@ -351,6 +364,7 @@ def add_proximity_factors(graph, t0=0, t1=0, rad=2, nms=2, beta=0.25, thresh=16.
 def install_proximity_hook(factor_graph_class):
     """replace `add_proximity_factors` of the reference's FactorGraph class (factor_graph.py:346) by the device version"""
     factor_graph_class.add_proximity_factors = add_proximity_factors
+    _record("install_proximity_hook", factor_graph_class)
     return factor_graph_class
 
 
@@ -365,6 +379,7 @@ def install_depth_video_hook(depth_video_class):
 
     depth_video_class.reproject = _reproject
     depth_video_class.upsample = _upsample
+    _record("install_depth_video_hook", depth_video_class)
     return depth_video_class
 
 
@@ -576,6 +591,7 @@ def install_factor_graph_hook(factor_graph_class, strict=True):
     unsupported = lambda graph, *args, **kwargs: _factor_graph_unsupported(graph)          # noqa: E731
     _replace(factor_graph_class, "update", _update, unsupported, strict)
     _replace(factor_graph_class, "update_lowmem", _update_lowmem, unsupported, strict)
+    _record("install_factor_graph_hook", factor_graph_class, strict=strict)
     return factor_graph_class
 
 
@@ -697,6 +713,7 @@ def install_trajectory_filler_hook(trajectory_filler_module, strict=True):
     _replace(trajectory_filler_module.PoseTrajectoryFiller, "__call__",
              lambda filler, image_stream: trajectory_filler_module.SE3(_fill_trajectory(filler, image_stream)),
              lambda filler, *args, **kwargs: _filler_unsupported(filler), strict)
+    _record("install_trajectory_filler_hook", trajectory_filler_module, strict=strict)
     return trajectory_filler_module
 
 
@@ -800,4 +817,182 @@ def install_motion_filter_hook(motion_filter_module, strict=True):
     be = install()
     _replace(motion_filter_module.MotionFilter, "track", _track,
              lambda filt, tstamp, image, *args, **kwargs: _motion_filter_unsupported(be, filt, image), strict)
+    _record("install_motion_filter_hook", motion_filter_module, strict=strict)
     return motion_filter_module
+
+
+# ---- the hook registry and DroidAsync's backend process -----------------------------------------------------------------------------
+
+_HOOKS = []        # every hook installed in this process, in order (see hook_registry)
+
+
+def _resolve(module, qualname):
+    """the module `module` (qualname None) or the object at `qualname` in it, importing the module"""
+    obj = importlib.import_module(module)
+    for part in (qualname.split(".") if qualname else ()):
+        obj = getattr(obj, part)
+    return obj
+
+
+def _record(installer, target, **kwargs):
+    """enter the hook `installer(target, **kwargs)` in the registry.  target is transferable when it is a module or a class that another
+    interpreter finds by name: the module sys.modules holds under its name, or the class at its qualified name in such a module"""
+    module, qualname = getattr(target, "__module__", None), getattr(target, "__qualname__", None)
+    if isinstance(target, types.ModuleType):
+        module, qualname = target.__name__, None
+    transferable = isinstance(target, (types.ModuleType, type)) and module in sys.modules and "<locals>" not in (qualname or "")
+    if transferable:
+        try:
+            transferable = _resolve(module, qualname) is target
+        except AttributeError:
+            transferable = False
+    entry = {"installer": installer, "module": module, "qualname": qualname, "kwargs": kwargs, "transferable": transferable,
+             "target": "%s.%s" % (module, qualname) if qualname else (module if transferable else repr(target))}
+    if transferable:                     # installing again on the same target replaces the entry
+        _HOOKS[:] = [e for e in _HOOKS if not (e["transferable"] and (e["installer"], e["module"], e["qualname"]) == (installer, module, qualname))]
+    _HOOKS.append(entry)
+
+
+def hook_registry():
+    """a copy of the registry: per installed hook, in installation order, a dict of installer (the install_* function's name), module
+    (the importable name of the reference module patched, or of the module defining the patched class), qualname (the class's qualified
+    name; None when the module itself was passed), kwargs (strict, fused_lookup), transferable (False for a target another interpreter
+    cannot find by name, e.g. a SimpleNamespace) and target (a readable name).  Plain data: it pickles."""
+    return copy.deepcopy(_HOOKS)
+
+
+def reinstall_hooks(hooks):
+    """install every transferable hook of `hooks` (as hook_registry gives them) in this interpreter, by module name, in order"""
+    install()
+    for e in hooks:
+        if e["transferable"]:
+            globals()[e["installer"]](_resolve(e["module"], e["qualname"]), **e["kwargs"])
+
+
+def install_update_module_hook(droid_net_module):
+    """droid_net_module = the imported reference module `droid_net`.  Sets its global `UpdateModule` (droid_net.py:111-143) to
+    droid_slam_b200.update.UpdateModule, so `DroidNet()` -- and both reference `load_network` functions, which build it -- construct the
+    native update operator.  Same parameter names: a DROID checkpoint loads unchanged (the callers already slice the heads to 2 rows)."""
+    from .update import UpdateModule
+    droid_net_module.UpdateModule = UpdateModule
+    _record("install_update_module_hook", droid_net_module)
+    return droid_net_module
+
+
+# the hooks the native backend loop runs on: DroidAsyncBackend -> FactorGraph.add_proximity_factors / update_lowmem(use_inactive=True)
+# on AltCorrBlock and DepthVideo.reproject / upsample, with the network's update operator
+_BACKEND_HOOKS = ("install_update_module_hook", "install_factor_graph_hook", "install_alt_corr_hook", "install_proximity_hook",
+                  "install_depth_video_hook")
+_HANDOVER_BUFFERS = ("poses", "disps", "disps_sens", "images", "tstamp", "intrinsics", "fmaps", "nets", "inps")
+
+
+def _async_unsupported(hooks):
+    """why a spawned backend process cannot run natively with these hooks (None: it can)"""
+    lost = [e["installer"] + " on " + e["target"] for e in hooks if not e["transferable"]]
+    if lost:
+        return "hooks on objects a spawned process cannot import by name: " + ", ".join(lost)
+    missing = [h for h in _BACKEND_HOOKS if not any(e["installer"] == h for e in hooks)]
+    if missing:
+        return "the native backend needs " + ", ".join(missing)
+    return None
+
+
+def handover_round(video1, video2, t0, t1, diagnostics=False):
+    """the hand-over of one backend round (reference droid_async.py:54-119) on droid_backends.fragment_handover: under video1's lock,
+    the slices [t0,t1) of video1's buffers go to video2, the fragment alignment and the re-anchoring of poses / disps run on video2's
+    device, and the lock is released after one synchronisation of video2's device's current stream -- the round's one host sync.
+    t0 == 0 or t0 >= 10 (what backend_process produces).  Returns the diagnostics [9] f64 (s, dG, align_scale) when asked, else None."""
+    be = install()
+    with video1.get_lock():
+        out = be.fragment_handover([getattr(video1, k) for k in _HANDOVER_BUFFERS], [getattr(video2, k) for k in _HANDOVER_BUFFERS],
+                                   int(t0), int(t1), bool(video2.stereo), diagnostics)
+        torch.cuda.current_stream(video2.poses.device).synchronize()
+    return out[0] if diagnostics else None
+
+
+_BACKEND_ITERS_SHARED, _BACKEND_ITERS_OWN_DEVICE = 8, 12   # global-BA iterations per round: backend on the frontend's GPU / on its own
+_BACKEND_START_FRAMES = 32          # the frontend's keyframe count above which rounds start before the end of the stream
+_BACKEND_FRONTIER_GAP = 5           # keyframes left to the frontend's local window in a round before the last
+_BACKEND_OVERLAP = 2                # keyframes of the previous round handed over again (t0 = counter2 - 2)
+_BACKEND_PAUSE_S = 10               # seconds between rounds while the stream lasts
+
+
+def _backend_loop(mod, args, front, back, device="cuda"):
+    """The decisions of the reference's backend_process (droid_async.py:37-130), with the hand-over on handover_round.
+
+    device "cuda" shares the frontend's GPU (8 iterations per round); any other device string is selected for this process and gets 12
+    (:40-50).  Rounds run while the frontend holds more than 32 keyframes or the stream has ended (back.ready, :55); a round hands over
+    keyframes [max(back.counter - 2, 0), t1) with t1 = the frontend's counter in the final round and 5 fewer before it (:57-71), sets
+    back.counter = t1 and calls the backend with normalize=False (:121-122).  The final round ends the loop; otherwise, unless the stream
+    ended meanwhile, the loop waits 10 s (:124-128).  load_network and DroidAsyncBackend are looked up in `mod`, as the reference's
+    module globals are."""
+    torch.set_num_threads(8)
+    own_device = device != "cuda"
+    if own_device:
+        torch.cuda.set_device(device)
+    iters = _BACKEND_ITERS_OWN_DEVICE if own_device else _BACKEND_ITERS_SHARED
+    with torch.no_grad():
+        ba = mod.DroidAsyncBackend(mod.load_network(args.weights, device=device), back, args)
+        while True:
+            if not (front.counter.value > _BACKEND_START_FRAMES or back.ready.value):
+                continue                                           # the reference polls without pausing here too
+            final = bool(back.ready.value)                         # read again, as the reference does
+            first = max(back.counter.value - _BACKEND_OVERLAP, 0)
+            end = front.counter.value - (0 if final else _BACKEND_FRONTIER_GAP)
+            handover_round(front, back, first, end)
+            back.counter.value = end
+            ba(iters, normalize=False)
+            if final:
+                return
+            if back.ready.value <= 0:
+                time.sleep(_BACKEND_PAUSE_S)
+
+
+class BackendProcess:
+    """The `backend_process` install_async_hook puts into the reference's droid_async module; DroidAsync starts it as a Process target.
+
+    Pickled (which is how `spawn` hands it to the new interpreter) it carries the hook registry of that moment, checked first: a hook on
+    an object that cannot be imported by name, or a missing hook of the native backend (_BACKEND_HOOKS), raises under strict=True --
+    in the parent, as DroidAsync starts the process -- and makes the child run the reference's own backend_process under strict=False.
+    In the child, __call__ runs droid_slam_b200.install(), re-installs every recorded hook by module name, then the native loop.  Called
+    without pickling (in the installing process, or a forked child, where the hooks are in place) it checks the same and runs the loop."""
+
+    def __init__(self, module, strict=True, reference=None, hooks=None, native=None):
+        self.module, self.strict, self.reference, self.hooks, self.native = module, strict, reference, hooks, native
+
+    def __reduce__(self):
+        if self.native is not None:                          # already a snapshot
+            return BackendProcess, (self.module, self.strict, None, self.hooks, self.native)
+        why = _async_unsupported(_HOOKS)
+        if why is not None and self.strict:
+            _require("droid_async.backend_process", why)
+        return BackendProcess, (self.module, self.strict, None, hook_registry(), why is None)
+
+    def prepare(self):
+        """install the native extension and the carried hooks in this interpreter -> the droid_async module"""
+        reinstall_hooks(self.hooks)
+        return importlib.import_module(self.module)
+
+    def __call__(self, args, depth_video1, depth_video2, device="cuda"):
+        if self.native is None:                              # not pickled: the hooks of this process apply
+            why = _async_unsupported(_HOOKS)
+            if why is not None and not self.strict:
+                return self.reference(args, depth_video1, depth_video2, device)
+            _require("droid_async.backend_process", why)
+            return _backend_loop(importlib.import_module(self.module), args, depth_video1, depth_video2, device)
+        if not self.native:                                  # a fresh interpreter: its droid_async holds the reference's function
+            return importlib.import_module(self.module).backend_process(args, depth_video1, depth_video2, device)
+        return _backend_loop(self.prepare(), args, depth_video1, depth_video2, device)
+
+
+def install_async_hook(droid_async_module, strict=True):
+    """droid_async_module = the imported reference module `droid_async`.  Replaces its global `backend_process` (droid_async.py:37-130,
+    the target of DroidAsync's backend Process) by a BackendProcess: in the spawned process it re-installs every hook recorded in this
+    process (hook_registry) and runs the reference's loop with the hand-over on handover_round.  Under strict=True, starting DroidAsync
+    raises when a recorded hook cannot be re-installed by name or a hook the native backend needs is missing (_BACKEND_HOOKS);
+    strict=False then keeps the reference's backend_process."""
+    ref = droid_async_module.backend_process
+    if isinstance(ref, BackendProcess):
+        ref = ref.reference
+    droid_async_module.backend_process = BackendProcess(droid_async_module.__name__, strict, ref)
+    return droid_async_module

@@ -257,6 +257,28 @@ int dba_pose_only_ba(float* poses, const float* disps, const float* intrinsics, 
                      const int64_t* ii, const int64_t* jj, int n_frames, int n_disps, int n_edges, int ht, int wd, int t0, int t1,
                      int iterations, float lm, float ep, int* status, double* sys_out, float* dx_out, dba_stream_t stream);
 
+/* ---- DroidAsync fragment hand-over (reference droid_slam/droid_async.py:54-119, droid_slam/align.py) -----------------------
+ * One backend round's hand-over of the frontend's keyframes [t0,t1) to the backend's video, on the backend's device, in two launches and
+ * without a host synchronisation.  The caller first copies the frontend's poses[t0:t1] and disps[t0:t1] into poses2 / disps2 rows [t0,t1)
+ * and, when t0 > 0, the frontend's poses[t0-10:t0-1] into poses1_align [9,7].  Then:
+ *   launch 1 (one CTA per slice of disps_sens1; the first one also aligns): any = any(disps_sens1 != 0) per slice, and when t0 > 0
+ *     (dG, s) = align_pose_fragements(poses1_align, poses2[t0-10:t0-1]) in fp64 from the fp32 poses: the 81 relative translations,
+ *     s = sum(dt1 . dt2) / sum(dt1 . dt1), dG from the s-scaled frontend poses with 3 log-mean-exp refinements; t0 == 0: dG = identity,
+ *     s = 1.
+ *   launch 2 (one CTA per frame and 1024-pixel chunk): align_scale = !stereo && !any; s_eff = align_scale ? s : 1 -- dG stays the one
+ *     computed from the s-scaled poses even when s is discarded, as the reference does; with s_f = (float)s_eff,
+ *     poses2[f] = dG * (poses2[f] with its translation * s_f in fp32), composed in fp64 and rounded once, and disps2[f] /= s_f (fp32
+ *     division), for t0 <= f < t1.
+ * poses2 [>= t1, 7] f32, disps2 [>= t1, hw] f32, disps_sens1: the frontend's whole disps_sens buffer (n_sens floats) readable from this
+ * device (the reference's torch.any spans the whole buffer).  Contract: t0 == 0 or t0 >= 10 -- what the reference's backend_process
+ * produces (t0 = counter2 - 2, counter2 being 0 in the first round and at least 28 after it); other t0 are rejected (the reference's
+ * Python slices would wrap at negative starts; that is not reproduced).  t1 <= t0 re-anchors nothing (an empty slice in the reference).
+ * workspace: DBA_HANDOVER_WORKSPACE_BYTES bytes of device memory, 8-byte aligned, no initialisation needed.  diagnostics (may be NULL):
+ * double [9] = s_eff, dG (tx,ty,tz,qx,qy,qz,qw), align_scale (0 / 1). */
+#define DBA_HANDOVER_WORKSPACE_BYTES 4096
+int dba_fragment_handover(const float* poses1_align, float* poses2, float* disps2, const float* disps_sens1, long long n_sens, int t0, int t1,
+                          int hw, int stereo, void* workspace, double* diagnostics, dba_stream_t stream);
+
 /* ---- update operator (ConvGRU + heads + GraphAgg) on the tensor cores -----------------------------------
  * replaces UpdateModule.forward (reference droid_slam/droid_net.py:111-143), ConvGRU.forward (droid_slam/modules/gru.py:19-32) and
  * GraphAgg.forward (droid_net.py:59-75) -- in the reference a chain of 19 cuDNN convolutions + ~25 elementwise launches.
