@@ -13,6 +13,7 @@ import torch
 import droid_slam_b200
 from droid_slam_b200 import modules, synth
 from droid_slam_b200.update import UpdateModule
+from util import syncs_not_counted
 
 
 def _corr_classes():
@@ -81,13 +82,9 @@ class Video:
             self.poses.copy_(poses)
             self.disps.copy_(disps)
             return
-        mode = torch.cuda.get_sync_debug_mode()
-        torch.cuda.set_sync_debug_mode(0)             # ba's own status reads are not the update's
-        try:
+        with syncs_not_counted():                      # ba's own status reads are not the update's
             droid_slam_b200.install().ba(self.poses, self.disps, self.intrinsics[0], self.disps_sens, target, weight, eta, ii, jj, t0, t1,
                                          itrs, lm, ep, motion_only)
-        finally:
-            torch.cuda.set_sync_debug_mode(mode)
         self.disps.clamp_(min=0.001)
         if self.ba_log is not None:
             self.ba_log.append((tuple(a.clone() if isinstance(a, torch.Tensor) else a for a in args), self.poses.clone(), self.disps.clone()))

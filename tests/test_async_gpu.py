@@ -5,7 +5,6 @@ import contextlib
 import os
 import sys
 import types
-import warnings
 
 import pytest
 import torch
@@ -17,6 +16,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import async_backend as oab  # noqa: E402
 from droid_slam_b200 import modules  # noqa: E402
 import async_stubs  # noqa: E402
+from util import host_syncs  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 TWO_GPUS = torch.cuda.is_available() and torch.cuda.device_count() > 1
@@ -107,15 +107,8 @@ def test_empty_round_and_rejected_t0(backends):
 def test_one_host_sync_per_round():
     v1, v2 = async_stubs.make_videos(512, 48, 64, "rgbd", 300, 364, seed=5)
     modules.handover_round(v1, v2, 300, 364)
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            modules.handover_round(v1, v2, 300, 364)
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    assert sum(str(w.message).startswith("called a synchronizing") for w in caught) == 1, [str(w.message) for w in caught]
+    n, _ = host_syncs(lambda: modules.handover_round(v1, v2, 300, 364))
+    assert n == 1, n
 
 
 @pytest.mark.parametrize("devices", [("cuda", "cuda"), ("cuda:0", "cuda:1")])

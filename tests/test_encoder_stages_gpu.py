@@ -35,10 +35,8 @@ and fraction; the worst share of the slot, merge and whole-image statistics tole
   128x256_n2             cnet  0.234  0.9970
 Over all cases by K: 147: 0.157, 288: 0.234, 576: 0.199, 1152: 0.172, conv2 (K = 128): 0.209 sqrt(K)."""
 import ctypes
-import functools
 import json
 import os
-import subprocess
 
 import pytest
 import torch
@@ -47,7 +45,7 @@ import oracle.encoder as oenc
 from droid_slam_b200 import c_api, synth
 from droid_slam_b200.encoder import pack_encoder_weights
 from test_encoder_stages_cpu import CASES, CASE_IDS, ENCODERS, bits, case_images, case_weights, check_stage, layout, stage_table
-from util import stream
+from util import card, stream
 
 pytestmark = pytest.mark.gpu
 dev = "cuda"
@@ -114,18 +112,14 @@ class Run:
         assert bool((self.buf[self.lay["total"]:] == 255).all()), "%s wrote past its workspace" % what
 
 
-@functools.lru_cache(None)
-def _card():
-    """the card's name and power limit, read (not set) in the run that measures"""
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30)
-        return q.stdout.strip() or torch.cuda.get_device_name(0)
-    except (OSError, subprocess.SubprocessError):
-        return torch.cuda.get_device_name(0)
+@pytest.fixture(scope="module")
+def gpu():
+    """the card the reports name, read once"""
+    return card()
 
 
-def _report(case, name, per_kind):
-    line = dict(case=case, encoder=name, gpu=_card(), **per_kind)
+def _report(gpu, case, name, per_kind):
+    line = dict(case=case, encoder=name, gpu=gpu, **per_kind)
     print("ENC_STAGES " + json.dumps(line))
     path = os.environ.get("ENC_STAGES_REPORT")
     if path:
@@ -141,7 +135,7 @@ def _kind(row):
 
 @pytest.mark.parametrize("name", ["fnet", "cnet"])
 @pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
-def test_every_launch_matches_fp64(capi, case, name):
+def test_every_launch_matches_fp64(capi, gpu, case, name):
     images = case_images(case)
     sd = case_weights(case, ENCODERS[name][0])
     run = Run(capi, name, sd, images)
@@ -163,7 +157,7 @@ def test_every_launch_matches_fp64(capi, case, name):
     full = run.forward()
     assert torch.equal(bits(full), bits(run.view(run.out))), "dba_encoder_forward differs from its own launches run as a prefix"
     assert not bool(torch.isnan(full).any())
-    _report(case[0], name, {k: {a: float("%.3g" % b) for a, b in v.items()} for k, v in per_kind.items()})
+    _report(gpu, case[0], name, {k: {a: float("%.3g" % b) for a, b in v.items()} for k, v in per_kind.items()})
 
 
 def _oracle_nan(sd, images, norm):

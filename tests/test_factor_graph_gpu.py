@@ -5,7 +5,6 @@ first one's BA results after checking its BA inputs bit for bit (factor_graph_st
 bit, host synchronisations per call, strict mode."""
 import os
 import sys
-import warnings
 
 import pytest
 import torch
@@ -15,6 +14,7 @@ from droid_slam_b200 import modules
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import factor_graph_stubs as fs  # noqa: E402
+from util import host_syncs  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -105,18 +105,6 @@ def test_lowmem_bits_do_not_depend_on_chunk_composition(monkeypatch):
     assert fs.differing(small, large) == []
 
 
-def _count_syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum("synchroniz" in str(w.message) for w in caught)
-
-
 @pytest.mark.parametrize("make,method,kw", [(_frontend, "update", dict(use_inactive=True)),
                                             (_stereo, "update_lowmem", dict(steps=3, use_inactive=True))])
 def test_at_most_one_host_sync_per_call(make, method, kw, monkeypatch):
@@ -124,7 +112,7 @@ def test_at_most_one_host_sync_per_call(make, method, kw, monkeypatch):
     graph = make()
     with torch.no_grad():
         getattr(modules, method)(graph, **kw)                              # warm-up: packs the operator's weights once
-        n = _count_syncs(lambda: getattr(modules, method)(graph, **kw))
+        n, _ = host_syncs(lambda: getattr(modules, method)(graph, **kw))
     assert n <= 1, n
 
 

@@ -5,7 +5,6 @@ import math
 import os
 import sys
 import types
-import warnings
 
 import pytest
 import torch
@@ -22,6 +21,7 @@ from droid_slam_b200 import modules, synth  # noqa: E402
 from droid_slam_b200.encoder import pack_encoder_weights  # noqa: E402
 import factor_graph_stubs as fs  # noqa: E402
 import make_motion_filter_golden as mmf  # noqa: E402
+from util import host_syncs  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -178,17 +178,8 @@ def test_track_one_host_read_per_frame(be):
     filt = _filter(mmf.Video(False, DEV, H, W, len(stream)), _reference_run(stream, H, W, 1)[0])
     for t, image, depth, intr in stream[:3]:                 # warm-up: packs the weights, reads MEAN / STDV once
         modules.track(filt, t, image, depth, intr)
-    torch.cuda.synchronize()
     kf0 = filt.video.counter.value
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            for t, image, depth, intr in stream[3:]:
-                modules.track(filt, t, image, depth, intr)
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    n = sum("called a synchronizing CUDA operation" in str(w.message) for w in caught)
+    n, _ = host_syncs(lambda: [modules.track(filt, t, image, depth, intr) for t, image, depth, intr in stream[3:]])
     assert n <= len(stream) - 3, n
     assert filt.video.counter.value > kf0                    # keyframes were appended inside the counted window
 

@@ -4,7 +4,6 @@ native operators.  Stand-ins for DepthVideo, FactorGraph and PoseTrajectoryFille
 import os
 import sys
 import types
-import warnings
 
 import pytest
 import torch
@@ -21,6 +20,7 @@ import oracle.encoder as oenc  # noqa: E402
 from oracle import trajectory_filler as otf  # noqa: E402
 from droid_slam_b200 import modules, synth  # noqa: E402
 import factor_graph_stubs as fs  # noqa: E402
+from util import host_syncs, syncs_not_counted  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -230,13 +230,9 @@ class FVideo:
         return modules.reproject(self.poses, self.disps, self.intrinsics, ii, jj)
 
     def ba(self, target, weight, eta, ii, jj, t0=1, t1=None, itrs=2, lm=1e-4, ep=0.1, motion_only=False):
-        mode = torch.cuda.get_sync_debug_mode()
-        torch.cuda.set_sync_debug_mode(0)
-        try:
+        with syncs_not_counted():
             droid_slam_b200.install().ba(self.poses, self.disps, self.intrinsics[0], self.disps_sens, target, weight, eta, ii, jj, t0, t1,
                                          itrs, lm, ep, motion_only)
-        finally:
-            torch.cuda.set_sync_debug_mode(mode)
 
 
 class FGraph:
@@ -352,17 +348,8 @@ def test_fill_trajectory_host_syncs_per_batch(be, monkeypatch):
     stream = _stream(video, 20, seed=4)
     with torch.no_grad():
         modules.fill_trajectory(filler, stream)          # warm-up: packs the weights once
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            with torch.no_grad():
-                modules.fill_trajectory(filler, stream)
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    n = sum("synchroniz" in str(w.message) for w in caught)
-    assert n <= 3, n                                      # three batches of at most 8 frames
+        n, _ = host_syncs(lambda: modules.fill_trajectory(filler, stream))
+    assert n <= 3, n                                     # three batches of at most 8 frames
 
 
 def _filler_class():

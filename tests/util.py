@@ -1,5 +1,10 @@
-"""helpers shared by the parity tests: calling the C ABI with torch CUDA tensors, comparison metrics"""
+"""helpers shared by the parity tests and the bench tools: calling the C ABI with torch CUDA tensors, comparison metrics, counting host
+synchronisations, reading the card and timing calls"""
+import contextlib
 import ctypes
+import subprocess
+import time
+import warnings
 
 import torch
 
@@ -144,3 +149,69 @@ def assert_bit_identical(a, b, what=""):
         if bool(neq.any()):
             d = (a.double() - b.double()).abs()
             raise AssertionError("%s: %d of %d elements differ, max |diff| %.3e" % (what, int(neq.sum()), a.numel(), float(d[neq].max())))
+
+
+SYNC_WARNING = "called a synchronizing CUDA operation"      # torch's warning per synchronising operation in sync debug mode "warn"
+
+
+def host_syncs(fn):
+    """(host synchronisations fn() makes, its result).  Counts torch's per-operation warnings only, not its one-time notice that the
+    debug mode is a prototype, so a count does not depend on whether an earlier window in the process already raised that notice."""
+    torch.cuda.synchronize()
+    mode = torch.cuda.get_sync_debug_mode()
+    with warnings.catch_warnings(record=True) as caught:
+        warnings.simplefilter("always")
+        torch.cuda.set_sync_debug_mode("warn")
+        try:
+            out = fn()
+        finally:
+            torch.cuda.set_sync_debug_mode(mode)
+    return sum(str(w.message).startswith(SYNC_WARNING) for w in caught), out
+
+
+@contextlib.contextmanager
+def syncs_not_counted():
+    """synchronisations inside the block are not counted by an enclosing host_syncs"""
+    mode = torch.cuda.get_sync_debug_mode()
+    torch.cuda.set_sync_debug_mode(0)
+    try:
+        yield
+    finally:
+        torch.cuda.set_sync_debug_mode(mode)
+
+
+def card():
+    """name, power limit and SM clocks of torch's current device, read (never set) with nvidia-smi.  The device is named to nvidia-smi
+    by its PCI bus id: nvidia-smi's indices ignore CUDA_VISIBLE_DEVICES.  Never raises; when nvidia-smi cannot answer, the name comes
+    from torch and the other fields say why they are unknown."""
+    d = torch.cuda.current_device()
+    p = torch.cuda.get_device_properties(d)
+    bus = "%08X:%02X:%02X.0" % (p.pci_domain_id, p.pci_bus_id, p.pci_device_id)
+    keys = ("name", "power_limit", "sm_clock", "max_sm_clock")
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", bus, "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30)
+        vals = [v.strip() for v in r.stdout.strip().split(",")]
+        if r.returncode == 0 and len(vals) == len(keys):
+            return dict(zip(keys, vals))
+        why = "nvidia-smi -i %s exited %d: %s" % (bus, r.returncode, (r.stderr or r.stdout).strip()[:200])
+    except (OSError, subprocess.SubprocessError) as e:
+        why = "%s: %s" % (type(e).__name__, e)
+    return dict(name=torch.cuda.get_device_name(d), **{k: "unknown (%s)" % why for k in keys[1:]})
+
+
+def timed(fn, calls=1, warmup=0):
+    """(CUDA-event ms per call, host-clock ms per call, the last call's result) over `calls` calls of fn after `warmup` calls.  The
+    device is synchronised before both clocks start and after the last call, so they cover the work, not only its launch."""
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0 = time.perf_counter()
+    start.record()
+    out = None
+    for _ in range(calls):
+        out = fn()
+    end.record()
+    torch.cuda.synchronize()
+    return start.elapsed_time(end) / calls, 1e3 * (time.perf_counter() - t0) / calls, out

@@ -8,15 +8,14 @@ Workloads (f16 feature maps, 128 channels):
                      issued in chunks of 8 source frames in update_lowmem's order (factor_graph.py:284-296)
   single_512_48x64   one 512-edge call, 72 frames
   single_512_72x96   one 512-edge call at c5's image size, 128 frames
-The pyramid build (AltCorrBlock.__init__ over all frames) and the lookups (__call__) are timed separately with CUDA events, the two
-paths alternating, median of --reps rounds.  Outputs of both paths are compared with torch.equal in the same run.
+The pyramid build (AltCorrBlock.__init__ over all frames) and the lookups (__call__) are timed separately, the two paths alternating,
+median of --reps rounds.  Outputs of both paths are compared with torch.equal in the same run.
 MACs = 4 levels x HW x 64 taps x C per edge.  Compulsory bytes per edge = source level-0 map + target maps of all levels + coords +
 output (the 0.79 MB per map at 48x64 of SURVEY section 8d; frames shared between edges are counted once per edge).
-Prints one JSON line per workload and a header line with the card name and power limit."""
+Prints a header line naming the card, then one JSON line per workload."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -24,22 +23,15 @@ import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import droid_slam_b200  # noqa: E402
 from droid_slam_b200 import synth  # noqa: E402
 from droid_slam_b200.modules import install_alt_corr_hook  # noqa: E402
+from util import card, timed  # noqa: E402
 
 be = droid_slam_b200.install()
 dev = "cuda"
 LEVELS, C = 4, 128
-
-
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
-        name, power, clock = [s.strip() for s in r.stdout.strip().splitlines()[torch.cuda.current_device()].split(",")]
-    except Exception as e:  # the numbers are still valid; the card is then described by torch alone
-        name, power, clock = torch.cuda.get_device_name(), "unknown (%s)" % type(e).__name__, "unknown"
-    return {"card": name, "power_limit": power, "max_sm_clock": clock}
 
 
 def ref_pyramid(fmaps):
@@ -71,19 +63,6 @@ class _Stub:
 Hooked = install_alt_corr_hook(type("m", (), {"AltCorrBlock": type("AltCorrBlock", (_Stub,), {})})).AltCorrBlock
 
 
-def elapsed_ms(fn, warm=2, n=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / n
-
-
 def median(xs):
     xs = sorted(xs)
     return xs[len(xs) // 2]
@@ -100,10 +79,10 @@ def workload(name, n_frames, ht, wd, ii, jj, coords, chunks, reps):
         equal = all(torch.equal(ref_lookup(ref_pyr, *a), blk(*a)) for a in calls)
         t = {"ref_pyramid": [], "hook_pyramid": [], "ref_lookup": [], "hook_lookup": []}
         for _ in range(reps):   # alternate the two paths so that drift on a shared host hits both
-            t["ref_pyramid"].append(elapsed_ms(lambda: ref_pyramid(fmaps)))
-            t["hook_pyramid"].append(elapsed_ms(lambda: Hooked(fmaps)))
-            t["ref_lookup"].append(elapsed_ms(lambda: [ref_lookup(ref_pyr, *a) for a in calls], warm=1))
-            t["hook_lookup"].append(elapsed_ms(lambda: [blk(*a) for a in calls], warm=1))
+            t["ref_pyramid"].append(timed(lambda: ref_pyramid(fmaps), calls=3, warmup=2)[0])
+            t["hook_pyramid"].append(timed(lambda: Hooked(fmaps), calls=3, warmup=2)[0])
+            t["ref_lookup"].append(timed(lambda: [ref_lookup(ref_pyr, *a) for a in calls], calls=3, warmup=1)[0])
+            t["hook_lookup"].append(timed(lambda: [blk(*a) for a in calls], calls=3, warmup=1)[0])
     t = {k: median(v) for k, v in t.items()}
     HW = ht * wd
     macs = E * LEVELS * HW * 64 * C

@@ -8,17 +8,14 @@ lietorch stand-in, the seven slice copies, then a synchronisation so that both e
 Shapes: buffers of 512 and 1024 keyframes at 48x64 and 44x69 feature maps (384x512 and 352x552 images), a round with t0 = 300 and 64
 new keyframes, mono (the scale aligned) and RGB-D (sensor depth on every keyframe); both videos on cuda:0, and frontend on cuda:0 with
 backend on cuda:1 when two GPUs are visible.  Host clock around each round (each ends in a synchronisation), the two paths alternating,
-median over --reps rounds after --warmup of each.  Host syncs per round counted with torch.cuda.set_sync_debug_mode("warn").  The
-reference's lietorch is a CUDA extension; the stand-in runs the same group operations as ATen kernels, so the reference-flow figure is
-an estimate of the reference's launch chain, not a run of it.  The card's name, power limit and SM clocks are printed with the numbers."""
+median over --reps rounds after --warmup of each.  The reference's lietorch is a CUDA extension; the stand-in runs the same group
+operations as ATen kernels, so the reference-flow figure is an estimate of the reference's launch chain, not a run of it."""
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
-import warnings
 
 import torch
 
@@ -29,6 +26,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from droid_slam_b200 import modules  # noqa: E402
 from oracle.async_backend import SE3, align_pose_fragments  # noqa: E402
 import async_stubs  # noqa: E402
+from util import card, host_syncs  # noqa: E402
 
 
 def reference_round(front, back, t0, t1, device):
@@ -54,27 +52,6 @@ def reference_round(front, back, t0, t1, device):
 
 def native_round(video1, video2, t0, t1, device):
     modules.handover_round(video1, video2, t0, t1)
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum(str(w.message).startswith("called a synchronizing") for w in caught)      # not the prototype-feature notice
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except OSError:
-        out = ""
-    return dict(zip(q.split(","), [s.strip() for s in out.split(",")])) if out else {"name": torch.cuda.get_device_name(0)}
 
 
 def main():
@@ -107,7 +84,7 @@ def main():
                             b = time.perf_counter()
                             if r >= args.warmup:
                                 times[p].append(1e3 * (b - a))
-                    n_sync = {p: syncs(lambda: fn(v1, v2, t0, t1, dev2)) for p, fn in paths}
+                    n_sync = {p: host_syncs(lambda: fn(v1, v2, t0, t1, dev2))[0] for p, fn in paths}
                     row = dict(frontend=dev1, backend=dev2, buffer=buffer, ht=ht, wd=wd, mode=mode,
                                native_ms=statistics.median(times["native"]), reference_flow_ms=statistics.median(times["reference flow"]),
                                native_syncs=n_sync["native"], reference_flow_syncs=n_sync["reference flow"])

@@ -8,13 +8,12 @@ bench config c5 -> 72x96, and 48x64 (TartanAir 384x512) as the control that runs
   build:  corr_volume_pyramid (one launch; plus the staging copy when wd % 8 != 0) against torch.matmul of the /4-scaled maps +
           3x avg_pool2d (CorrBlock.__init__).  Reported as achieved GB/s over the 1.33 * HW^2 * 2 bytes of volume per edge.
   lookup: corr_lookup_pyramid (one launch, reference layout) against 4x corr_index_forward + cat (CorrBlock.__call__).
-CUDA events around each call, the two paths alternating, median of --reps rounds.  The volumes are compared (max |diff| against the
+Each call timed on its own, the two paths alternating, median of --reps rounds.  The volumes are compared (max |diff| against the
 cuBLAS pipeline, 6e-2 in f16) and the lookups with torch.equal in the same run.  The first line describes the card."""
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -22,22 +21,14 @@ import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import droid_slam_b200  # noqa: E402
+from util import card, timed  # noqa: E402
 
 be = droid_slam_b200.install()
 dev = "cuda"
 C = 128
 SIZES = [("tum", 30, 40), ("eth3d", 43, 70), ("euroc_raw", 44, 69), ("video_16x9", 41, 73), ("c5", 72, 96), ("control_48x64", 48, 64)]
-
-
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30)
-        name, power, maxclk, clk = [s.strip() for s in r.stdout.strip().splitlines()[torch.cuda.current_device()].split(",")]
-    except Exception as e:  # the numbers are still valid; the card is then described by torch alone
-        name, power, maxclk, clk = torch.cuda.get_device_name(), "unknown (%s)" % type(e).__name__, "unknown", "unknown"
-    return {"card": name, "power_limit": power, "max_sm_clock": maxclk, "sm_clock_at_start": clk}
 
 
 def ref_build(f, ii, jj):
@@ -55,15 +46,6 @@ def ref_lookup(pyr, coords):
     return torch.cat([be.corr_index_forward(pyr[l], coords / 2 ** l, 3)[0].view(E, 49, ht, wd) for l in range(4)], dim=1)
 
 
-def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    out = fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1), out
-
-
 def run(name, ht, wd, E, reps, g):
     N = max(8, E // 4)
     f = torch.randn(N, C, ht, wd, generator=g).half().to(dev)
@@ -77,8 +59,8 @@ def run(name, ht, wd, E, reps, g):
     torch.cuda.synchronize()
     tb_n, tb_r = [], []
     for _ in range(reps):
-        t, _ = timed(nat); tb_n.append(t)
-        t, _ = timed(ref); tb_r.append(t)
+        tb_n.append(timed(nat)[0])
+        tb_r.append(timed(ref)[0])
     pyr, rpyr = nat(), ref()
     err = 0.0
     for l in range(4):
@@ -91,8 +73,8 @@ def run(name, ht, wd, E, reps, g):
     lk_n(); lk_r()
     tl_n, tl_r = [], []
     for _ in range(reps):
-        t, a = timed(lk_n); tl_n.append(t)
-        t, b = timed(lk_r); tl_r.append(t)
+        t, _, a = timed(lk_n); tl_n.append(t)
+        t, _, b = timed(lk_r); tl_r.append(t)
     same = bool(torch.equal(a, b))
     HW = ht * wd
     vol_bytes = E * HW * HW * 2 * (1 + 1 / 4 + 1 / 16 + 1 / 64)
@@ -128,7 +110,7 @@ def main():
             r = run(name, ht, wd, E, args.reps, g)
             lines.append(r)
             print(json.dumps(r), flush=True)
-    lines[0]["sm_clock_at_end"] = card()["sm_clock_at_start"]
+    lines[0]["sm_clock_at_end"] = card()["sm_clock"]
     if args.out:
         with open(args.out, "w") as fh:
             json.dump(lines, fh, indent=1)

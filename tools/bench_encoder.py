@@ -5,14 +5,13 @@ autocast (cuDNN convolutions + ATen instance norms, as the reference runs) again
     python tools/bench_encoder.py --profile [--trace-dir DIR]     # one torch.profiler run of hooked fnet + cnet at n = 1, 384x512
 
 Workloads, at 384x512 and 352x552: fnet n = 1 and cnet n = 1 (MotionFilter.track, per frame), fnet n = 16 (one PoseTrajectoryFiller
-batch); plus native fnet + cnet at n = 1 (384x512) captured as one CUDA graph.  CUDA events, the two paths alternating, median of --reps
-rounds of 20 calls each after warm-up.  FLOP/s from the shape-derived FLOPs (2 MACs per conv tap, every convolution of the encoder).
-Prints one JSON line per workload and a header line with the card name, power limit and SM clock read in the same run."""
+batch); plus native fnet + cnet at n = 1 (384x512) captured as one CUDA graph.  The two paths alternating, median of --reps rounds of
+20 calls each after warm-up.  FLOP/s from the shape-derived FLOPs (2 MACs per conv tap, every convolution of the encoder).  Prints a
+header line naming the card, then one JSON line per workload."""
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import types
 
@@ -20,24 +19,16 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import droid_slam_b200  # noqa: E402
 import oracle.encoder as oenc  # noqa: E402
 from droid_slam_b200 import synth  # noqa: E402
 from droid_slam_b200.encoder import pack_encoder_weights  # noqa: E402
+from util import card, timed  # noqa: E402
 
 be = droid_slam_b200.install()
 dev = "cuda"
 ENC = {"fnet": ("instance", 128, 1, 0), "cnet": ("none", 256, 0, 1)}   # norm_fn, output_dim, norm code, weight seed
-
-
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30)
-        name, power, clock, maxclock = [s.strip() for s in r.stdout.strip().splitlines()[torch.cuda.current_device()].split(",")]
-    except Exception as e:  # the numbers are still valid; the card is then described by torch alone
-        name, power, clock, maxclock = torch.cuda.get_device_name(), "unknown (%s)" % type(e).__name__, "unknown", "unknown"
-    return {"card": name, "power_limit": power, "sm_clock": clock, "max_sm_clock": maxclock}
 
 
 def flops(H, W, output_dim):
@@ -53,13 +44,7 @@ def time_rounds(fns, reps, calls=20):
     ts = {k: [] for k in fns}
     for _ in range(reps):
         for k, f in fns.items():
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            for _ in range(calls):
-                f()
-            b.record()
-            b.synchronize()
-            ts[k].append(a.elapsed_time(b) / calls)
+            ts[k].append(timed(f, calls)[0])
     return {k: statistics.median(v) for k, v in ts.items()}
 
 

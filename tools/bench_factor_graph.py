@@ -6,9 +6,8 @@
   c3         one update_lowmem step on the 2048-edge / 400-keyframe global-BA graph at 48x64 (synth "c3_global")
   rig2       one update_lowmem step with use_inactive at 43x70, rig 2 (stereo)
 
-CUDA events around each call, the two paths alternating, median over --reps rounds after --warmup calls of each.  Host synchronisations
-per call are counted with torch.cuda.set_sync_debug_mode("warn"), BA's own status reads excluded.  The card's name, power limit and SM
-clock are read in the same run.
+Each call timed on its own, the two paths alternating, median over --reps rounds after --warmup calls of each.  BA's own status reads
+are left out of the host-sync count (the stub video's ba).
 
     python tools/bench_factor_graph.py [--reps 15] [--warmup 3] [--json out.json]
 """
@@ -16,9 +15,7 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
-import warnings
 
 import torch
 
@@ -29,6 +26,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import oracle.factor_graph as ofg  # noqa: E402
 from droid_slam_b200 import modules, synth  # noqa: E402
 import factor_graph_stubs as fs  # noqa: E402
+from util import card, host_syncs, timed  # noqa: E402
 
 
 def frontend():
@@ -76,37 +74,6 @@ def reference_flow(graph, method, kw):
         ofg.update_lowmem(graph, alt_corr_block=fs.AltCorrBlock, **kw)
 
 
-def timed(fn):
-    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    start.record()
-    fn()
-    end.record()
-    end.synchronize()
-    return start.elapsed_time(end)
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum("synchroniz" in str(w.message) for w in caught)
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except OSError:
-        out = ""
-    return dict(zip(q.split(","), [s.strip() for s in out.split(",")])) if out else {"name": torch.cuda.get_device_name(0)}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=15)
@@ -126,8 +93,8 @@ def main():
             times = {p: [] for p, _, _ in paths}
             for r in range(args.reps):
                 for p, fn, g in (paths if r % 2 == 0 else paths[::-1]):
-                    times[p].append(timed(lambda: fn(g, method, kw)))
-            n_sync = {p: syncs(lambda: fn(g, method, kw)) for p, fn, g in paths}
+                    times[p].append(timed(lambda: fn(g, method, kw))[0])
+            n_sync = {p: host_syncs(lambda: fn(g, method, kw))[0] for p, fn, g in paths}
             row = dict(shape=name, edges=int(g_nat.ii.numel()),
                        native_ms=statistics.median(times["native"]), reference_flow_ms=statistics.median(times["reference flow"]),
                        native_syncs=n_sync["native"], reference_flow_syncs=n_sync["reference flow"])

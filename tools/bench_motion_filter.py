@@ -6,10 +6,8 @@ droid_slam_b200.update.UpdateModule).
 Synthetic stream: synth.make_frames, 1000 frames of one camera at 384x512 and at 352x552 (48x64 and 44x69 feature maps), held on the
 host as a camera delivers them; thresh is set by bisection on the native path over the whole stream, aiming at a third of the frames as
 keyframes (the count is not monotonic in thresh, so the count reached is reported).  Each pass runs the whole stream on a fresh filter and video; the two paths alternate, median over --reps passes
-after --warmup passes of each.  Per frame: wall time (the host clock around the pass, which ends in a device synchronise; every frame
-waits for its own statistic, so this is what a caller sees), CUDA-event time over the pass, and host synchronisations counted with
-torch.cuda.set_sync_debug_mode("warn").  The two paths must make the same keyframe decisions.  The card's name, power limit and SM
-clock are read in the same run.
+after --warmup passes of each.  Per frame: wall time (every frame waits for its own statistic, so this is what a caller sees), event
+time and host synchronisations.  The two paths must make the same keyframe decisions.
 
     python tools/bench_motion_filter.py [--reps 3] [--warmup 1] [--frames 1000] [--json out.json]
 """
@@ -17,16 +15,14 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 import types
-import warnings
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 import droid_slam_b200  # noqa: E402
@@ -35,6 +31,7 @@ from oracle import motion_filter as omf  # noqa: E402
 from droid_slam_b200 import modules, synth  # noqa: E402
 from droid_slam_b200.update import UpdateModule  # noqa: E402
 from make_motion_filter_golden import Video  # noqa: E402  (DepthVideo's buffers and append)
+from util import card, host_syncs, timed  # noqa: E402
 
 DEV = "cuda"
 SIZES = [(384, 512), (352, 552)]
@@ -101,39 +98,6 @@ def calibrate(parts, H, W, stream, share):
     return 0.5 * (lo + hi)
 
 
-def timed(fn):
-    """(wall ms, CUDA-event ms, result) of fn()"""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    a.record()
-    out = fn()
-    b.record()
-    torch.cuda.synchronize()
-    return 1e3 * (time.perf_counter() - t0), a.elapsed_time(b), out
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum("called a synchronizing CUDA operation" in str(w.message) for w in caught)
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except OSError:
-        out = ""
-    return dict(zip(q.split(","), [s.strip() for s in out.split(",")])) if out else {"name": torch.cuda.get_device_name(0)}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
@@ -161,14 +125,14 @@ def main():
             for r in range(args.reps):
                 for p, fn in (paths if r % 2 == 0 else paths[::-1]):
                     filt = fresh()
-                    w, e, decisions[p] = timed(lambda: fn(filt, stream, CorrBlock))
+                    e, w, decisions[p] = timed(lambda: fn(filt, stream, CorrBlock))
                     wall[p].append(w)
                     event[p].append(e)
             assert decisions["native"] == decisions["reference flow"], "the two flows made different keyframe decisions"
             n_sync = {}
             for p, fn in paths:
                 filt = fresh()
-                n_sync[p] = syncs(lambda: fn(filt, stream, CorrBlock))
+                n_sync[p] = host_syncs(lambda: fn(filt, stream, CorrBlock))[0]
             n = len(stream)
             row = dict(input="%dx%d" % (H, W), frames=n, keyframes=decisions["native"][-1], thresh=thresh)
             for p, key in (("native", "native"), ("reference flow", "reference_flow")):

@@ -4,9 +4,8 @@ running on the hooked native operators (native encoder, CorrBlock, reprojection,
 The lietorch calls of that flow run on the pure-torch stand-in (oracle/shims), the only lietorch available here.
 
 Synthetic video: 100 keyframes stamped 10 frames apart, a stream of 1000 frames, at 384x512 and 352x552 input (48x64 and 44x69 feature
-maps).  CUDA events around each whole stream, the two paths alternating, median over --reps rounds after --warmup runs of each.  Host
-synchronisations per stream are counted with torch.cuda.set_sync_debug_mode("warn") (all of them, BA's status reads included).  The
-card's name, power limit and SM clock are read in the same run.
+maps).  Each whole stream timed, the two paths alternating, median over --reps rounds after --warmup runs of each.  The host-sync count
+per stream includes BA's status reads.
 
     python tools/bench_trajectory_filler.py [--reps 3] [--warmup 1] [--frames 1000] [--json out.json]
 """
@@ -14,16 +13,15 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import types
-import warnings
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import lietorch  # noqa: E402  (the stand-in)
 import droid_slam_b200  # noqa: E402
@@ -31,6 +29,7 @@ import oracle.encoder as oenc  # noqa: E402
 from oracle import trajectory_filler as otf  # noqa: E402
 from droid_slam_b200 import modules, synth  # noqa: E402
 from droid_slam_b200.update import UpdateModule  # noqa: E402
+from util import card, host_syncs, timed  # noqa: E402
 
 DEV = "cuda"
 KEYFRAMES = 100
@@ -122,37 +121,6 @@ def reference_flow(filler, stream, CorrBlock):
     return otf.fill(filler, stream, graph, lietorch.SE3)[0]
 
 
-def timed(fn):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    a.record()
-    fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b)
-
-
-def syncs(fn):
-    torch.cuda.synchronize()
-    with warnings.catch_warnings(record=True) as caught:
-        warnings.simplefilter("always")
-        torch.cuda.set_sync_debug_mode("warn")
-        try:
-            fn()
-        finally:
-            torch.cuda.set_sync_debug_mode(0)
-    return sum("synchroniz" in str(w.message) for w in caught)
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i", "0"], capture_output=True, text=True).stdout.strip()
-    except OSError:
-        out = ""
-    return dict(zip(q.split(","), [s.strip() for s in out.split(",")])) if out else {"name": torch.cuda.get_device_name(0)}
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
@@ -174,8 +142,8 @@ def main():
             times = {p: [] for p, _ in paths}
             for r in range(args.reps):
                 for p, fn in (paths if r % 2 == 0 else paths[::-1]):
-                    times[p].append(timed(lambda: fn(filler, stream, CorrBlock)))
-            n_sync = {p: syncs(lambda: fn(filler, stream, CorrBlock)) for p, fn in paths}
+                    times[p].append(timed(lambda: fn(filler, stream, CorrBlock))[0])
+            n_sync = {p: host_syncs(lambda: fn(filler, stream, CorrBlock))[0] for p, fn in paths}
             got, want = native(filler, stream, None), reference_flow(filler, stream, CorrBlock)
             dt = float((got[:, :3] - want[:, :3]).norm(dim=1).max()) / float(want[:, :3].norm(dim=1).max())
             n = len(stream)

@@ -5,9 +5,9 @@ bench.py:reference_update_operator_ms times it.
   43x70  ETH3D through evaluation_scripts/test_eth3d.py        44x69  raw EuRoC through demo.py      41x73  16:9 video through demo.py
   48x64, 30x40, 72x96: widths that are multiples of 8 (rectangular tiles), as controls
 
-512 edges over 72 source frames, with flow and aggregation.  CUDA events around each call, the two paths alternating, the median of
---rounds rounds of --iters calls.  TFLOP/s counts the useful FLOPs (SURVEY section 8d): 14.03 GFLOP per edge and 1.37 GFLOP per source
-frame at 48x64, scaled by HW / 3072.  Prints the card, its power limit and SM clock, then one JSON line per size.
+512 edges over 72 source frames, with flow and aggregation.  The two paths alternating, the median of --rounds rounds of --iters
+calls.  TFLOP/s counts the useful FLOPs (SURVEY section 8d): 14.03 GFLOP per edge and 1.37 GFLOP per source frame at 48x64, scaled by
+HW / 3072.  Prints the card, then one JSON line per size, then the card again.
 
   python tools/bench_update_sizes.py [--sizes 43x70,44x69] [--edges 512] [--frames 72] [--rounds 7] [--iters 5]
 """
@@ -15,36 +15,17 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from util import card, timed  # noqa: E402
 
 SIZES = "43x70,44x69,41x73,48x64,30x40,72x96"
 GFLOP_EDGE, GFLOP_FRAME = 14.03, 1.37
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                           capture_output=True, text=True, timeout=30)
-        vals = [v.strip() for v in r.stdout.strip().split(",")]
-        return dict(zip(q.split(","), vals)) if len(vals) == 4 else {"name": torch.cuda.get_device_name(), "nvidia-smi": r.stdout.strip()}
-    except (OSError, subprocess.SubprocessError) as e:
-        return {"name": torch.cuda.get_device_name(), "nvidia-smi": str(e)}
-
-
-def time_ms(fn, iters):
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / iters
 
 
 def run_size(ht, wd, E, frames, rounds, iters, dev):
@@ -75,8 +56,8 @@ def run_size(ht, wd, E, frames, rounds, iters, dev):
             native(); reference()
         t_nat, t_ref = [], []
         for _ in range(rounds):
-            t_nat.append(time_ms(native, iters))
-            t_ref.append(time_ms(reference, iters))
+            t_nat.append(timed(native, iters)[0])
+            t_ref.append(timed(reference, iters)[0])
     n_src = min(E, frames)
     gflop = (GFLOP_EDGE * E + GFLOP_FRAME * n_src) * ht * wd / 3072.0
     ms_n, ms_r = statistics.median(t_nat), statistics.median(t_ref)

@@ -1,24 +1,16 @@
 """CUDA-event timing of the damped SPD solve (`dba_solve_spd`): 20 warm-up solves, then 200 back-to-back solves of one seeded system,
-printed with the card's name and power limit.  usage: python tools/chol_timing.py [n ...]   (default 426; n <= 448 runs the resident
-kernel, larger n the cluster kernel)."""
+printed with the card.  usage: python tools/chol_timing.py [n ...]   (default 426; n <= 448 runs the resident kernel, larger n the
+cluster kernel)."""
 import ctypes
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch  # noqa: E402
 from droid_slam_b200 import c_api  # noqa: E402
-
-
-def power_limit_w():
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-        return "%.0f W" % float(out)
-    except (OSError, ValueError, subprocess.SubprocessError):
-        return "unknown"
+from util import card, timed  # noqa: E402
 
 
 def time_solve(L, n):
@@ -36,29 +28,21 @@ def time_solve(L, n):
                                     ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(fail.data_ptr()), ctypes.c_void_p(ws.data_ptr()), ws.numel(), None),
                     "dba_solve_spd")
 
-    for _ in range(20):
-        solve()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(200):
-        solve()
-    e1.record()
-    torch.cuda.synchronize()
+    ms, _, _ = timed(solve, calls=200, warmup=20)
     Hd = Hc.clone()
     Hd.diagonal().add_(0.1 + 1e-4 * Hc.diagonal())
     ref = torch.linalg.solve(Hd, bc)
     err = float((x.cpu().double() - ref).abs().max() / ref.abs().max())
-    return 1e3 * e0.elapsed_time(e1) / 200, int(fail), err
+    return 1e3 * ms, int(fail), err
 
 
 def main():
     L = c_api.load()
-    card = "%s, power limit %s" % (torch.cuda.get_device_name(), power_limit_w())
+    gpu = card()
     for n in [int(a) for a in sys.argv[1:]] or [426]:
         us, fail, err = time_solve(L, n)
         print("n=%d  %s kernel: %.1f us per solve (200 back-to-back), fail=%d, max rel err vs fp64 LAPACK %.2e  [%s]"
-              % (n, "resident" if n <= 448 else "cluster", us, fail, err, card))
+              % (n, "resident" if n <= 448 else "cluster", us, fail, err, gpu))
 
 
 if __name__ == "__main__":
