@@ -810,6 +810,83 @@ std::vector<torch::Tensor> fragment_handover(std::vector<torch::Tensor> front, s
   return {diag};
 }
 
+// ---- Lie groups SO3 / SE3 (droid_slam_b200/lietorch) -------------------------------------------------------------------------------
+constexpr torch::ScalarType F64 = torch::kFloat64;
+
+// The checks of one lie_forward / lie_backward call: the operands' device and dtype (float32 / float64, one for all), the last dimension
+// of each (the operation's record sizes), the rank and broadcast compatibility (each batch size equal or 1, at most DBA_LIE_MAX_DIMS batch
+// dimensions).  Makes the operands contiguous (never expanded) and gives the output batch shape and each operand's batch strides in
+// records, 0 where it broadcasts.
+struct LieCall {
+  int da = 0, db = 0, dout = 0;
+  torch::Tensor a, b;
+  std::vector<int64_t> shape, sa, sb;
+  LieCall(const char* fn, int op, int group, const torch::Tensor& a_in, const c10::optional<torch::Tensor>& b_in, const Expect& expect) {
+    TORCH_CHECK(dba_lie_record_sizes(op, group, &da, &db, &dout) == DBA_OK, "droid_backends.", fn, ": no operation ", op, " for group ", group);
+    expect(a_in, "a", {F32, F64}, {}, kAnyLayout);
+    TORCH_CHECK(a_in.dim() >= 1 && a_in.size(-1) == da, "droid_backends.", fn, ": a must be [...,", da, "], got shape ", a_in.sizes());
+    const int64_t nd = a_in.dim() - 1;
+    TORCH_CHECK(nd <= DBA_LIE_MAX_DIMS, "droid_backends.", fn, ": at most ", DBA_LIE_MAX_DIMS, " batch dimensions, got ", nd);
+    a = a_in.contiguous();
+    if (db > 0) {
+      TORCH_CHECK(b_in.has_value() && b_in->defined(), "droid_backends.", fn, ": operation ", op, " takes a second operand");
+      expect(*b_in, "b", {a_in.scalar_type()}, {}, kAnyLayout);
+      TORCH_CHECK(b_in->dim() == a_in.dim() && b_in->size(-1) == db, "droid_backends.", fn, ": b must be [...,", db, "] of a's rank ",
+                  a_in.dim(), ", got shape ", b_in->sizes());
+      b = b_in->contiguous();
+    } else {
+      TORCH_CHECK(!b_in.has_value() || !b_in->defined(), "droid_backends.", fn, ": operation ", op, " takes one operand");
+    }
+    shape.resize(nd); sa.resize(nd); sb.resize(nd, 0);
+    int64_t ra = 1, rb = 1;
+    for (int64_t d = nd - 1; d >= 0; d--) {
+      const int64_t n = a.size(d), m = db > 0 ? b.size(d) : n;
+      TORCH_CHECK(n == m || n == 1 || m == 1, "droid_backends.", fn, ": a ", a.sizes(), " and b ", b.sizes(), " do not broadcast in dimension ", d,
+                  " (sizes must be equal or 1)");
+      shape[d] = n == 1 ? m : n;
+      sa[d] = n == 1 ? 0 : ra;
+      ra *= n;
+      if (db > 0) { sb[d] = m == 1 ? 0 : rb; rb *= m; }
+    }
+  }
+  std::vector<int64_t> out_sizes(int64_t last) const { auto s = shape; s.push_back(last); return s; }
+};
+
+torch::Tensor lie_forward(int op, int group, torch::Tensor a, c10::optional<torch::Tensor> b) {
+  const Expect expect("lie_forward", a, "a");
+  const LieCall c("lie_forward", op, group, a, b, expect);
+  c10::cuda::CUDAGuard guard(expect.dev);
+  auto out = torch::empty(c.out_sizes(c.dout), c.a.options());
+  check_status(dba_lie_forward(op, group, c.a.scalar_type() == F64 ? DBA_F64 : DBA_F32, c.a.data_ptr(), c.sa.data(),
+                               c.db > 0 ? c.b.data_ptr() : nullptr, c.db > 0 ? c.sb.data() : nullptr, out.data_ptr(), (int)c.shape.size(),
+                               c.shape.data(), cur_stream()), "lie_forward");
+  return out;
+}
+
+// need_a / need_b: which gradients to compute; one not asked for is returned as None and never computed (at least one must be asked for)
+std::vector<c10::optional<torch::Tensor>> lie_backward(int op, int group, torch::Tensor grad, torch::Tensor a, c10::optional<torch::Tensor> b,
+                                                       bool need_a, bool need_b) {
+  const Expect expect("lie_backward", a, "a");
+  const LieCall c("lie_backward", op, group, a, b, expect);
+  const auto grad_sizes = c.out_sizes(c.dout);
+  expect(grad, "grad", {a.scalar_type()}, dims(grad_sizes), kAnyLayout);
+  c10::cuda::CUDAGuard guard(expect.dev);
+  need_b = need_b && c.db > 0;
+  TORCH_CHECK(need_a || need_b, "droid_backends.lie_backward: no gradient asked for");
+  auto g = grad.contiguous();
+  const bool empty = g.numel() == 0;
+  torch::Tensor ga, gb;
+  if (need_a) ga = empty ? torch::zeros_like(c.a) : torch::empty_like(c.a);
+  if (need_b) gb = empty ? torch::zeros_like(c.b) : torch::empty_like(c.b);
+  check_status(dba_lie_backward(op, group, c.a.scalar_type() == F64 ? DBA_F64 : DBA_F32, g.data_ptr(), c.a.data_ptr(), c.sa.data(),
+                                c.db > 0 ? c.b.data_ptr() : nullptr, c.db > 0 ? c.sb.data() : nullptr, need_a ? ga.data_ptr() : nullptr,
+                                need_b ? gb.data_ptr() : nullptr, (int)c.shape.size(), c.shape.data(), cur_stream()), "lie_backward");
+  std::vector<c10::optional<torch::Tensor>> out;
+  out.push_back(need_a ? c10::optional<torch::Tensor>(ga) : c10::nullopt);
+  if (c.db > 0) out.push_back(need_b ? c10::optional<torch::Tensor>(gb) : c10::nullopt);
+  return out;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
   // bundle adjustment kernels
@@ -867,5 +944,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "-> [diagnostics (s, dG, align_scale)] or [], native extension",
         pybind11::arg("front"), pybind11::arg("back"), pybind11::arg("t0"), pybind11::arg("t1"), pybind11::arg("stereo"),
         pybind11::arg("diagnostics") = false);
+  m.def("lie_forward", &lie_forward, "SO3 / SE3 group operation (group 1: SO3, 3: SE3; op: include/droid_b200.h DBA_LIE_*) with broadcasting in "
+        "the kernel -> out, native extension", pybind11::arg("op"), pybind11::arg("group"), pybind11::arg("a"), pybind11::arg("b") = pybind11::none());
+  m.def("lie_backward", &lie_backward, "gradients of lie_forward (lietorch's convention; broadcast operands reduced in the kernel) -> [grad_a(, "
+        "grad_b)], None for a gradient not asked for, native extension", pybind11::arg("op"), pybind11::arg("group"), pybind11::arg("grad"),
+        pybind11::arg("a"), pybind11::arg("b") = pybind11::none(), pybind11::arg("need_a") = true, pybind11::arg("need_b") = true);
   m.def("_b200_native", []() { return true; });
 }

@@ -33,6 +33,8 @@ kernel for is offered as a hook:
   * `install_async_hook(droid_async)`: DroidAsync's backend process (droid_async.py:37-130), started with `spawn`, re-installs every hook
     of the parent (`hook_registry`) and runs the reference's loop with the frontend -> backend hand-over on the device
     (`handover_round` -> `droid_backends.fragment_handover`, one host sync per round).
+  * `droid_slam_b200.install_dependencies()` (the package's, recorded here too): `lietorch` / `torch_scatter` resolve to the package's own,
+    in the spawned backend before its arguments are unpickled (`_unpickle_backend`).
 
 The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
 it.  If not, strict=True (the default) raises RuntimeError naming the replaced method and the reason; strict=False runs the reference's
@@ -861,12 +863,21 @@ def hook_registry():
     return copy.deepcopy(_HOOKS)
 
 
+def _installer(name):
+    """the function a registry entry's installer names: an install_* hook of this module, or the package's install_dependencies (which
+    takes no target)"""
+    if name == "install_dependencies":
+        from . import install_dependencies
+        return lambda target, **kwargs: install_dependencies()
+    return globals()[name]
+
+
 def reinstall_hooks(hooks):
     """install every transferable hook of `hooks` (as hook_registry gives them) in this interpreter, by module name, in order"""
     install()
     for e in hooks:
         if e["transferable"]:
-            globals()[e["installer"]](_resolve(e["module"], e["qualname"]), **e["kwargs"])
+            _installer(e["installer"])(_resolve(e["module"], e["qualname"]), **e["kwargs"])
 
 
 def install_update_module_hook(droid_net_module):
@@ -948,13 +959,24 @@ def _backend_loop(mod, args, front, back, device="cuda"):
                 time.sleep(_BACKEND_PAUSE_S)
 
 
+def _unpickle_backend(module, strict, reference, hooks, native):
+    """a BackendProcess as a spawned interpreter unpickles it.  The Process object pickles its target before its arguments, so this runs
+    before DepthVideo is unpickled -- which imports the reference's depth_video and, with it, `lietorch`: a recorded install_dependencies
+    therefore registers the packages here, not in prepare()"""
+    if any(e["installer"] == "install_dependencies" and e["transferable"] for e in hooks or ()):
+        from . import install_dependencies
+        install_dependencies()
+    return BackendProcess(module, strict, reference, hooks, native)
+
+
 class BackendProcess:
     """The `backend_process` install_async_hook puts into the reference's droid_async module; DroidAsync starts it as a Process target.
 
     Pickled (which is how `spawn` hands it to the new interpreter) it carries the hook registry of that moment, checked first: a hook on
     an object that cannot be imported by name, or a missing hook of the native backend (_BACKEND_HOOKS), raises under strict=True --
     in the parent, as DroidAsync starts the process -- and makes the child run the reference's own backend_process under strict=False.
-    In the child, __call__ runs droid_slam_b200.install(), re-installs every recorded hook by module name, then the native loop.  Called
+    In the child, unpickling runs a recorded install_dependencies first (_unpickle_backend); __call__ runs droid_slam_b200.install(),
+    re-installs every recorded hook by module name, then the native loop.  Called
     without pickling (in the installing process, or a forked child, where the hooks are in place) it checks the same and runs the loop."""
 
     def __init__(self, module, strict=True, reference=None, hooks=None, native=None):
@@ -962,11 +984,11 @@ class BackendProcess:
 
     def __reduce__(self):
         if self.native is not None:                          # already a snapshot
-            return BackendProcess, (self.module, self.strict, None, self.hooks, self.native)
+            return _unpickle_backend, (self.module, self.strict, None, self.hooks, self.native)
         why = _async_unsupported(_HOOKS)
         if why is not None and self.strict:
             _require("droid_async.backend_process", why)
-        return BackendProcess, (self.module, self.strict, None, hook_registry(), why is None)
+        return _unpickle_backend, (self.module, self.strict, None, hook_registry(), why is None)
 
     def prepare(self):
         """install the native extension and the carried hooks in this interpreter -> the droid_async module"""

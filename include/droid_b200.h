@@ -428,6 +428,37 @@ int dba_solve_spd(const double* H, const double* b, int n, float lm, float ep, f
  * (i == number of tile rows: a right-hand-side piece; 0xFF: none).  Returns the cluster size, 0 when n is served by the barrier kernel. */
 int dba_solve_tile_placement(int n, unsigned char* map_i, unsigned char* map_j);
 
+/* ---- Lie groups SO3 / SE3 (the `lietorch` package, droid_slam_b200/lietorch) ---------------------------------------------------------
+ * replaces lietorch_backends.* (reference thirdparty/lietorch/lietorch/src/lietorch_gpu.cu).  group: DBA_LIE_SO3 (data qx,qy,qz,qw;
+ * tangent 3) or DBA_LIE_SE3 (data tx,ty,tz,qx,qy,qz,qw; tangent tau,phi); dtype DBA_F32 or DBA_F64 for every operand.  The quaternion is
+ * normalised on load; exp / log / the left Jacobian and its inverse take their small-angle branches below lietorch's EPS = 1e-6.
+ * Operands a (and b for the binary ops), records of dba_lie_record_sizes' sizes, the last dimension contiguous.  Broadcasting: the
+ * output batch is shape[ndim] (0 <= ndim <= DBA_LIE_MAX_DIMS); a_strides / b_strides [ndim] are each operand's batch strides in records,
+ * 0 where it broadcasts (its size 1).  out and grad are contiguous over shape.  No operand is copied to the output's batch.
+ *   op          a            b              out
+ *   EXP         tangent      -              group            LOG        group   -        tangent
+ *   INV         group        -              group            MUL        group   group    group
+ *   ADJ / ADJT  group        tangent        tangent          JINV       group   tangent  tangent = Jl(log a)^-1 b
+ *   ACT         group        point [3]      point [3]        ACT4       group   [4]      [4] (homogeneous)
+ *   PROJECTOR   group        -              [N*N] row-major (the orthogonal projector vec() / InitFromVec's gradients use)
+ *   VEC / FROMVEC: backward only (their forward is the identity): grad_a = grad P(a) / grad pinv(P(a)), N entries each.
+ * dba_lie_backward: grad [shape, out record] -> grad_a laid out like a, grad_b like b, fully overwritten (nothing is written when the
+ * output batch is empty).  grad_a or grad_b may be NULL (not both, for a binary op): that gradient is neither computed nor written, so
+ * no reduction runs for a broadcast operand whose gradient is not asked for.  The gradient of a group operand is lietorch's left-tangent gradient d/de L(Exp(e) X) at e = 0 in the first K
+ * entries of its N-entry record, the rest 0; a group output's upstream gradient is read from the same K entries.  A broadcast operand's
+ * gradient is summed over its broadcast dimensions inside the launch, in a fixed order (bit-reproducible).  Jinv and PROJECTOR have no
+ * backward.  Neither entry point synchronises the host. */
+#define DBA_LIE_MAX_DIMS 8
+enum { DBA_LIE_SO3 = 1, DBA_LIE_SE3 = 3 };          /* lietorch's group ids */
+enum { DBA_LIE_EXP = 0, DBA_LIE_LOG, DBA_LIE_INV, DBA_LIE_MUL, DBA_LIE_ADJ, DBA_LIE_ADJT, DBA_LIE_JINV, DBA_LIE_ACT, DBA_LIE_ACT4,
+       DBA_LIE_PROJECTOR, DBA_LIE_VEC, DBA_LIE_FROMVEC, DBA_LIE_OPS };
+/* host only: the record sizes of operation op on group: *a, *b (0: unary), *out; DBA_ERR_INVALID for an unknown op or group */
+int dba_lie_record_sizes(int op, int group, int* a, int* b, int* out);
+int dba_lie_forward(int op, int group, int dtype, const void* a, const int64_t* a_strides, const void* b, const int64_t* b_strides,
+                    void* out, int ndim, const int64_t* shape, dba_stream_t stream);
+int dba_lie_backward(int op, int group, int dtype, const void* grad, const void* a, const int64_t* a_strides, const void* b,
+                     const int64_t* b_strides, void* grad_a, void* grad_b, int ndim, const int64_t* shape, dba_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
