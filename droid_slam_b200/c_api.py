@@ -16,6 +16,7 @@ SYMBOLS = [
     "dba_update_workspace_bytes", "dba_update_workspace_layout", "dba_update_forward", "dba_conv_nhwc", "dba_conv_nhwc_plan", "dba_encoder_workspace_bytes", "dba_encoder_forward",
     "dba_encoder_forward_frames", "dba_encoder_workspace_layout", "dba_encoder_forward_prefix", "dba_proximity_workspace_bytes", "dba_proximity_edges",
     "dba_fill_interpolate", "dba_pose_only_ba", "dba_fragment_handover", "dba_lie_record_sizes", "dba_lie_forward", "dba_lie_backward",
+    "dba_ba_layer_workspace_bytes", "dba_ba_layer_forward", "dba_ba_layer_backward",
 ]
 
 DBA_F32, DBA_F16, DBA_F64, DBA_BF16 = 0, 1, 2, 3

@@ -887,6 +887,93 @@ std::vector<c10::optional<torch::Tensor>> lie_backward(int op, int group, torch:
   return out;
 }
 
+// ---- the differentiable dense BA layer (droid_slam_b200.modules.ba_layer) ---------------------------------------------------------
+// The checks of one ba_layer_forward / ba_layer_backward call: every tensor fp32 (ii / jj int64), contiguous, on one device, with the
+// extents of include/droid_b200.h; fixedp in [0, N) and at most DBA_BA_LAYER_MAX_POSES pose unknowns.  Fills the args struct and the
+// workspace.
+static dba_ba_layer_args ba_layer_args(const char* fn, const Expect& expect, const torch::Tensor& target, const torch::Tensor& weight,
+                                       const torch::Tensor& eta, const torch::Tensor& poses, const torch::Tensor& disps,
+                                       const torch::Tensor& intrinsics, const torch::Tensor& ii, const torch::Tensor& jj, int64_t fixedp,
+                                       double ep, double lm, torch::Tensor& ws) {
+  expect(disps, "disps", {F32}, dims({kAny, kAny, kAny, kAny}));
+  const int64_t B = disps.size(0), N = disps.size(1), ht = disps.size(2), wd = disps.size(3);
+  expect(ii, "ii", {I64}, dims({kAny}));
+  const int64_t E = ii.size(0);
+  expect(jj, "jj", {I64}, dims({E}));
+  expect(target, "target", {F32}, dims({B, E, ht, wd, 2}));
+  expect(weight, "weight", {F32}, dims({B, E, ht, wd, 2}));
+  expect(eta, "eta", {F32}, dims({B, kAny, ht, wd}));
+  expect(poses, "poses", {F32}, dims({B, N, 7}));
+  expect(intrinsics, "intrinsics", {F32}, dims({B, N, 4}));
+  TORCH_CHECK(B >= 1 && N >= 1 && E >= 1 && ht >= 1 && wd >= 1 && eta.size(1) >= 1, "droid_backends.", fn,
+              ": empty batch, frames, edges, depth frames or image");
+  TORCH_CHECK(fixedp >= 0 && fixedp < N, "droid_backends.", fn, ": fixedp must be in [0, N) = [0, ", N, "), got ", fixedp);
+  TORCH_CHECK(N - fixedp <= DBA_BA_LAYER_MAX_POSES, "droid_backends.", fn, ": at most ", DBA_BA_LAYER_MAX_POSES,
+              " pose unknowns (N - fixedp) are factored in one launch, got ", N - fixedp);
+  dba_ba_layer_args a{};
+  a.target = target.data_ptr<float>(); a.weight = weight.data_ptr<float>(); a.eta = eta.data_ptr<float>();
+  a.poses = poses.data_ptr<float>(); a.disps = disps.data_ptr<float>(); a.intrinsics = intrinsics.data_ptr<float>();
+  a.ii = ii.data_ptr<int64_t>(); a.jj = jj.data_ptr<int64_t>();
+  a.B = (int)B; a.N = (int)N; a.E = (int)E; a.M = (int)eta.size(1); a.ht = (int)ht; a.wd = (int)wd; a.fixedp = (int)fixedp;
+  a.ep = (float)ep; a.lm = (float)lm;
+  const size_t bytes = dba_ba_layer_workspace_bytes(a.B, a.N, a.E, a.M, a.ht, a.wd, a.fixedp);
+  ws = torch::empty({(int64_t)bytes}, disps.options().dtype(torch::kUInt8));
+  a.workspace = ws.data_ptr(); a.workspace_bytes = bytes;
+  a.stream = cur_stream();
+  return a;
+}
+
+// -> [poses', disps', factor, dx, dz, flags]; check=True reads the status word (one host sync) and raises on an out-of-range ii / jj or
+// a source-frame count other than eta's M
+std::vector<torch::Tensor> ba_layer_forward(torch::Tensor target, torch::Tensor weight, torch::Tensor eta, torch::Tensor poses, torch::Tensor disps,
+                                            torch::Tensor intrinsics, torch::Tensor ii, torch::Tensor jj, int64_t fixedp, double ep, double lm,
+                                            bool check) {
+  const Expect expect("ba_layer_forward", disps, "disps");
+  c10::cuda::CUDAGuard guard(expect.dev);
+  torch::Tensor ws;
+  dba_ba_layer_args a = ba_layer_args("ba_layer_forward", expect, target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp, ep, lm, ws);
+  const int64_t n = 6 * (a.N - a.fixedp);
+  auto f64 = disps.options().dtype(F64);
+  auto poses_out = torch::empty_like(poses), disps_out = torch::empty_like(disps);
+  auto factor = torch::empty({a.B, n, n}, f64), dx = torch::empty({a.B, n}, f64), dz = torch::zeros({a.B, a.M, a.ht * a.wd}, f64);
+  auto flags = torch::empty({1 + a.B}, disps.options().dtype(torch::kInt32));
+  a.poses_out = poses_out.data_ptr<float>(); a.disps_out = disps_out.data_ptr<float>();
+  a.factor = factor.data_ptr<double>(); a.dx = dx.data_ptr<double>(); a.dz = dz.data_ptr<double>(); a.flags = flags.data_ptr<int>();
+  check_status(dba_ba_layer_forward(&a), "ba_layer_forward");
+  if (check) {
+    const int st = flags[0].item<int>();
+    TORCH_CHECK_INDEX(!(st & DBA_BA_LAYER_BAD_INDEX), "droid_backends.ba_layer_forward: ii / jj index a frame outside [0, ", a.N, ")");
+    TORCH_CHECK(!(st & DBA_BA_LAYER_BAD_M), "droid_backends.ba_layer_forward: eta has ", a.M, " depth frames, not the number of distinct ii");
+  }
+  return {poses_out, disps_out, factor, dx, dz, flags};
+}
+
+// -> [grad_target, grad_weight, grad_eta, grad_poses, grad_disps]
+std::vector<torch::Tensor> ba_layer_backward(torch::Tensor grad_poses, torch::Tensor grad_disps, torch::Tensor target, torch::Tensor weight,
+                                             torch::Tensor eta, torch::Tensor poses, torch::Tensor disps, torch::Tensor intrinsics, torch::Tensor ii,
+                                             torch::Tensor jj, int64_t fixedp, double ep, double lm, torch::Tensor factor, torch::Tensor dx,
+                                             torch::Tensor dz, torch::Tensor flags) {
+  const Expect expect("ba_layer_backward", disps, "disps");
+  c10::cuda::CUDAGuard guard(expect.dev);
+  torch::Tensor ws;
+  dba_ba_layer_args a = ba_layer_args("ba_layer_backward", expect, target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp, ep, lm, ws);
+  const int64_t n = 6 * (a.N - a.fixedp);
+  expect(grad_poses, "grad_poses", {F32}, dims({a.B, a.N, 7}));
+  expect(grad_disps, "grad_disps", {F32}, dims({a.B, a.N, a.ht, a.wd}));
+  expect(factor, "factor", {F64}, dims({a.B, n, n}));
+  expect(dx, "dx", {F64}, dims({a.B, n}));
+  expect(dz, "dz", {F64}, dims({a.B, a.M, a.ht * a.wd}));
+  expect(flags, "flags", {torch::kInt32}, dims({1 + a.B}));
+  auto g_target = torch::empty_like(target), g_weight = torch::empty_like(weight), g_eta = torch::empty_like(eta);
+  auto g_poses = torch::empty_like(poses), g_disps = torch::empty_like(disps);
+  a.factor = factor.data_ptr<double>(); a.dx = dx.data_ptr<double>(); a.dz = dz.data_ptr<double>(); a.flags = flags.data_ptr<int>();
+  a.grad_poses_out = grad_poses.data_ptr<float>(); a.grad_disps_out = grad_disps.data_ptr<float>();
+  a.grad_target = g_target.data_ptr<float>(); a.grad_weight = g_weight.data_ptr<float>(); a.grad_eta = g_eta.data_ptr<float>();
+  a.grad_poses = g_poses.data_ptr<float>(); a.grad_disps = g_disps.data_ptr<float>();
+  check_status(dba_ba_layer_backward(&a), "ba_layer_backward");
+  return {g_target, g_weight, g_eta, g_poses, g_disps};
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
   // bundle adjustment kernels
@@ -949,5 +1036,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lie_backward", &lie_backward, "gradients of lie_forward (lietorch's convention; broadcast operands reduced in the kernel) -> [grad_a(, "
         "grad_b)], None for a gradient not asked for, native extension", pybind11::arg("op"), pybind11::arg("group"), pybind11::arg("grad"),
         pybind11::arg("a"), pybind11::arg("b") = pybind11::none(), pybind11::arg("need_a") = true, pybind11::arg("need_b") = true);
+  m.def("ba_layer_forward", &ba_layer_forward, "the dense BA layer of DroidNet (reference geom/ba.py BA), forward -> [poses', disps', factor, "
+        "dx, dz, flags], native extension", pybind11::arg("target"), pybind11::arg("weight"), pybind11::arg("eta"), pybind11::arg("poses"),
+        pybind11::arg("disps"), pybind11::arg("intrinsics"), pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("fixedp") = 1,
+        pybind11::arg("ep") = 0.1, pybind11::arg("lm") = 1e-4, pybind11::arg("check") = true);
+  m.def("ba_layer_backward", &ba_layer_backward, "gradients of ba_layer_forward -> [grad_target, grad_weight, grad_eta, grad_poses, grad_disps], "
+        "native extension", pybind11::arg("grad_poses"), pybind11::arg("grad_disps"), pybind11::arg("target"), pybind11::arg("weight"),
+        pybind11::arg("eta"), pybind11::arg("poses"), pybind11::arg("disps"), pybind11::arg("intrinsics"), pybind11::arg("ii"),
+        pybind11::arg("jj"), pybind11::arg("fixedp"), pybind11::arg("ep"), pybind11::arg("lm"), pybind11::arg("factor"), pybind11::arg("dx"),
+        pybind11::arg("dz"), pybind11::arg("flags"));
   m.def("_b200_native", []() { return true; });
 }

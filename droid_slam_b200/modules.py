@@ -35,6 +35,8 @@ kernel for is offered as a hook:
     (`handover_round` -> `droid_backends.fragment_handover`, one host sync per round).
   * `droid_slam_b200.install_dependencies()` (the package's, recorded here too): `lietorch` / `torch_scatter` resolve to the package's own,
     in the spawned backend before its arguments are unpickled (`_unpickle_backend`).
+  * `ba_layer(...)` / `install_ba_layer_hook(droid_net)`: DroidNet's differentiable dense BA (geom/ba.py:31-106, `droid_net.BA`) forward
+    and backward on csrc/ba_layer.cu (`droid_backends.ba_layer_forward` / `ba_layer_backward`), so `train.py` trains through it.
 
 The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
 it.  If not, strict=True (the default) raises RuntimeError naming the replaced method and the reason; strict=False runs the reference's
@@ -53,7 +55,7 @@ from . import install
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
            "install_trajectory_filler_hook", "track", "install_motion_filter_hook", "hook_registry", "reinstall_hooks",
-           "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook"]
+           "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook", "ba_layer", "install_ba_layer_hook"]
 
 
 def _require(entry, why):
@@ -1018,3 +1020,87 @@ def install_async_hook(droid_async_module, strict=True):
         ref = ref.reference
     droid_async_module.backend_process = BackendProcess(droid_async_module.__name__, strict, ref)
     return droid_async_module
+
+
+# ---- the differentiable dense BA layer under DroidNet ----------------------------------------------------------------------------------
+
+BA_LAYER_MAX_POSES = 20       # pose unknowns (N - fixedp) the layer factors in one launch (include/droid_b200.h DBA_BA_LAYER_MAX_POSES)
+_BA_EP, _BA_LM = 0.1, 1e-4    # schur_solve's damping (geom/chol.py:46)
+
+
+class _BALayer(torch.autograd.Function):
+    """geom/ba.py BA on droid_backends.ba_layer_forward / ba_layer_backward.  The forward keeps the fp64 factor, dx, dz and the flags;
+    the backward recomputes the per-pixel terms.  intrinsics, ii and jj get no gradient."""
+
+    @staticmethod
+    def forward(ctx, target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp):
+        be = install()
+        out = be.ba_layer_forward(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp, _BA_EP, _BA_LM, False)
+        ctx.fixedp = fixedp
+        ctx.save_for_backward(target, weight, eta, poses, disps, intrinsics, ii, jj, *out[2:])
+        return out[0], out[1]
+
+    @staticmethod
+    def backward(ctx, grad_poses, grad_disps):
+        target, weight, eta, poses, disps, intrinsics, ii, jj, factor, dx, dz, flags = ctx.saved_tensors
+        gp = torch.zeros_like(poses) if grad_poses is None else grad_poses.contiguous()
+        gd = torch.zeros_like(disps) if grad_disps is None else grad_disps.contiguous()
+        g = install().ba_layer_backward(gp, gd, target, weight, eta, poses, disps, intrinsics, ii, jj, ctx.fixedp, _BA_EP, _BA_LM,
+                                        factor, dx, dz, flags)
+        return g[0], g[1], g[2], g[3], g[4], None, None, None, None
+
+
+def _ba_layer_unsupported(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp=1, rig=1):
+    """why the native layer cannot run this BA call, or None"""
+    if type(poses).__name__ != "SE3" or not hasattr(poses, "data") or poses.data.shape[-1:] != (7,):
+        return "poses must be SE3 (got %s)" % type(poses).__name__
+    if rig != 1:
+        return "rig = %r (only rig = 1)" % (rig,)
+    N = disps.shape[1] if torch.is_tensor(disps) and disps.dim() == 4 else 0
+    if not 0 <= fixedp < N:
+        return "fixedp = %r outside [0, N) = [0, %d)" % (fixedp, N)
+    named = (("target", target), ("weight", weight), ("eta", eta), ("poses", poses.data), ("disps", disps), ("intrinsics", intrinsics))
+    for name, t in named:
+        if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32):
+            return "%s must be a CUDA float32 tensor" % name
+    if intrinsics.requires_grad:
+        return "intrinsics requires grad (the layer gives it none)"
+    if N - fixedp > BA_LAYER_MAX_POSES:
+        return "%d pose unknowns, more than the %d one launch factors" % (N - fixedp, BA_LAYER_MAX_POSES)
+    return None
+
+
+def ba_layer(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp=1, rig=1):
+    """BA(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp=1, rig=1) of geom/ba.py:31-106 -> (poses', disps'), poses' of
+    the caller's SE3 class, differentiable in target, weight, eta, poses (every frame) and disps.  One autograd Function over the
+    native forward and backward; under no_grad (or with no input requiring grad) nothing is kept.  No host synchronisation."""
+    _require("BA", _ba_layer_unsupported(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp, rig))
+    dev = disps.device
+    ii = ii.to(device=dev, dtype=torch.long).contiguous()
+    jj = jj.to(device=dev, dtype=torch.long).contiguous()
+    args = (target.contiguous(), weight.contiguous(), eta.contiguous(), poses.data.contiguous(), disps.contiguous(), intrinsics.contiguous())
+    if torch.is_grad_enabled() and any(t.requires_grad for t in args):
+        p, d = _BALayer.apply(*args, ii, jj, int(fixedp))
+    else:
+        p, d = install().ba_layer_forward(*args, ii, jj, int(fixedp), _BA_EP, _BA_LM, False)[:2]
+    return type(poses)(p), d
+
+
+def install_ba_layer_hook(droid_net_module, strict=True):
+    """droid_net_module = the imported reference module `droid_net`.  Sets its global `BA` (droid_net.py:13, called twice per update
+    iteration in DroidNet.forward) to the native layer (`ba_layer`), forward and backward.  A call the layer cannot run (poses not SE3,
+    tensors not CUDA float32, rig != 1, fixedp outside [0, N), intrinsics requiring grad, more than BA_LAYER_MAX_POSES pose unknowns)
+    raises under strict=True and runs the reference's BA under strict=False."""
+    ref = getattr(droid_net_module, "_b200_reference_BA", None) or droid_net_module.BA
+
+    def BA(*args, **kwargs):
+        why = _ba_layer_unsupported(*args, **kwargs)
+        if why is not None and not strict:
+            return ref(*args, **kwargs)
+        _require("BA", why)
+        return ba_layer(*args, **kwargs)
+
+    droid_net_module._b200_reference_BA = ref
+    droid_net_module.BA = BA
+    _record("install_ba_layer_hook", droid_net_module, strict=strict)
+    return droid_net_module

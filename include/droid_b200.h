@@ -459,6 +459,38 @@ int dba_lie_forward(int op, int group, int dtype, const void* a, const int64_t* 
 int dba_lie_backward(int op, int group, int dtype, const void* grad, const void* a, const int64_t* a_strides, const void* b,
                      const int64_t* b_strides, void* grad_a, void* grad_b, int ndim, const int64_t* shape, dba_stream_t stream);
 
+/* ---- the differentiable dense BA layer (DroidNet's BA, reference geom/ba.py:31-106), forward and backward -------------------------
+ * fp32, contiguous: target / weight [B,E,ht,wd,2], eta [B,M,ht,wd] (M = the number of distinct source frames), poses [B,N,7] (SE3),
+ * disps [B,N,ht,wd], intrinsics [B,N,4] (per frame); ii / jj [E] int64.  Pose unknowns are frames fixedp .. N-1 (fixedp in [0, N),
+ * N - fixedp <= DBA_BA_LAYER_MAX_POSES: the reduced pose system is factored by one CTA in shared memory).  Damping ep, lm as in
+ * schur_solve (0.1, 1e-4).
+ * dba_ba_layer_forward writes poses_out / disps_out and keeps, for the backward, the fp64 Cholesky factor [B, n, n] (n = 6 (N - fixedp),
+ * lower triangle), dx [B, n] and dz [B, M, ht*wd] (zero-filled by the caller), and flags [1 + B] (device ints): flags[0] the status word
+ * (DBA_BA_LAYER_BAD_*: edges with an out-of-range ii / jj are skipped instead of read), flags[1 + b] batch element b's factor failed
+ * (any failure: dx = 0 for the whole batch).  dba_ba_layer_backward takes the upstream gradients grad_poses_out [B,N,7] (lietorch's
+ * left-tangent convention) and grad_disps_out [B,N,ht,wd] with the same inputs and kept tensors, and writes grad_target, grad_weight,
+ * grad_eta, grad_poses (all frames; 7th entry 0) and grad_disps, each shaped like its input.  The workspace is scratch for either call.
+ * Neither entry point synchronises the host; no floating-point atomics (bit-reproducible, batch elements independent). */
+#define DBA_BA_LAYER_MAX_POSES 20
+enum { DBA_BA_LAYER_BAD_INDEX = 1, DBA_BA_LAYER_BAD_M = 2 };
+typedef struct {
+  const float *target, *weight, *eta, *poses, *disps, *intrinsics;
+  const int64_t *ii, *jj;
+  int B, N, E, M, ht, wd, fixedp;
+  float ep, lm;
+  float *poses_out, *disps_out;                       /* forward outputs */
+  double *factor, *dx, *dz;                           /* written by the forward, read by the backward */
+  int* flags;                                         /* [1 + B] */
+  const float *grad_poses_out, *grad_disps_out;       /* backward inputs */
+  float *grad_target, *grad_weight, *grad_eta, *grad_poses, *grad_disps;
+  void* workspace;
+  size_t workspace_bytes;
+  dba_stream_t stream;
+} dba_ba_layer_args;
+size_t dba_ba_layer_workspace_bytes(int B, int N, int E, int M, int ht, int wd, int fixedp);
+int dba_ba_layer_forward(const dba_ba_layer_args* args);
+int dba_ba_layer_backward(const dba_ba_layer_args* args);
+
 #ifdef __cplusplus
 }
 #endif
