@@ -78,17 +78,9 @@ __device__ __forceinline__ Elem<SE3g, T> edge_gij(const float* __restrict__ pb, 
     G.t[0] = T(-0.1f); G.t[1] = G.t[2] = T(0); G.q[0] = G.q[1] = G.q[2] = T(0); G.q[3] = T(1);
     return G;
   }
-  T a[7], b[7];
-  for (int k = 0; k < 7; k++) { a[k] = T(pb[7 * j + k]); b[k] = T(pb[7 * i + k]); }
   Elem<SE3g, T> Pj, Pi;
-  Pj.load(a); Pi.load(b);
-  const Elem<SE3g, T> Ii = dba_lie::g_inv(Pi);
-  T r[3];
-  dba_lie::rot(Pj.q, Ii.t, r);
-  for (int k = 0; k < 3; k++) G.t[k] = Pj.t[k] + r[k];
-  dba_lie::qmul(Pj.q, Ii.q, G.q);
-  dba_lie::qnormalize(G.q);
-  return G;
+  Pj.load(pb + 7 * j); Pi.load(pb + 7 * i);
+  return dba_lie::g_mul(Pj, dba_lie::g_inv(Pi));
 }
 
 // one edge pixel's primal terms
@@ -413,14 +405,9 @@ __global__ void bal_pose_retr_kernel(const float* __restrict__ poses, double* __
       }
     }
     const Elem<SE3g, float> X = dba_lie::g_exp<SE3g, float>(xi);
-    Elem<SE3g, float> Y, Z;
+    Elem<SE3g, float> Y;
     Y.load(poses + ((int64_t)b * N + f) * 7);
-    float r[3];
-    dba_lie::rot(X.q, Y.t, r);
-    for (int k = 0; k < 3; k++) Z.t[k] = X.t[k] + r[k];
-    dba_lie::qmul(X.q, Y.q, Z.q);
-    dba_lie::qnormalize(Z.q);
-    Z.store(out + ((int64_t)b * N + f) * 7);
+    dba_lie::g_mul(X, Y).store(out + ((int64_t)b * N + f) * 7);
   }
 }
 

@@ -3,7 +3,7 @@
 // All four are HBM-streaming (4-16 B per pixel); one CTA computes the edge transform once into shared memory,
 // pixels are thread-strided so every global access is warp-coalesced, outputs are written once (no memset, and
 // no atomics in depth_filter: a thread owns its pixel and loops over the six neighbours).
-#include "common.cuh"
+#include "droid_se3.cuh"
 
 namespace dba {
 

@@ -61,14 +61,9 @@ template <class G, typename T, int OP> __device__ __forceinline__ void fwd_elem(
     } else if constexpr (OP == DBA_LIE_INV) {
       g_inv(X).store(out);
     } else if constexpr (OP == DBA_LIE_MUL) {
-      Elem<G, T> Y, Z;
+      Elem<G, T> Y;
       Y.load(pb);
-      T r[3];
-      rot(X.q, Y.t, r);
-      for (int k = 0; k < 3; k++) Z.t[k] = X.t[k] + r[k];
-      qmul(X.q, Y.q, Z.q);
-      qnormalize(Z.q);
-      Z.store(out);
+      g_mul(X, Y).store(out);
     } else if constexpr (OP == DBA_LIE_ADJ || OP == DBA_LIE_ADJT || OP == DBA_LIE_JINV) {
       T a[G::K], b[G::K];
       for (int k = 0; k < G::K; k++) a[k] = pb[k];

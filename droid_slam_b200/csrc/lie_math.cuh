@@ -1,5 +1,7 @@
-// lie_math.cuh -- the SO3 / SE3 arithmetic of the `lietorch` package, shared by lie.cu (the group ops and their gradients) and
-// ba_layer.cu (the dense BA layer's Gij, retraction and their gradients).  Templated on the scalar type; conventions in lie.cu's header.
+// lie_math.cuh -- the SO3 / SE3 arithmetic of lietorch's convention (quaternion normalised on load, small-angle branches at EPS = 1e-6;
+// details in lie.cu's header), for every kernel that computes in it: the group ops and their gradients (lie.cu), the dense BA layer
+// (ba_layer.cu), the trajectory filler's interpolation (filler.cu) and DroidAsync's hand-over (handover.cu).  Templated on the scalar
+// type.  The reference kernels' convention (no renormalisation, their own branch thresholds) is droid_se3.cuh's.
 #pragma once
 #include "common.cuh"
 
@@ -139,10 +141,11 @@ template <typename T> __device__ __forceinline__ void mtv3(const T* M, const T* 
 // ---- a group element, quaternion normalised on load ------------------------------------------------------------------------------------
 template <class G, typename T> struct Elem {
   T t[3], q[4];
-  __device__ __forceinline__ void load(const T* d) {
-    if constexpr (G::N == 7) { t[0] = d[0]; t[1] = d[1]; t[2] = d[2]; d += 3; }
+  // from data of any scalar type S (fp64 elements from fp32 poses), converted before the normalisation
+  template <typename S> __device__ __forceinline__ void load(const S* d) {
+    if constexpr (G::N == 7) { t[0] = T(d[0]); t[1] = T(d[1]); t[2] = T(d[2]); d += 3; }
     else { t[0] = t[1] = t[2] = T(0); }
-    q[0] = d[0]; q[1] = d[1]; q[2] = d[2]; q[3] = d[3];
+    q[0] = T(d[0]); q[1] = T(d[1]); q[2] = T(d[2]); q[3] = T(d[3]);
     qnormalize(q);
   }
   __device__ __forceinline__ void store(T* d) const {
@@ -158,6 +161,16 @@ template <class G, typename T> __device__ __forceinline__ Elem<G, T> g_inv(const
   rot(Y.q, X.t, r);
   Y.t[0] = -r[0]; Y.t[1] = -r[1]; Y.t[2] = -r[2];
   return Y;
+}
+// X Y = (R_X t_Y + t_X, q_X q_Y normalised)
+template <class G, typename T> __device__ __forceinline__ Elem<G, T> g_mul(const Elem<G, T>& X, const Elem<G, T>& Y) {
+  Elem<G, T> Z;
+  T r[3];
+  rot(X.q, Y.t, r);
+  for (int k = 0; k < 3; k++) Z.t[k] = X.t[k] + r[k];
+  qmul(X.q, Y.q, Z.q);
+  qnormalize(Z.q);
+  return Z;
 }
 // Adj(X) a: SE3 (R a_tau + t x R a_phi, R a_phi); SO3 R a
 template <class G, typename T> __device__ __forceinline__ void g_adj(const Elem<G, T>& X, const T* a, T* b) {
