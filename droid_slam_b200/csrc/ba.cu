@@ -12,8 +12,9 @@
 //     (the reference accumulates all 78+12 sums per pixel and does 90 serial block reductions);
 //   * reductions: fp32 per thread over its pixels -> warp shuffles -> fp64 across warps -> fp64 atomics into the
 //     dense reduced system Hsys [6P x 6P] / bsys [6P] (this is the buffer an edge-sharded multi-GPU run all-reduces);
-//   * the Schur complement S = sum_k E_k Q_k E_k^T is a per-frame SYRK over the (1+deg_k) rows of frame k with the
-//     6x6 block pairs register-tiled per thread (the reference enumerates (i,j,k) triples on the CPU, O(P^2 deg^2));
+//   * the Schur complement S = sum_k E_k Q_k E_k^T is a per-frame SYRK over the (1+deg_k) rows of frame k on the tensor cores, all
+//     frames in one launch of one CTA per SM, balanced by a work plan ba_prepare_kernel writes (the reference enumerates (i,j,k)
+//     triples on the CPU, O(P^2 deg^2));
 //   * solve: damping (diag += ep + lm*diag) and a tiled fp64 Cholesky on the device; a non-positive pivot gives
 //     dx = 0 like the reference's `solver.info() != Success` branch;
 //   * back-substitution dz = Q (w - E^T dx) keeps the reference quirk Q9 (rows whose pose index is <= 0 are skipped,
@@ -31,7 +32,7 @@ constexpr int kBuildThreads = 256;
 constexpr int kEdgeBatch = 16;     // edges whose transforms / partial sums live in shared memory at once
 
 struct Layout {
-  size_t off_hdr, off_frame2k, off_kx, off_rowptr, off_edgeidx, off_big, off_sys, off_L, off_dx, off_Eij, off_C, off_w, off_Ei, total;
+  size_t off_hdr, off_frame2k, off_kx, off_rowptr, off_edgeidx, off_plan, off_sys, off_L, off_dx, off_Eij, off_C, off_w, off_Ei, total;
   int P, n;
 };
 
@@ -53,7 +54,7 @@ __host__ inline Layout make_layout(int N, int E, int ht, int wd, int t0, int t1)
   L.off_kx = o;       o = align_up(o + (size_t)(N + 1) * sizeof(int), 256);
   L.off_rowptr = o;   o = align_up(o + (size_t)(N + 2) * sizeof(int), 256);
   L.off_edgeidx = o;  o = align_up(o + (size_t)(E + 1) * sizeof(int), 256);
-  L.off_big = o;      o = align_up(o + (size_t)(N + 1) * sizeof(int), 256);     // depth frames with more than 21 possible rows (pair-mode Schur)
+  L.off_plan = o;     o = align_up(o + 4 * (size_t)(N + 1) * sizeof(int), 256); // SchurPlan
   L.off_sys = o;      o = align_up(o + ((size_t)L.n * L.n + L.n) * sizeof(double), 256);
   L.off_L = o;        o = align_up(o + chol_workspace_bytes(L.n), 256);
   L.off_dx = o;       o = align_up(o + (size_t)(L.n + 6) * sizeof(float), 256);
@@ -67,10 +68,35 @@ __host__ inline Layout make_layout(int N, int E, int ht, int wd, int t0, int t1)
 }
 
 // header words
-enum { HDR_STATUS = 0, HDR_M = 1, HDR_CHOL_FAIL = 2, HDR_NBIG = 3 };
+enum { HDR_STATUS = 0, HDR_M = 1, HDR_CHOL_FAIL = 2, HDR_NBIG = 3, HDR_NPAIR = 4 };
 enum { ST_BAD_INDEX = 1, ST_ETA_ROWS = 2, ST_CHOL_FAIL = 4, ST_DEGREE = 8 };
 
-constexpr int kSchurMaxRows = 255;   // Schur rows per depth frame (out-degree + 1); larger frames raise ST_DEGREE
+// Schur routes by the rows of a depth frame (see the Schur section): packed tiles up to kPackedRowsMax rows, one tile up to kTcRowsMax,
+// pairs of kPairTileRows-row tiles up to kSchurMaxRows (out-degree + 1; larger frames raise ST_DEGREE)
+constexpr int kPackedRowsMax = 10;
+constexpr int kTcRowsMax = 21;
+constexpr int kPairTileRows = 10;        // 60 lines + the w line <= 64 operand rows
+constexpr int kSchurMaxRows = 255;
+
+// The Schur launch's work plan, written by ba_prepare_kernel (four arrays of N + 1 ints at Layout::off_plan):
+//   rows[m]   Schur rows of depth frame m: its own pose if it is in [t0, t1), plus one per out-edge whose target is; 0 without out-edges
+//   cost[m]   exclusive prefix sum over the frames of their packed / single-tile cost (schur_cost), cost[M] = the total
+//   big[i]    the depth frames above kTcRowsMax rows (pair route), ascending, i < hdr[HDR_NBIG]
+//   pairs[i]  exclusive prefix sum of their tile-pair counts; hdr[HDR_NPAIR] = the total
+struct SchurPlan { int *rows, *cost, *big, *pairs; };
+__host__ __device__ inline SchurPlan schur_plan(void* base, int N) {
+  int* p = reinterpret_cast<int*>(base);
+  return SchurPlan{p, p + (N + 1), p + 2 * (N + 1), p + 3 * (N + 1)};
+}
+// Cost of a frame's packed or single-tile Schur work in the units the launch balances: one per 64-pixel packed chunk (an M = N = 64
+// product per warpgroup), two per 32-pixel single-tile chunk (M = 64, N = 128: twice the MMA work).  0 on the pair route.
+__device__ __forceinline__ int schur_cost(int rows, int HW) {
+  return rows == 0 || rows > kTcRowsMax ? 0 : rows <= kPackedRowsMax ? (HW + 63) / 64 : 2 * ((HW + 31) / 32);
+}
+__device__ __forceinline__ int schur_pair_count(int rows) {
+  const int T = (min(rows, kSchurMaxRows) + kPairTileRows - 1) / kPairTileRows;
+  return T * (T - 1) / 2;
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // prepare: kx = sorted unique(ii U [t0,t1)), frame2k, CSR of edges by source frame (stable in edge order)
@@ -101,7 +127,7 @@ __device__ __forceinline__ int block_exclusive_scan(int count, int* s_scan, Valu
 
 __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restrict__ ii, const int64_t* __restrict__ jj, int E, int N,
                                                           int t0, int t1, int eta_rows, int motion_only, int* __restrict__ hdr,
-                                                          int* __restrict__ frame2k, int* __restrict__ kx, int* __restrict__ rowptr, int* __restrict__ big,
+                                                          int* __restrict__ frame2k, int* __restrict__ kx, int* __restrict__ rowptr, SchurPlan plan,
                                                           int HW, float* __restrict__ Eij, float* __restrict__ C, float* __restrict__ w,
                                                           float* __restrict__ Ei) {
   __shared__ int s_scan[1024];
@@ -150,11 +176,25 @@ __global__ void __launch_bounds__(1024) ba_prepare_kernel(const int64_t* __restr
   if (!motion_only)
     for (int m = tid; m < M; m += blockDim.x)
       if (rowptr[m + 1] - rowptr[m] > kSchurMaxRows - 1) atomicOr(&hdr[HDR_STATUS], ST_DEGREE);
-  // depth frames that can have more than kTcRowsMax (21) rows = out-degree + 1: the pair-mode Schur launch only visits these
-  // (ascending order; there are at most E / 21 of them, which is what sizes that launch's grid)
-  const int nbig = block_exclusive_scan(M, s_scan, [&](int m) { return rowptr[m + 1] - rowptr[m] + 1 > 21 ? 1 : 0; },
-                                        [&](int m, int flag, int idx) { if (flag) big[idx] = m; });
-  if (tid == 0) hdr[HDR_NBIG] = nbig;
+  // the Schur plan: rows per depth frame, the prefix sum of the packed / single-tile costs, the pair-route frames and their tile pairs
+  for (int m = tid; m < M; m += blockDim.x) plan.rows[m] = 0;
+  __syncthreads();
+  for (int e = tid; e < E; e += blockDim.x) {
+    const long long i = ii[e], j = jj[e];
+    if (i < 0 || i >= N || j < 0 || j >= N) continue;
+    if (j >= t0 && j < t1) atomicAdd(&plan.rows[frame2k[i]], 1);
+  }
+  __syncthreads();
+  for (int m = tid; m < M; m += blockDim.x)
+    plan.rows[m] = rowptr[m + 1] > rowptr[m] ? plan.rows[m] + (kx[m] >= t0 && kx[m] < t1 ? 1 : 0) : 0;
+  __syncthreads();
+  const int total = block_exclusive_scan(M, s_scan, [&](int m) { return schur_cost(plan.rows[m], HW); },
+                                         [&](int m, int, int before) { plan.cost[m] = before; });
+  const int nbig = block_exclusive_scan(M, s_scan, [&](int m) { return plan.rows[m] > kTcRowsMax ? 1 : 0; },
+                                        [&](int m, int flag, int idx) { if (flag) plan.big[idx] = m; });
+  const int npair = block_exclusive_scan(nbig, s_scan, [&](int i) { return schur_pair_count(plan.rows[plan.big[i]]); },
+                                         [&](int i, int, int before) { plan.pairs[i] = before; });
+  if (tid == 0) { plan.cost[M] = total; hdr[HDR_NBIG] = nbig; hdr[HDR_NPAIR] = npair; }
 }
 
 // stable placement of every edge inside its source frame's segment: rank = #earlier edges with the same source.
@@ -400,12 +440,14 @@ __global__ void __launch_bounds__(kBuildThreads, 2) ba_build_kernel(
 // Schur complement:  Hsys -= sum_k E_k Q_k E_k^T ,  bsys -= sum_k E_k Q_k w_k       (reference K9/K10 + schur_block)
 // rows of frame k: (pose k, Ei_k) if k is in [t0,t1), then (pose jj[e], Eij[e]) for the out-edges e of k; rows whose pose
 // is outside [t0,t1) are dropped (they contribute nothing, reference :1155,:1257).
-// The rows of a frame decide the kernel, for every image size (the workspace rows are padded to ba_pitch, i.e. 16-byte aligned):
-//   <= kTcRowsMax rows (every frame of a sliding-window graph)   ba_schur_tc_kernel<false>: tensor cores, packed or single tile
-//   kTcRowsMax+1 .. kSchurMaxRows rows (dense graphs, sharded)   ba_schur_tc_kernel<true>:  tensor cores, pairs of row tiles
-// Both flush once per tile (pair) with fp64 atomics into the LOWER triangle of the reduced system.
+// The rows of a frame decide its route, for every image size (the workspace rows are padded to ba_pitch, i.e. 16-byte aligned):
+//   <= kPackedRowsMax rows (every frame of a sliding-window graph)   packed: two 32-pixel halves per 64-pixel chunk
+//   <= kTcRowsMax rows                                               single: one row tile per 32-pixel chunk
+//   kTcRowsMax+1 .. kSchurMaxRows rows (dense graphs, sharded)       pair:   pairs of row tiles over the whole pixel range
+// All three run in one launch (ba_schur_tc_kernel) and flush once per pass with fp64 atomics into the LOWER triangle of the reduced
+// system.
 // ---------------------------------------------------------------------------------------------------------
-constexpr int kTcRowsMax = 21;
+enum SchurRoute { kPacked = 0, kSingle = 1, kPair = 2 };
 constexpr int kTcThreads = 256;
 // Q = 1/C of the eliminated depth block.  C <= 0 only for a pixel with eta = 0 and no weight on any edge; the reference divides
 // anyway (inf -> NaN system -> zero pose update and NaN depths at that pixel).  The Schur kernel and the back-substitution here
@@ -443,7 +485,7 @@ __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, i
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Schur complement on the tensor cores (frames with at most kTcRowsMax rows; PAIR mode below: up to kSchurMaxRows rows):
+// Schur complement on the tensor cores (packed and single routes; PAIR mode below: up to kSchurMaxRows rows):
 //   S = X X^T  with  X = [ E_r / sqrt(C) ; w / sqrt(C) ]  (6R + 1 rows x pixels),  so that S[:6R,:6R] = sum E q E^T and
 //   S[:6R, 6R] = sum E q w  -- one symmetric rank-K update per frame, K = pixels.
 // fp32 accuracy on the tf32 pipe by operand splitting (3xTF32): x = hi + lo with hi = tf32(x), lo = x - hi (exact), and
@@ -452,19 +494,17 @@ __device__ __forceinline__ void build_row_list(const int64_t* __restrict__ jj, i
 // The tensor core truncates every addend to the accumulator's exponent, so a long accumulation chain drifts (one accumulator over
 // the whole pixel range -> 1e-4 on the depths).  hi hi^T therefore gets a fresh register accumulator per chunk which is added into
 // an fp32 running sum when the next chunk's MMAs are issued; G is 2^-11 smaller and keeps one accumulator for the whole range.
-// CTA = (frame, pixel range), 256 threads = two warpgroups.  Every warp cp.asyncs its own raw rows of a chunk into a 4-deep
+// A pass = (frame, pixel range), 256 threads = two warpgroups.  Every warp cp.asyncs its own raw rows of a chunk into a 4-deep
 // warp-private raw ring and splits them into the two K-major SWIZZLE_128B operand tiles [128 rows x 32 px] of a 4-deep operand
-// ring (generic-proxy stores + fence.proxy.async); after a CTA barrier warpgroup w issues the chunk's wgmma.m64n128k8 for operand
-// rows 64 w .. 64 w + 63 against all 128 rows (both operands described from the SAME tile) and splits the next chunk while they
-// run.  Finally G goes through shared memory and the lower triangle is added into the reduced system with fp64 atomics.
-// Frames with 6R + 2 <= 64 (R <= 10) run "packed": the two halves of a 64-pixel chunk sit in operand rows 0..63 and 64..127,
-// one M = N = 128 product then yields both halves' products on the diagonal blocks (the MMA cost is set by the 128 operand rows
-// it streams whether they are live or not).
+// ring (generic-proxy stores + fence.proxy.async); after a CTA barrier warpgroup w issues the chunk's MMAs for operand rows
+// 64 w .. 64 w + 63 (both operands described from the SAME tile) and splits the next chunk while they run.  Finally G goes through
+// shared memory and the lower triangle is added into the reduced system with fp64 atomics.
+//   single, PAIR: wgmma.m64n128k8 against all 128 operand rows (PAIR: the rows of tile a and tile b).
+//   packed (6R + 2 <= 64, R <= kPackedRowsMax): the two 32-pixel halves of a 64-pixel chunk sit in operand rows 0..63 and 64..127 with
+//   the same lines, and warpgroup w needs only its own half's product: wgmma.m64n64k8 of rows 64 w .. 64 w + 63 against themselves.
 // The copies move whole 16-byte pieces, so the last piece of a row also carries the pad pixels [HW, pitch).  They are zero in E, w
 // and C, and rsqrt(C) is taken as 0 there, so they add nothing.
 // ---------------------------------------------------------------------------------------------------------
-constexpr int kPairTileRows = 10;               // pair mode: row tiles of 10 frame rows (60 lines + the w line <= 64 operand rows)
-constexpr int kPairGridZ = 45;                  // CTAs per frame in pair mode: the tile pairs of a 100-row frame (10 tiles)
 constexpr int kTcRawStages = 4;
 constexpr int kTcRawBytes = 128 * 128;          // up to 128 lines (6R rows, w, C; two halves when packed) x 128 bytes
 constexpr int kTcOpBytes = 128 * 128;           // one operand tile (hi or lo)
@@ -487,19 +527,21 @@ __device__ __forceinline__ void sts_f32(uint32_t addr, float v) { asm volatile("
 // PAIR mode the row tiles ta < tb, whose diagonal blocks S_aa / S_bb are added only where emit_a / emit_b.  A caller that runs
 // another pass must put a CTA barrier in between: the epilogue reads s_gidx and the operand ring, which the next pass rewrites.
 // lane and warp come from the caller, which in PAIR mode makes warp opaque per pass (see the pair loop).
-template <bool PAIR>
+template <int MODE>
 __device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nrows, int ta, int tb, bool emit_a, bool emit_b,
                                               int px_begin, int px_end, int pitch, int n, const float* __restrict__ Cin,
                                               const float* __restrict__ win, double* __restrict__ Hsys, double* __restrict__ bsys,
                                               const int* s_pose, const float* const* s_ptr, int* s_gidx) {
+  constexpr bool PAIR = MODE == kPair;
+  constexpr bool packed = MODE == kPacked;               // two PIXEL halves of a 64-pixel chunk in operand rows 0..63 / 64..127 (R6 + 2 <= 64)
+  constexpr int NC = packed ? 64 : 128;                  // columns of a warpgroup's products
   const int tid = threadIdx.x;
   extern __shared__ uint8_t tc_smem_raw[];
   const int R6a = PAIR ? 6 * min(kPairTileRows, nrows - kPairTileRows * ta) : 6 * nrows;
   const int R6b = PAIR ? 6 * min(kPairTileRows, nrows - kPairTileRows * tb) : 6 * nrows;
   const int R6 = R6a;                                    // operand rows 0..R6-1: E rows, row R6: w  (PAIR: of tile a, R6b of tile b)
-  const bool packed = !PAIR && (R6 + 2 <= 64);          // two PIXEL halves of a 64-pixel chunk in operand rows 0..63 / 64..127
-  const bool two_halves = PAIR || packed;                // operand rows 64..127 carry a second set of lines
-  const int nhalf = packed ? 2 : 1;
+  constexpr bool two_halves = PAIR || packed;                // operand rows 64..127 carry a second set of lines
+  constexpr int nhalf = packed ? 2 : 1;
   const int cpx = 32 * nhalf;                            // pixels per chunk
   const int nchunks = (px_end - px_begin + cpx - 1) / cpx;
 
@@ -581,9 +623,9 @@ __device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nro
   };
   float4 Cn0 = load_c4(0, 0), Cn1 = packed ? load_c4(0, 1) : make_float4(0.f, 0.f, 0.f, 0.f);
   const int wg = warp >> 2;
-  float acc[64], D[64], G[64];                              // running hi hi^T, this chunk's hi hi^T, hi lo^T (m64n128 fragments)
+  float acc[NC / 2], D[NC / 2], G[NC / 2];                  // running hi hi^T, this chunk's hi hi^T, hi lo^T (m64nNC fragments)
 #pragma unroll
-  for (int j = 0; j < 64; j++) acc[j] = 0.f;
+  for (int j = 0; j < NC / 2; j++) acc[j] = 0.f;
   // Operand stage c % 4 is rewritten at chunk c: the MMAs of chunk c - 4 that read it are complete, because each warpgroup waits
   // for its chunk c - 2 before issuing chunk c - 1, and both passed the CTA barrier of chunk c - 1.
   for (int c = 0; c < nchunks; c++) {
@@ -620,16 +662,23 @@ __device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nro
       wgmma_wait<0>();
       wgmma_fence_regs(D);
 #pragma unroll
-      for (int j = 0; j < 64; j++) acc[j] += D[j];
+      for (int j = 0; j < NC / 2; j++) acc[j] += D[j];
     }
     wgmma_fence();
     {
       const uint32_t hi0 = ophi, lo0 = ophi + kTcOpBytes;
+      const uint32_t b0 = packed ? wg * 64 * 128 : 0;                    // first operand row of the B side
 #pragma unroll
       for (int k = 0; k < 4; k++) {
         const uint64_t da = gmma_desc_sw128(hi0 + wg * 64 * 128 + k * 32, 16, 1024);
-        wgmma_tf32_n128(D, da, gmma_desc_sw128(hi0 + k * 32, 16, 1024), k > 0 ? 1 : 0);
-        wgmma_tf32_n128(G, da, gmma_desc_sw128(lo0 + k * 32, 16, 1024), (c > 0 || k > 0) ? 1 : 0);
+        const uint64_t dbh = gmma_desc_sw128(hi0 + b0 + k * 32, 16, 1024), dbl = gmma_desc_sw128(lo0 + b0 + k * 32, 16, 1024);
+        if constexpr (packed) {
+          wgmma_tf32_n64(D, da, dbh, k > 0 ? 1 : 0);
+          wgmma_tf32_n64(G, da, dbl, (c > 0 || k > 0) ? 1 : 0);
+        } else {
+          wgmma_tf32_n128(D, da, dbh, k > 0 ? 1 : 0);
+          wgmma_tf32_n128(G, da, dbl, (c > 0 || k > 0) ? 1 : 0);
+        }
       }
     }
     wgmma_commit();
@@ -640,13 +689,14 @@ __device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nro
   wgmma_fence_regs(D);
   wgmma_fence_regs(G);
 #pragma unroll
-  for (int j = 0; j < 64; j++) acc[j] += D[j];
+  for (int j = 0; j < NC / 2; j++) acc[j] += D[j];
 
   // ================= G = hi lo^T: through shared memory (the operand ring is idle now) so that G + G^T can be formed
   __syncthreads();                                         // both warpgroups' MMAs have completed: the ring may be overwritten
-  const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2), c_base = 2 * (lane & 3);
+  // staged as [operand row][local column]: G of operand rows (r, c) is at [r][c - cb0], cb0 the operand row of local column 0
+  const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2), c_base = 2 * (lane & 3), cb0 = packed ? wg * 64 : 0;
 #pragma unroll
-  for (int j = 0; j < 16; j++)
+  for (int j = 0; j < NC / 8; j++)
 #pragma unroll
     for (int e = 0; e < 4; e++)
       sts_f32(op_base + (uint32_t)((r_base + 8 * (e >> 1)) * kTcCxStride + 8 * j + c_base + (e & 1)) * 4, G[4 * j + e]);
@@ -656,29 +706,23 @@ __device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nro
 #pragma unroll
   for (int ih = 0; ih < 2; ih++) {
     const int row = r_base + 8 * ih;
-    const int lrow = packed ? (row & 63) : row;                       // line of this row
+    const int lrow = row - cb0;                                        // line of this row (packed), operand row otherwise
     const int gr = PAIR ? s_gidx[row] : ((lrow < R6) ? s_gidx[lrow] : -2);
     if (gr < 0) continue;
     const bool rb = row >= 64;
 #pragma unroll
-    for (int j = 0; j < 16; j++) {
+    for (int j = 0; j < NC / 8; j++) {
 #pragma unroll
       for (int e = 0; e < 2; e++) {
         const int col = 8 * j + c_base + e;
         const bool cbk = col >= 64;
-        int gc;
-        if (PAIR) {          // rows of tile a need S_aa (if this CTA emits it); rows of tile b need S_ba and S_bb (if emitted)
+        if (PAIR) {          // rows of tile a need S_aa (if this pass emits it); rows of tile b need S_ba and S_bb (if emitted)
           if (!rb && (cbk || !emit_a)) continue;
           if (rb && cbk && !emit_b) continue;
-          gc = s_gidx[col];
-        } else if (packed) {  // the diagonal block of this row's half
-          if (cbk != rb) continue;
-          gc = s_gidx[col & 63];
-        } else {
-          gc = s_gidx[col];
         }
+        const int gc = s_gidx[col];                                    // packed: local columns are the lines of this row's half
         if (gc == -2) continue;
-        const float g = lds_f32(op_base + (uint32_t)(row * kTcCxStride + col) * 4) + lds_f32(op_base + (uint32_t)(col * kTcCxStride + row) * 4);
+        const float g = lds_f32(op_base + (uint32_t)(row * kTcCxStride + col) * 4) + lds_f32(op_base + (uint32_t)((cb0 + col) * kTcCxStride + lrow) * 4);
         const double v = -(double)(acc[4 * j + 2 * ih + e] + g);
         if (PAIR && rb != cbk) {                                     // lower-left block S_ba: every unordered row pair appears once
           if (gc < 0) continue;                                      // the rhs comes from the diagonal blocks
@@ -695,26 +739,54 @@ __device__ __forceinline__ void schur_tc_pass(int lane, int warp, int m, int nro
   }
 }
 
+// The passes of one route (packed or single) over the frames m0.. whose chunks start in the cost interval [lo, hi).  Each frame part
+// gets its own row list and pass.
+template <int MODE>
+__device__ __forceinline__ void schur_sweep(int m0, int M, int lo, int hi, const SchurPlan& plan, const int64_t* __restrict__ jj,
+                                            int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
+                                            const int* __restrict__ edgeidx, int HW, int t0, int P, const float* __restrict__ Eij,
+                                            const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
+                                            double* __restrict__ Hsys, double* __restrict__ bsys, int* s_pose, const float** s_ptr,
+                                            int* s_nrows, int* s_wcount, int* s_gidx) {
+  constexpr int w = MODE == kPacked ? 1 : 2, cpx = 64 / w;        // cost and pixels of one chunk (schur_cost)
+  const int pitch = ba_pitch(HW);
+  for (int m = m0; m < M && plan.cost[m] < hi; m++) {
+    const int off = plan.cost[m], cost = plan.cost[m + 1] - off;
+    if (cost == 0 || (plan.rows[m] <= kPackedRowsMax) != (MODE == kPacked)) continue;
+    const int c_begin = lo > off ? (lo - off + w - 1) / w : 0;
+    const int c_end = min(cost / w, (hi - off + w - 1) / w);
+    if (c_begin >= c_end) continue;
+    const int e_begin = rowptr[m];
+    build_row_list(jj, hdr, edgeidx, e_begin, rowptr[m + 1] - e_begin, kx[m], m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, s_nrows, s_wcount);
+    const int nrows = *s_nrows;
+    if (nrows == 0 || nrows > (MODE == kPacked ? kPackedRowsMax : kTcRowsMax)) continue;
+    // lane and warp made opaque per pass: the copy slots and swizzled offsets derived from them are then computed inside the pass.
+    // Hoisted out of it, they would stay live across every pass and the kernel would spill.
+    int lane_p = threadIdx.x & 31, warp_p = threadIdx.x >> 5;
+    asm volatile("" : "+r"(lane_p), "+r"(warp_p));
+    schur_tc_pass<MODE>(lane_p, warp_p, m, nrows, 0, 0, true, true, c_begin * cpx, min(HW, c_end * cpx), pitch, 6 * P, Cin, win, Hsys, bsys,
+                        s_pose, s_ptr, s_gidx);
+    __syncthreads();                              // the next pass rewrites the row list, s_gidx and the operand ring
+  }
+}
+
 // PAIR mode (frames with 22..kSchurMaxRows rows: dense graphs, edge-sharded ranks): the rows are cut into T <= 26 tiles of 10, and a pass
 // stacks tile a in operand rows 0..63 and tile b in rows 64..127 over the SAME 32 pixels (the packed layout with a zero pixel offset
 // for the second half), so the one M = N = 128 product holds S_ba in its lower-left block and S_aa / S_bb on the diagonal (emitted
 // only by the designated pair (t, t+1)); G + G^T symmetrisation unchanged.  Off-diagonal-block entries go to (max, min) of the global
-// indices and count twice where two different rows share a pose.  CTA (frame, z) runs the tile pairs z, z + gridDim.z, ... of the
-// T (T - 1) / 2, each over the whole pixel range: one pair per CTA up to 100 rows (45 pairs), at most 8 at 255 rows (325 pairs).
-template <bool PAIR>
+// indices and count twice where two different rows share a pose.  A pass covers one tile pair over the whole pixel range.
+//
+// One persistent launch of one CTA per SM does every route (one CTA fits an SM: 255 registers x 256 threads, ~194 KB of shared
+// memory).  The plan of ba_prepare_kernel (SchurPlan) orders the packed and single-tile work as one cost line, frame after frame;
+// CTA b takes the chunks that START in [b T / grid, (b + 1) T / grid) of its total T, which may be parts of several frames, and runs
+// one pass per frame part.  The tile pairs of the pair-route frames are one flat list of items after that, taken round-robin.
+// The plan's row counts pick each frame's route; the row list a pass builds counts the same rows (fewer only for a frame with more
+// than kSchurMaxRows - 1 out-edges, which raises ST_DEGREE), and the single-tile pass takes any count up to kTcRowsMax.
 __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
     const int64_t* __restrict__ jj, int* __restrict__ hdr, const int* __restrict__ kx, const int* __restrict__ rowptr,
-    const int* __restrict__ edgeidx, int HW, int t0, int P, int px_per_cta,
-    const float* __restrict__ Eij, const float* __restrict__ Cin, const float* __restrict__ win, const float* __restrict__ Eiin,
-    double* __restrict__ Hsys, double* __restrict__ bsys, const int* __restrict__ big) {
-  if (PAIR && (int)blockIdx.y >= hdr[HDR_NBIG]) return;          // PAIR: blockIdx.y runs over the list of high-degree depth frames
-  const int m = PAIR ? big[blockIdx.y] : blockIdx.y;
-  if (m >= hdr[HDR_M]) return;
-  const int ix = kx[m];
-  const int e_begin = rowptr[m];
-  const int deg = rowptr[m + 1] - e_begin;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = 6 * P;
+    const int* __restrict__ edgeidx, int HW, int t0, int P, const float* __restrict__ Eij, const float* __restrict__ Cin,
+    const float* __restrict__ win, const float* __restrict__ Eiin, double* __restrict__ Hsys, double* __restrict__ bsys, SchurPlan plan) {
+  const int M = hdr[HDR_M];
   const int pitch = ba_pitch(HW);
 
   __shared__ int s_pose[kSchurMaxRows + 1];
@@ -723,37 +795,50 @@ __global__ void __launch_bounds__(kTcThreads, 1) ba_schur_tc_kernel(
   __shared__ int s_wcount[kTcThreads / 32];
   __shared__ int s_gidx[128];                     // operand row / column -> index in the reduced system (-1: rhs, -2: padding)
 
-  if (deg == 0) return;                           // no out-edge (e.g. a frame another rank owns): E_k = 0, nothing to subtract
-  if (PAIR) {                                     // cheap exits before the row-list build: at most deg + 1 rows
-    if (deg + 1 <= kTcRowsMax) return;
-    const int tmax = (min(deg + 1, kSchurMaxRows) + kPairTileRows - 1) / kPairTileRows;
-    if ((int)blockIdx.z >= tmax * (tmax - 1) / 2) return;
+  // ---- packed and single-tile routes: this CTA's interval [lo, hi) of the cost line, one sweep per route (a sweep that runs both
+  // routes' passes would spill)
+  const long long total = plan.cost[M];
+  const int lo = (int)((long long)blockIdx.x * total / gridDim.x), hi = (int)((long long)(blockIdx.x + 1) * total / gridDim.x);
+  if (lo < hi) {
+    int m0 = 0;                                   // the first frame whose cost interval ends after lo
+    for (int top = M - 1; m0 < top;) {
+      const int mid = (m0 + top) >> 1;
+      if (plan.cost[mid + 1] > lo) top = mid; else m0 = mid + 1;
+    }
+    schur_sweep<kPacked>(m0, M, lo, hi, plan, jj, hdr, kx, rowptr, edgeidx, HW, t0, P, Eij, Cin, win, Eiin, Hsys, bsys, s_pose, s_ptr,
+                         &s_nrows, s_wcount, s_gidx);
+    schur_sweep<kSingle>(m0, M, lo, hi, plan, jj, hdr, kx, rowptr, edgeidx, HW, t0, P, Eij, Cin, win, Eiin, Hsys, bsys, s_pose, s_ptr,
+                         &s_nrows, s_wcount, s_gidx);
   }
-  build_row_list(jj, hdr, edgeidx, e_begin, deg, ix, m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
-  const int nrows = s_nrows;
-  if (!PAIR && (nrows == 0 || nrows > kTcRowsMax)) return;            // larger frames belong to the pair-mode launch
-  if (PAIR && nrows <= kTcRowsMax) return;
-  const int px_begin = blockIdx.x * px_per_cta;
-  const int px_end = min(HW, px_begin + px_per_cta);
-  if (px_begin >= px_end) return;
-  if (!PAIR) {
-    schur_tc_pass<false>(lane, warp, m, nrows, 0, 0, true, true, px_begin, px_end, pitch, n, Cin, win, Hsys, bsys, s_pose, s_ptr, s_gidx);
-    return;
-  }
-  const int T = (nrows + kPairTileRows - 1) / kPairTileRows;         // 3 .. 26
-  for (int pr = blockIdx.z; pr < T * (T - 1) / 2; pr += gridDim.z) {
+
+  // ---- pair route: items (frame big[i], tile pair pr) numbered from plan.pairs[i]
+  const int nbig = hdr[HDR_NBIG], npair = hdr[HDR_NPAIR];
+  int listed = -1;                                // the frame whose rows are in s_pose / s_ptr
+  for (int item = blockIdx.x; item < npair; item += gridDim.x) {
+    int i = 0;                                    // the last big frame whose items start at or before this one
+    for (int top = nbig - 1; i < top;) {
+      const int mid = (i + top + 1) >> 1;
+      if (plan.pairs[mid] <= item) i = mid; else top = mid - 1;
+    }
+    const int m = plan.big[i], pr = item - plan.pairs[i];
+    if (m != listed) {
+      const int e_begin = rowptr[m];
+      build_row_list(jj, hdr, edgeidx, e_begin, rowptr[m + 1] - e_begin, kx[m], m, pitch, t0, P, Eij, Eiin, s_pose, s_ptr, &s_nrows, s_wcount);
+      listed = m;
+    }
+    const int nrows = s_nrows;
+    const int T = (nrows + kPairTileRows - 1) / kPairTileRows;         // 3 .. 26
+    if (nrows <= kTcRowsMax || pr >= T * (T - 1) / 2) continue;
     int tb = (int)((sqrtf(8.f * (float)pr + 1.f) + 1.f) * 0.5f);       // the two row tiles of this pass (ta < tb)
     while (tb * (tb - 1) / 2 > pr) tb--;
     while ((tb + 1) * tb / 2 <= pr) tb++;
     const int ta = pr - tb * (tb - 1) / 2;
-    // warp made opaque per pass: the copy slots and swizzled offsets derived from it are then computed inside the loop.  Hoisted out
-    // of it, they would stay live across every pass and the kernel would spill.
-    int warp_p = warp;
-    asm volatile("" : "+r"(warp_p));
+    int lane_p = threadIdx.x & 31, warp_p = threadIdx.x >> 5;
+    asm volatile("" : "+r"(lane_p), "+r"(warp_p));
     // S_tt of tile t < T-1 comes from pair (t, t+1), of tile T-1 from pair (T-2, T-1)
-    schur_tc_pass<true>(lane, warp_p, m, nrows, ta, tb, tb == ta + 1, tb == T - 1 && ta == T - 2, px_begin, px_end, pitch, n, Cin,
-                        win, Hsys, bsys, s_pose, s_ptr, s_gidx);
-    __syncthreads();                                     // the next pass rewrites s_gidx and the operand ring
+    schur_tc_pass<kPair>(lane_p, warp_p, m, nrows, ta, tb, tb == ta + 1, tb == T - 1 && ta == T - 2, 0, HW, pitch, 6 * P, Cin,
+                         win, Hsys, bsys, s_pose, s_ptr, s_gidx);
+    __syncthreads();                              // the next pass rewrites s_gidx and the operand ring
   }
 }
 
@@ -859,8 +944,8 @@ extern "C" int dba_ba_prepare(const dba_ba_args* a) {
   cudaStream_t st = (cudaStream_t)a->stream;
   ba_prepare_kernel<<<1, 1024, 0, st>>>(a->ii, a->jj, a->n_edges, a->n_frames, a->t0, a->t1, (a->motion_only || a->eta_by_frame) ? 1 : a->eta_rows,
                                         a->motion_only,
-                                        WS(int, L.off_hdr), WS(int, L.off_frame2k), WS(int, L.off_kx), WS(int, L.off_rowptr), WS(int, L.off_big),
-                                        a->ht * a->wd, WS(float, L.off_Eij), WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei));
+                                        WS(int, L.off_hdr), WS(int, L.off_frame2k), WS(int, L.off_kx), WS(int, L.off_rowptr),
+                                        schur_plan(WS(void, L.off_plan), a->n_frames), a->ht * a->wd, WS(float, L.off_Eij), WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei));
   DBA_CHECK_LAUNCH("ba_prepare");
   if (a->n_edges > 0) {
     ba_fill_csr_kernel<<<(a->n_edges + 7) / 8, 256, 0, st>>>(a->ii, a->jj, a->n_edges, a->n_frames, WS(int, L.off_frame2k),
@@ -897,26 +982,13 @@ extern "C" int dba_ba_build(const dba_ba_args* a) {
   if (!a->motion_only && L.P > 0) {
     static bool attr_set = false;
     if (!attr_set) {
-      DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc smem attr");
-      DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc pair smem attr");
+      DBA_CHECK_CUDA(cudaFuncSetAttribute(ba_schur_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem), "schur tc smem attr");
       attr_set = true;
     }
-    // one launch per routing-table entry (see the Schur section): frames with at most kTcRowsMax rows on the packed / single-tile
-    // kernel, more on the pair kernel.  Each exits on the other's frames.
-    const int tiles64 = (HW + 63) / 64;
-    const int chunks_tc = std::max(1, std::min(tiles64, (sms + eff_frames / 2) / eff_frames));     // one CTA per SM
-    const int px_per_cta_tc = ((tiles64 + chunks_tc - 1) / chunks_tc) * 64;
-    const int gx_tc = (HW + px_per_cta_tc - 1) / px_per_cta_tc;
-    ba_schur_tc_kernel<false><<<dim3(gx_tc, a->n_frames, 1), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, px_per_cta_tc, WS(float, L.off_Eij),
-                                                         WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
-    // pair mode: kPairGridZ CTAs per listed frame share its tile pairs, whole pixel range per CTA; CTAs beyond a frame's pair count
-    // and CTAs of frames with at most kTcRowsMax rows (targets outside the window) exit before any Schur work.
-    const int max_big = std::min(a->n_frames, a->n_edges / kTcRowsMax);     // a frame with 22+ rows has 21+ out-edges
-    if (max_big > 0)
-      ba_schur_tc_kernel<true><<<dim3(1, max_big, kPairGridZ), kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr),
-                                                         WS(int, L.off_edgeidx), HW, a->t0, L.P, ((HW + 31) / 32) * 32, WS(float, L.off_Eij),
-                                                         WS(float, L.off_C), WS(float, L.off_w), WS(float, L.off_Ei), Hsys, bsys, WS(int, L.off_big));
+    // one CTA per SM shares every route's work by the plan ba_prepare_kernel wrote (see ba_schur_tc_kernel)
+    ba_schur_tc_kernel<<<sms, kTcThreads, kTcSmem, st>>>(a->jj, WS(int, L.off_hdr), WS(int, L.off_kx), WS(int, L.off_rowptr), WS(int, L.off_edgeidx),
+                                                        HW, a->t0, L.P, WS(float, L.off_Eij), WS(float, L.off_C), WS(float, L.off_w),
+                                                        WS(float, L.off_Ei), Hsys, bsys, schur_plan(WS(void, L.off_plan), a->n_frames));
     DBA_CHECK_LAUNCH("ba_schur");
   }
   return DBA_OK;
