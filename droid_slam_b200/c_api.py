@@ -17,6 +17,7 @@ SYMBOLS = [
     "dba_encoder_forward_frames", "dba_encoder_workspace_layout", "dba_encoder_forward_prefix", "dba_proximity_workspace_bytes", "dba_proximity_edges",
     "dba_fill_interpolate", "dba_pose_only_ba", "dba_fragment_handover", "dba_lie_record_sizes", "dba_lie_forward", "dba_lie_backward",
     "dba_ba_layer_workspace_bytes", "dba_ba_layer_forward", "dba_ba_layer_backward",
+    "dba_corr_volume_pyramid_f32", "dba_corr_grad_accumulate", "dba_corr_adjoint_workspace_bytes", "dba_corr_adjoint",
 ]
 
 DBA_F32, DBA_F16, DBA_F64, DBA_BF16 = 0, 1, 2, 3
@@ -65,6 +66,11 @@ def load():
     L.dba_corr_volume_supported.argtypes = [ci] * 5
     L.dba_corr_volume_workspace_bytes.restype = ctypes.c_size_t
     L.dba_corr_volume_workspace_bytes.argtypes = [ci] * 5
+    L.dba_corr_volume_pyramid_f32.argtypes = [vp] * 6 + [ci] * 4 + [vp]
+    L.dba_corr_grad_accumulate.argtypes = [vp] * 3 + [ci] * 3 + [vp]
+    L.dba_corr_adjoint_workspace_bytes.restype = ctypes.c_size_t
+    L.dba_corr_adjoint_workspace_bytes.argtypes = [ci] * 4
+    L.dba_corr_adjoint.argtypes = [vp] * 5 + [ci] * 4 + [vp, ctypes.c_size_t, vp]
     L.dba_altcorr_forward.argtypes = [vp, vp, vp, vp, vp, vp] + [ci] * 11 + [vp]
     L.dba_altcorr_backward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp] + [ci] * 11 + [vp]
     L.dba_altcorr_pyramid.argtypes = [vp] * 5 + [ci] * 7 + [vp]

@@ -373,19 +373,71 @@ std::vector<torch::Tensor> corr_volume_pyramid(torch::Tensor fmap1, torch::Tenso
 }
 
 // CorrBlock.__call__ (reference modules/corr.py:40-50) in one launch.  pyramid = 4 f16 tensors [E,h1,w1,h1/2^l,w1/2^l] (reference
-// layout, or levels 0-1 tiled when `tiled`), coords [E,2,h1,w1] f32 at level-0 scale -> [E,196,h1,w1] = cat over levels of corr_index_forward
+// layout, or levels 0-1 tiled when `tiled`) or 4 f32 tensors in the reference layout, coords [E,2,h1,w1] f32 at level-0 scale -> [E,196,h1,w1] = cat over levels of corr_index_forward
 torch::Tensor corr_lookup_pyramid(std::vector<torch::Tensor> pyramid, torch::Tensor coords, bool tiled) {
   TORCH_CHECK(pyramid.size() == 4, "droid_backends.corr_lookup_pyramid: 4 pyramid levels expected, got ", pyramid.size());
   const Expect expect("corr_lookup_pyramid", pyramid[0], "pyramid[0]");
-  expect(pyramid[0], "pyramid[0]", F16, dims({kAny, kAny, kAny, kAny, kAny}));
+  expect(pyramid[0], "pyramid[0]", {F16, F32}, dims({kAny, kAny, kAny, kAny, kAny}));
+  const torch::ScalarType vt = pyramid[0].scalar_type();
   const int n = (int)pyramid[0].size(0), h1 = (int)pyramid[0].size(1), w1 = (int)pyramid[0].size(2);
-  for (int l = 0; l < 4; l++) expect(pyramid[l], item("pyramid", l).c_str(), F16, dims({n, h1, w1, h1 >> l, w1 >> l}));
+  for (int l = 0; l < 4; l++) expect(pyramid[l], item("pyramid", l).c_str(), vt, dims({n, h1, w1, h1 >> l, w1 >> l}));
   expect(coords, "coords", F32, dims({n, 2, h1, w1}));
   c10::cuda::CUDAGuard guard(expect.dev);
   auto out = torch::empty({n, 196, h1, w1}, pyramid[0].options());
   check_status(dba_corr_lookup_pyramid(pyramid[0].data_ptr(), pyramid[1].data_ptr(), pyramid[2].data_ptr(), pyramid[3].data_ptr(), coords.data_ptr<float>(), out.data_ptr(),
-                                       n, h1, w1, tiled ? 3 : 0, DBA_F16, cur_stream()), "corr_lookup_pyramid");
+                                       n, h1, w1, tiled ? 3 : 0, dtype_code(pyramid[0], "corr_lookup_pyramid"), cur_stream()), "corr_lookup_pyramid");
   return out;
+}
+
+// The training CorrBlock (include/droid_b200.h): fmap1, fmap2 [E,128,ht,wd] f32 -> 4 f32 pyramid levels [E,ht,wd,ht>>l,wd>>l]
+std::vector<torch::Tensor> corr_volume_pyramid_f32(torch::Tensor fmap1, torch::Tensor fmap2) {
+  const Expect expect("corr_volume_pyramid_f32", fmap1, "fmap1");
+  expect(fmap1, "fmap1", F32, dims({kAny, kAny, kAny, kAny}));
+  const int E = (int)fmap1.size(0), C = (int)fmap1.size(1), ht = (int)fmap1.size(2), wd = (int)fmap1.size(3);
+  expect(fmap2, "fmap2", F32, dims({E, C, ht, wd}));
+  c10::cuda::CUDAGuard guard(expect.dev);
+  std::vector<torch::Tensor> out;
+  for (int l = 0; l < 4; l++) out.push_back(torch::empty({E, ht, wd, ht >> l, wd >> l}, fmap1.options()));
+  check_status(dba_corr_volume_pyramid_f32(fmap1.data_ptr<float>(), fmap2.data_ptr<float>(), out[0].data_ptr<float>(), out[1].data_ptr<float>(),
+                                           out[2].data_ptr<float>(), out[3].data_ptr<float>(), E, C, ht, wd, cur_stream()),
+               "corr_volume_pyramid_f32");
+  return out;
+}
+
+static int64_t grad_pyramid_row(int64_t ht, int64_t wd) {
+  int64_t q = 0;
+  for (int l = 0; l < 4; l++) q += (ht >> l) * (wd >> l);
+  return q;
+}
+
+// gpyr [E,ht*wd,Q] f32 += the gradient of one corr_lookup_pyramid call: grad [E,196,ht,wd] f32 at coords [E,2,ht,wd]
+void corr_grad_accumulate(torch::Tensor coords, torch::Tensor grad, torch::Tensor gpyr) {
+  const Expect expect("corr_grad_accumulate", coords, "coords");
+  expect(coords, "coords", F32, dims({kAny, 2, kAny, kAny}));
+  const int E = (int)coords.size(0), ht = (int)coords.size(2), wd = (int)coords.size(3);
+  expect(grad, "grad", F32, dims({E, 196, ht, wd}));
+  expect(gpyr, "gpyr", F32, dims({E, (int64_t)ht * wd, grad_pyramid_row(ht, wd)}));
+  c10::cuda::CUDAGuard guard(expect.dev);
+  check_status(dba_corr_grad_accumulate(coords.data_ptr<float>(), grad.data_ptr<float>(), gpyr.data_ptr<float>(), E, ht, wd, cur_stream()),
+               "corr_grad_accumulate");
+}
+
+// (grad_fmap1, grad_fmap2) [E,128,ht,wd] of the training CorrBlock from its accumulated gradient pyramid gpyr [E,ht*wd,Q]
+std::vector<torch::Tensor> corr_adjoint(torch::Tensor fmap1, torch::Tensor fmap2, torch::Tensor gpyr) {
+  const Expect expect("corr_adjoint", fmap1, "fmap1");
+  expect(fmap1, "fmap1", F32, dims({kAny, kAny, kAny, kAny}));
+  const int E = (int)fmap1.size(0), C = (int)fmap1.size(1), ht = (int)fmap1.size(2), wd = (int)fmap1.size(3);
+  expect(fmap2, "fmap2", F32, dims({E, C, ht, wd}));
+  expect(gpyr, "gpyr", F32, dims({E, (int64_t)ht * wd, grad_pyramid_row(ht, wd)}));
+  c10::cuda::CUDAGuard guard(expect.dev);
+  auto g1 = torch::empty_like(fmap1), g2 = torch::empty_like(fmap2);
+  const size_t ws_bytes = dba_corr_adjoint_workspace_bytes(E, C, ht, wd);
+  torch::Tensor ws;
+  void* ws_p = ws_bytes > 0 ? workspace(ws_bytes, expect.dev, ws) : nullptr;
+  check_status(dba_corr_adjoint(fmap1.data_ptr<float>(), fmap2.data_ptr<float>(), gpyr.data_ptr<float>(), g1.data_ptr<float>(), g2.data_ptr<float>(),
+                                E, C, ht, wd, ws_p, ws_bytes, cur_stream()),
+               "corr_adjoint");
+  return {g1, g2};
 }
 
 // AltCorrBlock.__init__ (reference modules/corr.py:90-101) as one launch.  fmaps [B,N,C,H,W] f16/f32 -> num_levels tensors
@@ -989,6 +1041,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("corr_index_backward", &corr_index_backward, "INDEX backward");
   m.def("corr_volume_pyramid", &corr_volume_pyramid, "all-pairs correlation + 4-level pyramid (wgmma), native extension", pybind11::arg("fmap1"), pybind11::arg("fmap2"),
         pybind11::arg("ii"), pybind11::arg("jj"), pybind11::arg("tiled") = false);
+  m.def("corr_volume_pyramid_f32", &corr_volume_pyramid_f32, "training CorrBlock: fp32 correlation volume + 4-level pyramid, native extension",
+        pybind11::arg("fmap1"), pybind11::arg("fmap2"));
+  m.def("corr_grad_accumulate", &corr_grad_accumulate, "training CorrBlock: add one lookup's gradient into the gradient pyramid, native extension",
+        pybind11::arg("coords"), pybind11::arg("grad"), pybind11::arg("gpyr"));
+  m.def("corr_adjoint", &corr_adjoint, "training CorrBlock: feature-map gradients from the gradient pyramid, native extension",
+        pybind11::arg("fmap1"), pybind11::arg("fmap2"), pybind11::arg("gpyr"));
   m.def("corr_lookup_pyramid", &corr_lookup_pyramid, "4-level radius-3 lookup in one launch -> [E,196,H,W], native extension", pybind11::arg("pyramid"), pybind11::arg("coords"),
         pybind11::arg("tiled") = false);
   m.def("altcorr_pyramid", &altcorr_pyramid, "AltCorrBlock pyramid in one launch -> levels [B,N,H>>l,W>>l,C] (private channels-last layout), native extension",

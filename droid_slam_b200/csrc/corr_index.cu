@@ -154,16 +154,9 @@ __global__ void __launch_bounds__(128, L1 ? 1 : 0) corr_lookup_pyramid_f16_kerne
   corr_pixel_f16_r3<(TILED_MASK & 1) != 0, __half, L1>(v0 + (size_t)p * h1 * w1, o, (size_t)hw1, x0, y0, h1, w1);
 }
 
-__global__ void __launch_bounds__(128) corr_index_fwd_f32_r3_kernel(const float* __restrict__ vol, const float* __restrict__ coords,
-                                                                    float* __restrict__ out, long long total, int hw1, int h2, int w2) {
-  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= total) return;
-  const int n = (int)(p / hw1);
-  const int pin = (int)(p - (long long)n * hw1);
-  const float x0 = coords[((size_t)n * 2 + 0) * hw1 + pin];
-  const float y0 = coords[((size_t)n * 2 + 1) * hw1 + pin];
-  const float* plane = vol + (size_t)p * h2 * w2;
-  float* out_px = out + (size_t)n * 49 * hw1 + pin;
+// one pixel, one level, f32, radius 3, w2 % 4 == 0 and a 16-byte aligned plane: the 8x8 tap window from 16-byte chunks
+__device__ __forceinline__ void corr_pixel_f32_r3(const float* __restrict__ plane, float* __restrict__ out_px, size_t hw1, float x0, float y0,
+                                                  int h2, int w2) {
   if (!(isfinite(x0) && isfinite(y0))) {
     corr_pixel_generic<float>(plane, out_px, (size_t)hw1, x0, y0, h2, w2, 3);
     return;
@@ -211,6 +204,39 @@ __global__ void __launch_bounds__(128) corr_index_fwd_f32_r3_kernel(const float*
     }
 #pragma unroll
     for (int i = 0; i < 8; i++) prev[i] = cur[i];
+  }
+}
+
+__global__ void __launch_bounds__(128) corr_index_fwd_f32_r3_kernel(const float* __restrict__ vol, const float* __restrict__ coords,
+                                                                    float* __restrict__ out, long long total, int hw1, int h2, int w2) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= total) return;
+  const int n = (int)(p / hw1);
+  const int pin = (int)(p - (long long)n * hw1);
+  corr_pixel_f32_r3(vol + (size_t)p * h2 * w2, out + (size_t)n * 49 * hw1 + pin, (size_t)hw1, coords[((size_t)n * 2 + 0) * hw1 + pin],
+                    coords[((size_t)n * 2 + 1) * hw1 + pin], h2, w2);
+}
+
+// the fused 4-level lookup on f32 volumes in the reference layout: per level the path corr_index_forward takes for that plane (the
+// chunked one where level rows are whole 16-byte chunks, else the generic one), so the result is that of 4 x corr_index_forward + cat
+__global__ void __launch_bounds__(128) corr_lookup_pyramid_f32_kernel(const float* __restrict__ v0, const float* __restrict__ v1,
+                                                                      const float* __restrict__ v2, const float* __restrict__ v3,
+                                                                      const float* __restrict__ coords, float* __restrict__ out,
+                                                                      long long total, int hw1, int h1, int w1) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= total) return;
+  const int n = (int)(p / hw1);
+  const int pin = (int)(p - (long long)n * hw1);
+  const float x0 = coords[((size_t)n * 2 + 0) * hw1 + pin];
+  const float y0 = coords[((size_t)n * 2 + 1) * hw1 + pin];
+#pragma unroll 1
+  for (int l = 3; l >= 0; l--) {
+    const int h2 = h1 >> l, w2 = w1 >> l;
+    const float s = 1.0f / (float)(1 << l);
+    const float* plane = (l == 0 ? v0 : l == 1 ? v1 : l == 2 ? v2 : v3) + (size_t)p * h2 * w2;
+    float* o = out + ((size_t)n * 196 + 49 * l) * hw1 + pin;
+    if (w2 % 4 == 0) corr_pixel_f32_r3(plane, o, (size_t)hw1, x0 * s, y0 * s, h2, w2);
+    else corr_pixel_generic<float>(plane, o, (size_t)hw1, x0 * s, y0 * s, h2, w2, 3);
   }
 }
 
@@ -298,17 +324,18 @@ extern "C" int dba_corr_index_backward(const float* coords, const void* corr_gra
   }
 }
 
-// fused 4-level lookup (f16, radius 3): out [n,196,h1,w1] = cat over levels of corr_index_forward(volume_l, coords / 2^l).
+// fused 4-level lookup (f16 or f32, radius 3): out [n,196,h1,w1] = cat over levels of corr_index_forward(volume_l, coords / 2^l).
 // tiled_mask bit l: level l is in the 4x8-tile layout of dba_corr_volume_pyramid(..., tiled = 1) (levels 0 and 1 there).
 // w1 % 64 == 0 and h1 % 8 == 0 (every level's rows are whole 16-byte chunks): corr_lookup_pyramid_f16_kernel; any other h1, w1 >= 8
-// (reference layout only): corr_lookup_pyramid_rows_f16_kernel.
+// (reference layout only): corr_lookup_pyramid_rows_f16_kernel.  f32 (reference layout): corr_lookup_pyramid_f32_kernel.
 extern "C" int dba_corr_lookup_pyramid(const void* v0, const void* v1, const void* v2, const void* v3, const float* coords, void* out,
                                        int n, int h1, int w1, int tiled_mask, int dtype, dba_stream_t stream) {
   DBA_CHECK_ARG(n >= 0 && h1 > 0 && w1 > 0, "bad extents");
-  DBA_CHECK_ARG(dtype == DBA_F16, "corr_lookup_pyramid: f16 volumes (the live system's autocast dtype) only; use corr_index_forward per level otherwise");
+  DBA_CHECK_ARG(dtype == DBA_F16 || dtype == DBA_F32, "corr_lookup_pyramid: f16 or f32 volumes only; use corr_index_forward per level otherwise");
   DBA_CHECK_ARG(h1 >= 8 && w1 >= 8, "corr_lookup_pyramid: h1 and w1 must be at least 8 (level 3 must have at least one pixel)");
   const bool chunk_rows = h1 % 8 == 0 && w1 % 64 == 0;
   DBA_CHECK_ARG(tiled_mask == 0 || (tiled_mask == 3 && chunk_rows), "tiled_mask must be 0, or 3 (levels 0 and 1 tiled) with w1 % 64 == 0 and h1 % 8 == 0");
+  DBA_CHECK_ARG(dtype == DBA_F16 || tiled_mask == 0, "corr_lookup_pyramid: f32 volumes are in the reference layout (tiled_mask 0)");
   const long long total = (long long)n * h1 * w1;
   if (total == 0) return DBA_OK;
   DBA_CHECK_ARG(v0 && v1 && v2 && v3 && coords && out, "null pointer");
@@ -316,6 +343,11 @@ extern "C" int dba_corr_lookup_pyramid(const void* v0, const void* v1, const voi
   DBA_CHECK_ARG((total + 127) / 128 < 0x7fffffffLL, "too many pixels for one launch");
   const unsigned blocks = (unsigned)((total + 127) / 128);
   cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == DBA_F32) {
+    corr_lookup_pyramid_f32_kernel<<<blocks, 128, 0, st>>>((const float*)v0, (const float*)v1, (const float*)v2, (const float*)v3, coords, (float*)out, total, h1 * w1, h1, w1);
+    DBA_CHECK_LAUNCH("corr_lookup_pyramid(f32)");
+    return DBA_OK;
+  }
   if (!chunk_rows)
     return corr_lookup_pyramid_rows_launch((const __half*)v0, (const __half*)v1, (const __half*)v2, (const __half*)v3, coords, (__half*)out, total, h1, w1, st);
   if (tiled_mask == 3)

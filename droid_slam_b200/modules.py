@@ -35,6 +35,8 @@ kernel for is offered as a hook:
     (`handover_round` -> `droid_backends.fragment_handover`, one host sync per round).
   * `droid_slam_b200.install_dependencies()` (the package's, recorded here too): `lietorch` / `torch_scatter` resolve to the package's own,
     in the spawned backend before its arguments are unpickled (`_unpickle_backend`).
+  * `install_corr_training_hook(droid_net)`: DroidNet's CorrBlock (modules/corr.py:6-71, `droid_net.CorrBlock`) on fp32 feature maps,
+    forward and backward, on csrc/corr_train.cu, so `train.py`'s loss reaches fnet through native kernels.
   * `ba_layer(...)` / `install_ba_layer_hook(droid_net)`: DroidNet's differentiable dense BA (geom/ba.py:31-106, `droid_net.BA`) forward
     and backward on csrc/ba_layer.cu (`droid_backends.ba_layer_forward` / `ba_layer_backward`), so `train.py` trains through it.
 
@@ -55,7 +57,8 @@ from . import install
 __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder_hook", "reproject", "upsample", "add_proximity_factors", "install_proximity_hook",
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
            "install_trajectory_filler_hook", "track", "install_motion_filter_hook", "hook_registry", "reinstall_hooks",
-           "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook", "ba_layer", "install_ba_layer_hook"]
+           "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook", "ba_layer", "install_ba_layer_hook",
+           "install_corr_training_hook"]
 
 
 def _require(entry, why):
@@ -134,6 +137,12 @@ def _lookup(be, pyramid, tiled, coords_t):
     return be.corr_lookup_pyramid([v.contiguous() for v in pyramid], coords_t, tiled).view(1, n, -1, ht, wd)
 
 
+def _no_grad_inputs(who, *ts):
+    """raise for a forward-only native `who` when one of ts is a tensor that requires grad under grad mode (its gradient would be dropped)"""
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts):
+        raise RuntimeError("the native %s is forward only: an input requires grad" % who)
+
+
 def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
     """why corr_volume_pyramid has no kernel for these CorrBlock arguments (None: it has one)"""
     if fmap1.dim() != 5 or fmap2.shape != fmap1.shape:
@@ -160,7 +169,8 @@ def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
     fused_lookup: additionally replace `CorrBlock.__call__` by the one-launch 4-level lookup `corr_lookup_pyramid`.  Where
     corr_volume_pyramid has a tiled builder (wd = 64, ht % 8 == 0) the volumes of levels 0 and 1 are kept in the tiled private layout
     (64-byte DRAM atoms, about a third less HBM traffic per lookup); elsewhere the reference layout.  Same tensor shapes, `cat` /
-    `__getitem__` over edges keep working, results bit-identical to the reference-layout path."""
+    `__getitem__` over edges keep working, results bit-identical to the reference-layout path.  Forward only: feature maps that require grad
+    under grad mode raise, whichever constructor would run (install_corr_training_hook is the differentiable block)."""
     be = install()
     cls = corr_module.CorrBlock
     ref_call = cls.__call__
@@ -180,8 +190,11 @@ def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
         return _lookup(be, self.corr_pyramid, self._b200_tiled, c).view(batch, num, -1, ht, wd)
 
     cls._b200_tiled = None                      # a block's volume layout (True: tiled); None where the reference's constructor ran
-    _replace(cls, "__init__", __init__, lambda blk, fmap1, fmap2, num_levels=4, radius=3: _corr_volume_unsupported(be, fmap1, fmap2, num_levels),
-             strict)
+    def unsupported(blk, fmap1, fmap2, num_levels=4, radius=3):
+        _no_grad_inputs("CorrBlock", fmap1, fmap2)   # an input check, ahead of the policy
+        return _corr_volume_unsupported(be, fmap1, fmap2, num_levels)
+
+    _replace(cls, "__init__", __init__, unsupported, strict)
     if fused_lookup:
         cls.__call__ = __call__
     _record("install_corr_volume_hook", corr_module, strict=strict, fused_lookup=fused_lookup)
@@ -219,22 +232,18 @@ def install_alt_corr_hook(corr_module, strict=True):
     cls = corr_module.AltCorrBlock
     ref_call = cls.__call__
 
-    def _no_grad_inputs(*ts):
-        if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts):
-            raise RuntimeError("the native AltCorrBlock is forward only: an input requires grad")
-
     def __init__(self, fmaps, num_levels=4, radius=3):
         self.num_levels, self.radius = num_levels, radius
         self._b200_pyramid = be.altcorr_pyramid(fmaps.contiguous(), num_levels)
 
     def unsupported(self, fmaps, num_levels=4, radius=3):
-        _no_grad_inputs(fmaps)                   # an input check, ahead of the policy
+        _no_grad_inputs("AltCorrBlock", fmaps)   # an input check, ahead of the policy
         return _alt_unsupported(fmaps, num_levels, radius)
 
     def __call__(self, coords, ii, jj):
         if self._b200_pyramid is None:
             return ref_call(self, coords, ii, jj)
-        _no_grad_inputs(coords)
+        _no_grad_inputs("AltCorrBlock", coords)
         if not (coords.is_cuda and coords.dtype == torch.float32 and coords.dim() == 5 and coords.shape[-1] == 2):
             raise RuntimeError("AltCorrBlock: coords must be a float32 CUDA tensor [B,M,H,W,2], got %s %s on %s"
                                % (tuple(coords.shape), coords.dtype, coords.device))
@@ -1103,4 +1112,131 @@ def install_ba_layer_hook(droid_net_module, strict=True):
     droid_net_module._b200_reference_BA = ref
     droid_net_module.BA = BA
     _record("install_ba_layer_hook", droid_net_module, strict=strict)
+    return droid_net_module
+
+
+# ---- the differentiable CorrBlock under DroidNet -----------------------------------------------------------------------------------
+
+class _CorrGrad:
+    """one training block's gradient pyramid [E,ht*wd,Q] during a backward pass (None outside one).  The backward contexts hold only
+    this, not the block's volumes, which no backward reads."""
+
+    def __init__(self):
+        self.gpyr = None
+
+
+class _CorrBuild(torch.autograd.Function):
+    """fmap1, fmap2 [E,128,ht,wd] f32 -> a token every lookup takes as an input.  Autograd runs this backward after every lookup that
+    reaches the loss has added its gradient into the block's gradient pyramid: the adjoint runs once, and the pyramid is released so
+    that the next backward pass starts from zero."""
+
+    @staticmethod
+    def forward(ctx, fmap1, fmap2, state):
+        ctx.state = state                      # a _CorrGrad
+        ctx.save_for_backward(fmap1, fmap2)
+        return fmap1.new_zeros(0)
+
+    @staticmethod
+    def backward(ctx, _):
+        fmap1, fmap2 = ctx.saved_tensors
+        state = ctx.state
+        if state.gpyr is None:                 # no lookup reached the loss
+            return torch.zeros_like(fmap1), torch.zeros_like(fmap2), None
+        g1, g2 = install().corr_adjoint(fmap1, fmap2, state.gpyr)
+        state.gpyr = None
+        return g1, g2, None
+
+
+class _CorrLookup(torch.autograd.Function):
+    """one CorrBlock.__call__: coords [E,2,ht,wd] -> [E,196,ht,wd]; its backward adds into the block's gradient pyramid (zeroed by the
+    first lookup of a backward pass) and gives the token a zero gradient, coords none"""
+
+    @staticmethod
+    def forward(ctx, token, coords, pyramid, state):
+        ctx.state = state                      # a _CorrGrad
+        ctx.save_for_backward(coords)
+        return install().corr_lookup_pyramid(pyramid, coords)
+
+    @staticmethod
+    def backward(ctx, grad):
+        coords, = ctx.saved_tensors
+        state = ctx.state
+        if state.gpyr is None:
+            E, _, ht, wd = coords.shape
+            q = sum((ht >> l) * (wd >> l) for l in range(4))
+            state.gpyr = torch.zeros(E, ht * wd, q, dtype=torch.float32, device=coords.device)
+        install().corr_grad_accumulate(coords, grad.contiguous(), state.gpyr)
+        return coords.new_zeros(0), None, None, None
+
+
+def _corr_training_unsupported(fmap1, fmap2, num_levels=4, radius=3):
+    """why the native training CorrBlock cannot run these arguments (None: it can)"""
+    if fmap1.dim() != 5 or fmap2.shape != fmap1.shape:
+        return "fmap1 and fmap2 must be [B,N,C,H,W] of one shape"
+    if not (fmap1.is_cuda and fmap2.is_cuda):
+        return "fmaps are not on a CUDA device"
+    if fmap1.dtype != torch.float32 or fmap2.dtype != torch.float32:
+        return "dtype %s / %s (float32 has a kernel)" % (fmap1.dtype, fmap2.dtype)
+    if num_levels != 4:
+        return "%d levels (4 has a kernel)" % num_levels
+    if radius != 3:
+        return "radius %d (3 has a kernel)" % radius
+    batch, num, dim, ht, wd = fmap1.shape
+    if dim != 128:
+        return "%d channels (128 has a kernel)" % dim
+    if ht < 8 or wd < 8:
+        return "%dx%d feature maps (ht and wd must be at least 8)" % (ht, wd)
+    if batch * num > 65535:
+        return "%d edges (at most 65535)" % (batch * num)
+    return None
+
+
+class CorrBlock:
+    """CorrBlock(fmap1, fmap2, num_levels=4, radius=3) of modules/corr.py:6-71 for fp32 [B,N,128,ht,wd] CUDA feature maps, differentiable
+    in both maps: the volume and its pooled levels (`droid_backends.corr_volume_pyramid_f32`), each call's 4-level lookup
+    (`corr_lookup_pyramid`, bit-identical to the reference's corr_index_forward + cat on these volumes) and one backward per pass
+    (`corr_grad_accumulate` per call into one gradient pyramid, `corr_adjoint` once).  coords get no gradient, as in the reference.
+    Under no_grad, or with maps that do not require grad, nothing is kept for backward.  No host synchronisation."""
+
+    def __init__(self, fmap1, fmap2, num_levels=4, radius=3):
+        _require("CorrBlock", _corr_training_unsupported(fmap1, fmap2, num_levels, radius))
+        be = install()
+        self.num_levels, self.radius = num_levels, radius
+        batch, num, dim, ht, wd = fmap1.shape
+        f1 = fmap1.reshape(batch * num, dim, ht, wd).contiguous()
+        f2 = fmap2.reshape(batch * num, dim, ht, wd).contiguous()
+        self.corr_pyramid = be.corr_volume_pyramid_f32(f1.detach(), f2.detach())
+        self._grad = _CorrGrad()
+        self._token = None
+        if torch.is_grad_enabled() and (f1.requires_grad or f2.requires_grad):
+            self._token = _CorrBuild.apply(f1, f2, self._grad)
+
+    def __call__(self, coords):
+        batch, num, ht, wd, _ = coords.shape
+        c = coords.detach().permute(0, 1, 4, 2, 3).contiguous().view(batch * num, 2, ht, wd).float()
+        if self._token is not None and torch.is_grad_enabled():
+            out = _CorrLookup.apply(self._token, c, self.corr_pyramid, self._grad)
+        else:
+            out = install().corr_lookup_pyramid(self.corr_pyramid, c)
+        return out.view(batch, num, -1, ht, wd)
+
+
+def install_corr_training_hook(droid_net_module, strict=True):
+    """droid_net_module = the imported reference module `droid_net`.  Sets its global `CorrBlock` (droid_net.py:8, built once per
+    DroidNet.forward and looked up once per update iteration) to the native training block (`CorrBlock` above), forward and backward.
+    A block it cannot build (not fp32 CUDA [B,N,128,ht,wd] maps with ht, wd >= 8, num_levels != 4, radius != 3; f16 / autocast training
+    among them) raises under strict=True and builds the reference's CorrBlock under strict=False.  modules.corr.CorrBlock, which the
+    frontend, the factor graph and the motion filter use, is not touched."""
+    ref = getattr(droid_net_module, "_b200_reference_CorrBlock", None) or droid_net_module.CorrBlock
+
+    def make(fmap1, fmap2, num_levels=4, radius=3):
+        why = _corr_training_unsupported(fmap1, fmap2, num_levels, radius)
+        if why is not None and not strict:
+            return ref(fmap1, fmap2, num_levels=num_levels, radius=radius)
+        _require("CorrBlock", why)
+        return CorrBlock(fmap1, fmap2, num_levels, radius)
+
+    droid_net_module._b200_reference_CorrBlock = ref
+    droid_net_module.CorrBlock = make
+    _record("install_corr_training_hook", droid_net_module, strict=strict)
     return droid_net_module

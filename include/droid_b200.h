@@ -74,10 +74,29 @@ int dba_corr_volume_pyramid(const void* fmap1, const void* fmap2, const int64_t*
 
 /* CorrBlock.__call__ (reference droid_slam/modules/corr.py:40-50) in one launch: out [n,196,h1,w1] = concatenation over the four levels
  * of corr_index_forward(volume_l, coords / 2^l, 3) -- bit-identical values; coords [n,2,h1,w1] f32 at level-0 scale are read once.
- * f16 volumes, h1, w1 >= 8, planes of level l [h1 >> l, w1 >> l], each level tensor 16-byte aligned; no load leaves a level tensor.
- * tiled_mask: 0 = reference layout, 3 = levels 0 and 1 in the tiled layout above (h1 % 8 == 0 and w1 % 64 == 0 only). */
+ * f16 or f32 volumes, h1, w1 >= 8, planes of level l [h1 >> l, w1 >> l], each level tensor 16-byte aligned; no load leaves a level tensor.
+ * tiled_mask: 0 = reference layout, 3 = levels 0 and 1 in the tiled layout above (f16, h1 % 8 == 0 and w1 % 64 == 0 only). */
 int dba_corr_lookup_pyramid(const void* v0, const void* v1, const void* v2, const void* v3, const float* coords, void* out,
                             int n, int h1, int w1, int tiled_mask, int dtype, dba_stream_t stream);
+
+/* ---- CorrBlock for training (fp32 feature maps, forward and backward) ------------------------------------------------------------
+ * DroidNet.forward's CorrBlock(fmaps[:,ii], fmaps[:,jj]) (reference droid_slam/modules/corr.py:6-71) with train.py's fp32 maps.
+ * fmap1, fmap2 [n,128,ht,wd] f32, one map pair per edge; ht, wd >= 8; n <= 65535.  Products on the tf32 tensor cores with 3xTF32 splitting
+ * (fp32-level accuracy), fixed summation order, no host synchronisation.
+ * dba_corr_volume_pyramid_f32: out_l [n,ht,wd,ht>>l,wd>>l] (reference layout), out_0 = (f1/4)^T (f2/4), out_{l+1} = 2x2 mean of out_l over
+ *   complete blocks.  Readable by dba_corr_lookup_pyramid(dtype DBA_F32) and dba_corr_index_forward.
+ * The gradient pyramid: gpyr [n][ht*wd][Q] f32, Q = sum_l (ht>>l)(wd>>l); row p holds the gradient of source pixel p's plane of each level,
+ *   level 0 first.  The caller zeroes it once per backward pass.
+ * dba_corr_grad_accumulate: adds the gradient of one lookup -- grad [n,196,ht,wd] of dba_corr_lookup_pyramid's output at coords [n,2,ht,wd]
+ *   -- into gpyr.  One thread owns each row: no atomics, the same bits every run.
+ * dba_corr_adjoint: grad1 = sum_l G_l P_l(f2) / 16, grad2 = sum_l P_l^T (G_l^T f1) / 16 into [n,128,ht,wd] (fully overwritten), P_l the
+ *   2^l block mean (floor rule).  workspace: 16-byte aligned, at least dba_corr_adjoint_workspace_bytes. */
+int dba_corr_volume_pyramid_f32(const float* fmap1, const float* fmap2, float* out0, float* out1, float* out2, float* out3, int n,
+                                int channels, int ht, int wd, dba_stream_t stream);
+int dba_corr_grad_accumulate(const float* coords, const float* grad, float* gpyr, int n, int ht, int wd, dba_stream_t stream);
+size_t dba_corr_adjoint_workspace_bytes(int n, int channels, int ht, int wd);
+int dba_corr_adjoint(const float* fmap1, const float* fmap2, const float* gpyr, float* grad1, float* grad2, int n, int channels, int ht,
+                     int wd, void* workspace, size_t workspace_bytes, dba_stream_t stream);
 
 /* ---- on-the-fly correlation ---------------------------------------------------------------------
  * replaces altcorr_cuda_forward / altcorr_cuda_backward (reference src/altcorr_kernel.cu:132-225, bound at
