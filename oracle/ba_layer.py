@@ -74,6 +74,13 @@ def _jacobians(poses, disps, intrinsics, ii, jj):
 
 def ba(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp=1, ep=0.1, lm=1e-4):
     """BA(target, weight, eta, poses (SE3 stand-in), disps, intrinsics, ii, jj, fixedp) -> (poses', disps'), rig = 1"""
+    out = ba_system(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp, ep, lm)
+    return out["poses"], out["disps"]
+
+
+def ba_system(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp=1, ep=0.1, lm=1e-4):
+    """ba() with its reduced system: dict(poses, disps (ba's outputs), S [B,6P,6P] (H + (ep + lm H) I - E Q E^T, both triangles),
+    y [B,6P] (v - E Q w), dx [B,6P] (0 when the factor failed anywhere in the batch), dz [B,M,HW]), all differentiable"""
     B, N, ht, wd = disps.shape
     E, D, HW = ii.shape[0], 6, ht * wd
     coords, valid, Ji, Jj, Jz = _jacobians(poses, disps, intrinsics, ii, jj)
@@ -114,14 +121,14 @@ def ba(target, weight, eta, poses, disps, intrinsics, ii, jj, fixedp=1, ep=0.1, 
     Et = Em.transpose(1, 2)
     S = H - Em @ (Q * Et)
     y = v - Em @ (Q * wv)
-    dx = _CholeskySolver.apply(S, y)
-    dz = (Q * (wv - Et @ dx)).view(B, M, ht, wd)
-    dx = dx.reshape(B, P, D)
+    dx1 = _CholeskySolver.apply(S, y)
+    dz = (Q * (wv - Et @ dx1)).view(B, M, ht, wd)
+    dx = dx1.reshape(B, P, D)
     dxa = scatter_sum(dx, torch.arange(P, device=dx.device) + fixedp, dim=1, dim_size=N)
     poses = poses.retr(dxa)
     disps = disps + scatter_sum(dz, kx, dim=1, dim_size=N)
     disps = torch.where(disps > 10, torch.zeros_like(disps), disps)
-    return poses, disps.clamp(min=0.0)
+    return dict(poses=poses, disps=disps.clamp(min=0.0), S=S, y=y.view(B, P * D), dx=dx1.view(B, P * D), dz=dz.view(B, M, HW))
 
 
 def left_perturbed(data, eps):

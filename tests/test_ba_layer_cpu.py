@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
-from ba_layer_cases import cases  # noqa: E402
+from ba_layer_cases import cases, domain_cases  # noqa: E402
 from oracle import ba_layer as oba  # noqa: E402
 
 GOLDEN = os.path.join(ROOT, "tests", "golden", "ba_layer.pt")
@@ -130,10 +130,9 @@ def test_unsupported_reasons(why, edit):
     assert why in modules._ba_layer_unsupported(*a, **k)
 
 
-def test_near_plane_case_covers_both_depth_branches_and_both_crossings():
-    """the near-plane case has pixels with 0.1 <= Z < 0.2 (invalid, no clamp) and Z < 0.1 (clamped to 1), and updated disparities above
-    10 and below 0 before the where / clamp"""
-    c = cases()["near_plane_crossings"]
+def _assert_near_plane_bands(c):
+    """pixels with 0.1 <= Z < 0.2 (invalid, no clamp) and Z < 0.1 (clamped to 1), and updated disparities above 10 and below 0 before
+    the where / clamp"""
     P = oba.SE3(c["poses"])
     ht, wd = c["disps"].shape[2:]
     fx, fy, cx, cy = c["intrinsics"][:, c["ii"], None, None, :].unbind(-1)
@@ -155,3 +154,75 @@ def test_near_plane_case_covers_both_depth_branches_and_both_crossings():
     finally:
         torch.where = where
     assert int((seen["pre"] > 10).sum()) > 0 and int((seen["pre"] < 0).sum()) > 0
+
+
+def test_near_plane_case_covers_both_depth_branches_and_both_crossings():
+    """the near-plane case has pixels with 0.1 <= Z < 0.2 (invalid, no clamp) and Z < 0.1 (clamped to 1), and updated disparities above
+    10 and below 0 before the where / clamp"""
+    _assert_near_plane_bands(cases()["near_plane_crossings"])
+
+
+def _facts(c):
+    B, N, ht, wd = c["disps"].shape
+    ii, jj = c["ii"], c["jj"]
+    P = N - c["fixedp"]
+    n = 6 * P
+    src = torch.unique(ii)
+    pairs = list(zip(ii.tolist(), jj.tolist()))
+    return dict(B=B, N=N, HW=ht * wd, P=P, n=n, E=len(pairs), outdeg=torch.bincount(ii, minlength=N),
+                src=src.tolist(), dup=len(pairs) - len(set(pairs)), self_edges=int((ii == jj).sum()))
+
+
+def test_domain_cases_reach_their_corners():
+    """each of domain_cases() reaches the corner of the layer's domain it is named for"""
+    d = {name: _facts(c) for name, c in domain_cases().items()}
+    for name in ("p20_48x64", "p20_60x80_chain4", "near_plane_p20"):
+        f = d[name]
+        # bal_factor_kernel at its largest: n = 120, P^2 = 400 blocks over 256 threads (the shared memory it launches with is read
+        # from the launch itself, tests/test_ba_layer_domain_gpu.py test_p20_factor_and_lambda_x_launch_with_the_full_system)
+        assert (f["P"], f["n"]) == (20, 120) and f["P"] ** 2 > 256, name
+    assert d["p20_48x64"]["HW"] == 48 * 64 and 85 <= d["p20_48x64"]["E"] <= 95
+    f = d["p20_60x80_chain4"]
+    assert f["HW"] % 128 == 64 and domain_cases()["p20_60x80_chain4"]["chain"] == 4
+    assert int(f["outdeg"].max()) >= 5 and int((f["outdeg"] == 0).sum()) > 0
+    assert (d["fixedp0"]["P"], d["fixedp0"]["N"]) == (6, 6)
+    f = d["p1"]
+    assert f["P"] == 1 and sum(1 for s in f["src"] if s < 6) >= 5          # one pose unknown; the other sources are fixed frames
+    f, c = d["many_fixed_gaps"], domain_cases()["many_fixed_gaps"]
+    assert f["N"] > 64 and f["P"] == 15 and max(f["src"]) >= 64
+    assert f["src"] != list(range(f["src"][0], f["src"][0] + len(f["src"])))  # the ii -> k map has gaps above its first source
+    assert len([s for s in range(40, 70) if s not in f["src"]]) >= 5 and int((c["jj"] < 55).sum()) > 0
+    touched = set(c["ii"].tolist()) | set(c["jj"].tolist())
+    assert all(s in touched for s in range(55, 70))                           # every pose unknown is on some edge
+    f = d["train24_batch4"]
+    assert (f["B"], f["E"], f["P"]) == (4, 24, 5) and int(f["outdeg"].max()) >= 5 and int((f["outdeg"] == 0).sum()) > 0
+    f = d["hub_duplicates"]
+    assert f["B"] == 2 and int(f["outdeg"].max()) == 12 and f["dup"] >= 2 and f["self_edges"] == 1
+    assert d["tiny_3x5"]["HW"] == 15 < 32
+    # the chained case keeps every disparity off the clamp at 0 (fp64, all 4 calls), by far more than D's fp32 error (~1e-6 of 2)
+    c = domain_cases()["p20_60x80_chain4"]
+    P, D = oba.SE3(c["poses"]), c["disps"]
+    for _ in range(c["chain"]):
+        P, D = oba.ba(c["target"], c["weight"], c["eta"], P, D, c["intrinsics"], c["ii"], c["jj"], fixedp=c["fixedp"])
+        assert float(D.min()) > 0.05
+
+
+def test_batch4_third_fails_fails_in_element_2_only():
+    c = domain_cases()["batch4_third_fails"]
+    S = oba.ba_system(c["target"], c["weight"], c["eta"], oba.SE3(c["poses"]), c["disps"], c["intrinsics"], c["ii"], c["jj"],
+                      fixedp=c["fixedp"])["S"]
+    assert (torch.linalg.cholesky_ex(S)[1] != 0).tolist() == [False, False, True, False]
+
+
+def test_near_plane_p20_covers_both_depth_branches_and_both_crossings():
+    _assert_near_plane_bands(domain_cases()["near_plane_p20"])
+
+
+def test_ba_system_returns_the_reduced_system_of_ba():
+    """ba() is ba_system()'s poses / disps, and dx solves S dx = y"""
+    c = domain_cases()["fixedp0"]
+    args = (c["target"], c["weight"], c["eta"], oba.SE3(c["poses"]), c["disps"], c["intrinsics"], c["ii"], c["jj"])
+    r = oba.ba_system(*args, fixedp=0, ep=1e-2, lm=1e-3)
+    P, D = oba.ba(*args, fixedp=0, ep=1e-2, lm=1e-3)
+    assert torch.equal(P.data, r["poses"].data) and torch.equal(D, r["disps"])
+    assert float((r["S"] @ r["dx"][..., None] - r["y"][..., None]).abs().max()) < 1e-10 * float(r["y"].abs().max())
