@@ -33,6 +33,79 @@ def make_inputs(B, N, ht, wd, calls, seed=0, C=128, dev="cpu"):
     return f1.to(dev), f2.to(dev), [c.to(dev) for c in coords], [w.to(dev) for w in weights]
 
 
+# the stage checks' cases (tests/test_corr_training_stages_*.py): name -> (n edges, ht, wd, calls); the corner each one reaches is
+# checked on the host by tests/test_corr_training_stages_cpu.py
+STAGES = {
+    "8x8": (3, 8, 8, 2),                     # one source tile, one target block, level 3 is 1x1
+    "odd_23x31": (2, 23, 31, 2),             # the floor rule drops a row and a column at every level; partial blocks; HW % 64 = 9
+    "portrait_70x43": (2, 70, 43, 2),        # more 8x8 block rows than columns; every level width takes the generic lookup
+    "rows8_8x136": (2, 8, 136, 2),           # level 3 is one row 17 wide
+    "cols8_136x8": (2, 136, 8, 2),           # level 3 is one column 17 high
+    "many_edges_9x13": (300, 9, 13, 2),      # grid.z = 300
+    "train_24x48x64": (24, 48, 64, 15),      # the training shape
+    "large_60x80": (4, 60, 80, 2),           # longer sums than training: Q = 6370, HW = 4800
+}
+# committed bounds kappa <= c sqrt(K) per stage (kappa = |native - exact| / (2^-24 A), A the summed magnitude of the terms), set from
+# the worst kappa measured on an H100 (tests/test_corr_training_stages_gpu.py) and held below the worst-case model
+# (tests/test_corr_training_stages_cpu.py)
+KAPPA_PER_SQRT_K = {"volume": 0.6, "g_f1": 0.6, "g_f2": 1.25}
+
+
+def stage_K(stage, ht, wd):
+    """terms per output: 128 channels for the volume, Q for g_f1, HW for g_f2"""
+    return {"volume": 128, "g_f1": sum((ht >> l) * (wd >> l) for l in range(4)), "g_f2": ht * wd}[stage]
+
+
+NONFINITE = ("nan_x", "nan_y", "nan_xy", "inf_x", "inf_y", "inf_xy", "ninf_x", "ninf_y", "ninf_xy")
+
+
+def stage_cases():
+    """[(name, n, ht, wd, calls)] of STAGES"""
+    return [(name,) + v for name, v in STAGES.items()]
+
+
+def special_coords(ht, wd):
+    """[(category, x, y)]: half-integers, points exactly on each level's last row and column (at level l the coordinate is scaled by
+    2^-l, so (w_l - 1) 2^l lands on w_l - 1), +-1e30 (the floor saturates) and, last, NaN / +inf / -inf in x, in y and in both"""
+    inf, nan = float("inf"), float("nan")
+    xm, ym = float(wd // 3), float(ht // 3)
+    out = [("half", 0.5, 0.5), ("half", wd / 2 + 0.5, ht / 2 - 0.5), ("half", wd - 1.5, ht - 1.5), ("half", -2.5, ym + 0.5)]
+    for l in range(4):
+        xl, yl = float(((wd >> l) - 1) << l), float(((ht >> l) - 1) << l)
+        out += [("last%d" % l, xl, yl), ("last%d" % l, xl, ym), ("last%d" % l, xm, yl)]
+    out += [("huge", 1e30, ym), ("huge", -1e30, ym), ("huge", xm, 1e30), ("huge", xm, -1e30), ("huge", 1e30, 1e30)]
+    out += [("nan_x", nan, ym), ("nan_y", xm, nan), ("nan_xy", nan, nan), ("inf_x", inf, ym), ("inf_y", xm, inf), ("inf_xy", inf, inf),
+            ("ninf_x", -inf, ym), ("ninf_y", xm, -inf), ("ninf_xy", -inf, -inf)]
+    return out
+
+
+def special_pixels(ht, wd, count, seed):
+    """`count` distinct source pixels (flat indices) below make_inputs's integer rows, off its last row and last column"""
+    y, x = torch.meshgrid(torch.arange(ht // 4, ht - 1), torch.arange(wd - 1), indexing="ij")
+    free = (y * wd + x).reshape(-1)
+    assert free.numel() >= count, (ht, wd, count)
+    return free[torch.randperm(free.numel(), generator=torch.Generator().manual_seed(seed))[:count]]
+
+
+def stage_inputs(name, seed=0, dev="cpu"):
+    """fmap1, fmap2 [n,128,ht,wd] f32; coords of every call [n,2,ht,wd] f32 (the C ABI's layout): make_inputs's coordinates with
+    special_coords placed at the same pixels in every call, the non-finite ones on edge 0 only; the lookup gradient of every call
+    [n,196,ht,wd] f32 (make_inputs's loss weights); the pixels and categories of the special coordinates"""
+    n, ht, wd, calls = STAGES[name]
+    f1, f2, coords, weights = make_inputs(1, n, ht, wd, calls, seed=seed)
+    spec = special_coords(ht, wd)
+    pix = special_pixels(ht, wd, len(spec), seed)
+    out = []
+    for c in coords:
+        c = c[0].permute(0, 3, 1, 2).contiguous()                   # [n, 2, ht, wd]
+        flat = c.view(n, 2, ht * wd)
+        for (cat, x, y), p in zip(spec, pix.tolist()):
+            edges = slice(0, 1) if cat in NONFINITE else slice(None)
+            flat[edges, 0, p], flat[edges, 1, p] = x, y
+        out.append(c.to(dev))
+    return f1[0].to(dev), f2[0].to(dev), out, [w[0].contiguous().to(dev) for w in weights], pix, [s[0] for s in spec]
+
+
 class _Sampler(torch.autograd.Function):
     """the reference's CorrSampler (modules/corr.py:8-22) on this package's corr_index_forward / corr_index_backward"""
 

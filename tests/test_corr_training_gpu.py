@@ -31,6 +31,8 @@ CASES = {
     "partial_loss": (1, 2, 16, 24, 4, (0, 2)),
     "wd_43x70": (1, 2, 43, 70, 2, None),
     "tiny_8x8": (1, 2, 8, 8, 2, None),
+    "portrait_70x43": (1, 2, 70, 43, 2, None),
+    "rows8_8x136": (1, 2, 8, 136, 2, None),
     "train_24x48x64": (1, 24, 48, 64, 15, None),
 }
 
@@ -76,7 +78,7 @@ def test_against_fp64_within_twice_the_reference_fp32_error(name):
         assert torch.equal(only[2], nat[2]) and torch.equal(only[3], nat[3])
 
 
-@pytest.mark.parametrize("name", ["odd_17x23", "batch2", "wd_43x70", "tiny_8x8", "three_edges"])
+@pytest.mark.parametrize("name", ["odd_17x23", "batch2", "wd_43x70", "tiny_8x8", "three_edges", "portrait_70x43", "rows8_8x136"])
 def test_lookup_is_corr_index_forward_on_the_native_volume(name):
     B, N, ht, wd, calls, _ = CASES[name]
     be = install()
