@@ -337,7 +337,7 @@ extern "C" int dba_frame_distance(const float* poses, const float* disps, const 
                                   const int64_t* jj, float* dist, int n_pairs, int ht, int wd, float beta, dba_stream_t stream) {
   DBA_CHECK_ARG(n_pairs >= 0 && ht >= 0 && wd >= 0, "negative extent");
   if (n_pairs == 0) return DBA_OK;
-  DBA_CHECK_ARG(poses && disps && intrinsics && ii && jj && dist, "null pointer");
+  DBA_CHECK_ARG(poses && (disps || ht * wd == 0) && intrinsics && ii && jj && dist, "null pointer");   // hw = 0: every pair is 1000
   frame_distance_kernel<<<n_pairs, 256, 0, (cudaStream_t)stream>>>(poses, disps, intrinsics, ii, jj, dist, ht, wd, beta);
   DBA_CHECK_LAUNCH("frame_distance");
   return DBA_OK;

@@ -3,9 +3,12 @@
 The reference build is oracle/_ref/droid_backends_ref (reference src/{droid.cpp,droid_kernels.cu,correlation_kernels.cu,
 altcorr_kernel.cu} compiled for sm_90a by oracle/build_ref.sh against the Eigen stand-in).  Regenerate on an H100 with it present:
     python tests/golden/make_reference_build_golden.py [out.pt]
+or, to add one group of entries to the existing file and leave the others as they are:
+    python tests/golden/make_reference_build_golden.py --add geometry_edges [out.pt]
 Outputs the tests require to be bit-identical are stored as SHA-256 digests of their bytes plus a seeded sample of values (for the
 failure message); frame distances in full; bundle adjustment as the updated poses and a seeded sample of the inverse depths.
-The sample positions are not stored: sample_index regenerates them from their seeds."""
+The geometry_edges group is kept small: digests alone, and frame distances in full up to N_FD_SAMPLE pairs, else a seeded sample of
+that many.  The sample positions are not stored: sample_index regenerates them from their seeds."""
 import hashlib
 import os
 import sys
@@ -16,10 +19,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 from droid_slam_b200 import synth  # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import geometry_cases  # noqa: E402
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_build.pt")
 N_SAMPLE = 4096
 N_DISP_SAMPLE = 16384
+N_FD_SAMPLE = 2048
 BA_CASES = {  # name: (scene, scene kwargs, iterations, motion_only)
     "ba_metric": ("metric", {}, 2, False),
     "ba_c4_stereo": ("c4_stereo", {}, 2, False),
@@ -100,6 +106,30 @@ def geometry(be, dev):
     return out
 
 
+GEOMETRY_EDGE_CASES = [n for n in geometry_cases.CASES if n != "empty"] + ["many_edges"]   # hw = 0 launches nothing in the reference
+
+
+def geometry_edges_case(be, dev, name):
+    """projmap, iproj, depth_filter and frame_distance (every beta of the case) on one case of tests/geometry_cases.py"""
+    c = geometry_cases.case(name)
+    P, D, K, ii, jj, ix, th = [c[k].to(dev).contiguous() for k in ("poses", "disps", "intr", "ii", "jj", "df_ix", "df_thresh")]
+    out = {}
+    out["projmap_coords"], out["projmap_valid"] = be.projmap(P, D, K, ii, jj)
+    out["iproj"] = be.iproj(P, D, K)
+    out["depth_filter"] = be.depth_filter(P, D, K, ix, th)
+    for beta in c["betas"]:
+        out["frame_distance beta=%g" % beta] = be.frame_distance(P, D, K, ii, jj, beta)
+    return out
+
+
+def geometry_edges(be, dev):
+    out = {}
+    for name in GEOMETRY_EDGE_CASES:
+        for k, v in geometry_edges_case(be, dev, name).items():
+            out["geometry_edges/%s/%s" % (name, k)] = v
+    return out
+
+
 def ba(be, dev, name):
     scene, kw, itrs, motion_only = BA_CASES[name]
     s = synth.make_scene(scene, **kw)
@@ -116,6 +146,35 @@ def record_identical(t):
     return {"sha256": digest(t), "shape": tuple(t.shape), "dtype": str(t.dtype), "val": flat[idx].clone()}
 
 
+def _record(k, v):
+    return {"full": v.cpu()} if "frame_distance" in k else record_identical(v)
+
+
+def fd_sample_index(n):
+    return sample_index(n, N_FD_SAMPLE, seed=2)
+
+
+def record_edge(k, v):
+    """a geometry_edges entry: the digest of a bit-identical output; a frame-distance vector's length and its values at
+    fd_sample_index (all of them, permuted, when there are at most N_FD_SAMPLE)"""
+    if "frame_distance" in k:
+        flat = v.detach().reshape(-1).cpu()
+        return {"n": flat.numel(), "val": flat[fd_sample_index(flat.numel())].clone()}
+    return {"sha256": digest(v), "shape": tuple(v.shape), "dtype": str(v.dtype)}
+
+
+def add_group(path, group):
+    """add one group's keys to an existing fixture file; every entry already in it stays as it is"""
+    sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
+    import droid_backends_ref as ref
+    gold = torch.load(path, weights_only=False)
+    new = {k: record_edge(k, v) for k, v in {"geometry_edges": geometry_edges}[group](ref, "cuda").items()}
+    assert not set(new) & set(gold), "only adds keys"
+    gold.update(new)
+    torch.save(gold, path)
+    print("added", len(new), "entries to", path, os.path.getsize(path), "bytes")
+
+
 def main(path):
     sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
     import droid_backends_ref as ref
@@ -127,7 +186,9 @@ def main(path):
     torch.cuda.empty_cache()
     for fn in (corr_f32, altcorr, geometry):
         for k, v in fn(ref, dev).items():
-            gold[k] = {"full": v.cpu()} if k == "frame_distance" else record_identical(v)
+            gold[k] = _record(k, v)
+    for k, v in geometry_edges(ref, dev).items():
+        gold[k] = record_edge(k, v)
     for name in BA_CASES:
         P, D, o = ba(ref, dev, name)
         Df = D.reshape(-1).cpu()
@@ -139,4 +200,7 @@ def main(path):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else GOLD)
+    if len(sys.argv) > 2 and sys.argv[1] == "--add":      # --add geometry_edges [out.pt]
+        add_group(sys.argv[3] if len(sys.argv) > 3 else GOLD, sys.argv[2])
+    else:
+        main(sys.argv[1] if len(sys.argv) > 1 else GOLD)
