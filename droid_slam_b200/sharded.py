@@ -81,17 +81,8 @@ class CApiEngine:
         self.system = self.ws[off:off + 8 * (n * n + n)].view(torch.float64)      # the all-reduce buffer, in place
         self.dx = torch.zeros(self.P, 6, device=self.device)
         self.dz = torch.zeros(N, ht * wd, device=self.device)                      # at most one depth frame per frame
-        a = c_api.BAArgs()
-        a.poses, a.disps, a.intrinsics, a.disps_sens = poses.data_ptr(), disps.data_ptr(), intrinsics.data_ptr(), disps_sens.data_ptr()
-        a.targets, a.weights = targets.data_ptr(), weights.data_ptr()
-        a.eta, a.eta_rows, a.eta_by_frame = eta_by_frame.data_ptr(), eta_by_frame.shape[0], 1
-        a.ii, a.jj = ii.data_ptr(), jj.data_ptr()
-        a.n_frames, a.n_edges, a.ht, a.wd, a.t0, a.t1 = N, E, ht, wd, t0, t1
-        a.lm, a.ep, a.motion_only = lm, ep, 0
-        a.dx_out, a.dz_out = self.dx.data_ptr(), self.dz.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws_bytes
-        a.stream = torch.cuda.current_stream(self.device).cuda_stream
-        a.own_lo, a.own_hi = own
+        a = c_api.ba_args(poses, disps, intrinsics, disps_sens, targets, weights, eta_by_frame, ii, jj, t0, t1, lm, ep, self.dx, self.dz,
+                          self.ws, torch.cuda.current_stream(self.device).cuda_stream, own=own, eta_by_frame=True)
         self.p2p = p2p
         if p2p is not None:
             assert p2p.nd == n * n + n, "P2PSystem was sized for another window"

@@ -151,9 +151,6 @@ def test_update_module_hook_sets_the_native_operator():
 def test_c_abi_rejects_bad_arguments_before_any_launch():
     L = c_api.load()
     f = L.dba_fragment_handover
-    f.restype = ctypes.c_int
-    f.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_longlong, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-                                          ctypes.c_void_p, ctypes.c_void_p]
     assert L.dba_fragment_handover and hasattr(L, "dba_last_error")
     p = ctypes.c_void_p(64)
     for t0 in (1, 5, 9, -1):                              # the reference's negative slices are not reproduced

@@ -73,17 +73,9 @@ class StageDriver:
         self.off = L.dba_ba_system_offset(N, E, ht, wd, self.t0, self.t1)
         self.dx = torch.full((max(self.P, 1), 6), float("nan"), device=dev)
         self.dz = torch.full((self.M, ht * wd), float("nan"), device=dev)
-        a = c_api.BAArgs()
-        a.poses, a.disps, a.intrinsics, a.disps_sens = self.poses.data_ptr(), self.disps.data_ptr(), self.intr.data_ptr(), self.ds.data_ptr()
-        a.targets, a.weights, a.eta, a.eta_rows = self.tg.data_ptr(), self.wt.data_ptr(), self.eta.data_ptr(), self.eta.shape[0]
-        a.ii, a.jj = self.ii.data_ptr(), self.jj.data_ptr()
-        a.n_frames, a.n_edges, a.ht, a.wd, a.t0, a.t1 = N, E, ht, wd, self.t0, self.t1
-        a.lm, a.ep, a.motion_only = s["lm"], s["ep"], 0
-        a.dx_out, a.dz_out = self.dx.data_ptr(), self.dz.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), ws_bytes
-        a.stream = torch.cuda.current_stream().cuda_stream
-        a.own_lo, a.own_hi, a.eta_by_frame = 0, N, int(s["eta_by_frame"])
-        self.a = a
+        self.a = c_api.ba_args(self.poses, self.disps, self.intr, self.ds, self.tg, self.wt, self.eta, self.ii, self.jj, self.t0, self.t1,
+                               s["lm"], s["ep"], self.dx, self.dz, self.ws, torch.cuda.current_stream().cuda_stream,
+                               eta_by_frame=s["eta_by_frame"])
 
     def call(self, fn):
         c_api.check(getattr(self.L, fn)(ctypes.byref(self.a)), fn)

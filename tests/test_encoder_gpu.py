@@ -66,20 +66,10 @@ def test_encoder_f16_images_match_oracle(backends, no_tf32, name):
     _compare(backends, name, 2, 240, 320, dtype=torch.float16)
 
 
-class _Weights(ctypes.Structure):
-    _fields_ = [("w", ctypes.c_void_p * 14), ("b", ctypes.c_void_p * 14)]
-
-
-class _Args(ctypes.Structure):
-    _fields_ = [("images", ctypes.c_void_p), ("images_dtype", ctypes.c_int), ("n_images", ctypes.c_int), ("H", ctypes.c_int), ("W", ctypes.c_int),
-                ("weights", ctypes.POINTER(_Weights)), ("norm", ctypes.c_int), ("output_dim", ctypes.c_int), ("out", ctypes.c_void_p),
-                ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t), ("stream", ctypes.c_void_p)]
-
-
 def test_encoder_argument_validation_launches_nothing(capi):
     H, W = 64, 96
     pk = pack_encoder_weights(synth.make_encoder_weights(0, 128), "instance", 128, "cuda")
-    wt = _Weights()
+    wt = c_api.EncoderWeights()
     for k in range(14):
         wt.w[k], wt.b[k] = pk[k].data_ptr(), pk[14 + k].data_ptr()
     img = torch.randn(1, 3, H, W, device="cuda")
@@ -90,7 +80,7 @@ def test_encoder_argument_validation_launches_nothing(capi):
     wsp = (ws.data_ptr() + 255) // 256 * 256
 
     def args(**over):
-        a = _Args(img.data_ptr(), c_api.DBA_F32, 1, H, W, ctypes.pointer(wt), 1, 128, out.data_ptr(), wsp, nbytes, None)
+        a = c_api.EncoderArgs(img.data_ptr(), c_api.DBA_F32, 1, H, W, ctypes.pointer(wt), 1, 128, out.data_ptr(), wsp, nbytes, None)
         for k, v in over.items():
             setattr(a, k, v)
         return a

@@ -549,31 +549,26 @@ def case_weights(case, norm):
     return sd
 
 
-@pytest.fixture(scope="module")
-def lib():
-    return c_api.load()
-
-
 # ---- tests -----------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["fnet", "cnet"])
-def test_stage_table_has_one_row_per_launch(lib, name):
+def test_stage_table_has_one_row_per_launch(capi, name):
     norm, _ = ENCODERS[name]
     rows = stage_table(norm)
     for n, H, W in ((1, 8, 8), (2, 64, 96), (1, 384, 512)):
-        lay = layout(lib, n, H, W, norm)
+        lay = layout(capi, n, H, W, norm)
         assert lay["n_launches"] == len(rows) == (43 if norm else 17)
         stats = [r["k"] for r in rows if r["kind"] == "conv" and r["epi"] == "stats"]
         assert [k for k in range(14) if lay["plans"][k]["slots"]] == stats
     assert sum(r["kind"] == "conv" for r in rows) == 14 and [r["k"] for r in rows if r["kind"] == "conv"] == list(range(14))
     bad = (ctypes.c_size_t * 8)()
-    assert lib.dba_encoder_workspace_layout(1, 12, 8, norm, bad, bad, ctypes.byref(ctypes.c_int()), (ctypes.c_int * 70)()) == 1
-    assert lib.dba_encoder_workspace_layout(1, 8, 8, 2, bad, bad, ctypes.byref(ctypes.c_int()), (ctypes.c_int * 70)()) == 1
+    assert capi.dba_encoder_workspace_layout(1, 12, 8, norm, bad, bad, ctypes.byref(ctypes.c_int()), (ctypes.c_int * 70)()) == 1
+    assert capi.dba_encoder_workspace_layout(1, 8, 8, 2, bad, bad, ctypes.byref(ctypes.c_int()), (ctypes.c_int * 70)()) == 1
 
 
-def _sweep(lib, norm, n, sizes):
+def _sweep(capi, norm, n, sizes):
     rows = stage_table(norm)
     for H, W in sizes:
-        lay = layout(lib, n, H, W, norm)
+        lay = layout(capi, n, H, W, norm)
         ends = sorted((lay["off"][r], lay["off"][r] + lay["size"][r]) for r in REGIONS)
         assert ends[0][0] == 0 and all(a[1] <= b[0] for a, b in zip(ends, ends[1:])), (n, H, W, "regions overlap")
         assert ends[-1][1] == lay["total"], (n, H, W, "workspace_bytes is not the end of the last region")
@@ -583,21 +578,21 @@ def _sweep(lib, norm, n, sizes):
 
 
 @pytest.mark.parametrize("name", ["fnet", "cnet"])
-def test_workspace_sweep_every_stage_fits_its_region(lib, name):
+def test_workspace_sweep_every_stage_fits_its_region(capi, name):
     """every H, W in multiples of 8 up to 1024 x 1024 at n = 1 (the extents scale with n; n = 2 and 16 on a coarser grid)"""
     norm, _ = ENCODERS[name]
     r8 = range(8, 1025, 8)
-    _sweep(lib, norm, 1, [(H, W) for H in r8 for W in r8])
+    _sweep(capi, norm, 1, [(H, W) for H in r8 for W in r8])
     coarse = [8, 16, 24, 40, 64, 72, 120, 128, 136, 248, 256, 264, 352, 384, 504, 512, 520, 552, 1016, 1024]
     for n in (2, 16):
-        _sweep(lib, norm, n, [(H, W) for H in coarse for W in r8])
+        _sweep(capi, norm, n, [(H, W) for H in coarse for W in r8])
 
 
-def test_case_table_covers_the_tilings(lib):
+def test_case_table_covers_the_tilings(capi):
     seen, flags = set(), set()
     for name, n, H, W, kind, dtype, wts in CASES:
         for norm in (0, 1):
-            lay = layout(lib, n, H, W, norm)
+            lay = layout(capi, n, H, W, norm)
             for row in stage_table(norm):
                 if row["kind"] != "conv":
                     continue
@@ -629,9 +624,9 @@ EMUL_CASES = [("24x72_n2_const1", 2, 24, 72, "const1", torch.float32, "synth"), 
 
 @pytest.mark.parametrize("name", ["fnet", "cnet"])
 @pytest.mark.parametrize("case", EMUL_CASES, ids=[c[0] for c in EMUL_CASES])
-def test_fp32_restatement_meets_every_bound(lib, name, case):
+def test_fp32_restatement_meets_every_bound(capi, name, case):
     norm, _ = ENCODERS[name]
-    lay = layout(lib, case[1], case[2], case[3], norm)
+    lay = layout(capi, case[1], case[2], case[3], norm)
     for seed in (0, 1):
         bad, report, msg = first_rejected(norm, lay, case_weights(case, norm), case_images(case), seed=seed)
         assert bad is None, msg
@@ -667,9 +662,9 @@ def _fault_images(case):
 
 
 @pytest.mark.parametrize("fault, name, case, stage", FAULTS, ids=["%s-%s-%s" % (f[0], f[1], f[2][0]) for f in FAULTS])
-def test_planted_fault_is_rejected_at_its_stage(lib, fault, name, case, stage):
+def test_planted_fault_is_rejected_at_its_stage(capi, fault, name, case, stage):
     norm, _ = ENCODERS[name]
-    lay = layout(lib, case[1], case[2], case[3], norm)
+    lay = layout(capi, case[1], case[2], case[3], norm)
     sd, img = case_weights(case, norm), _fault_images(case)
     assert first_rejected(norm, lay, sd, img)[0] is None                                  # the same run without the fault passes
     bad, report, msg = first_rejected(norm, lay, sd, img, faults=(fault,))
@@ -677,10 +672,10 @@ def test_planted_fault_is_rejected_at_its_stage(lib, fault, name, case, stage):
 
 
 @pytest.mark.parametrize("name", ["fnet", "cnet"])
-def test_fmaxf_relu_is_rejected_where_the_nan_is_dropped(lib, name):
+def test_fmaxf_relu_is_rejected_where_the_nan_is_dropped(capi, name):
     """a ReLU that turns NaN into 0 (fmaxf) fails at the first stage that applies it to a NaN; the NaN-keeping one passes everywhere"""
     norm, _ = ENCODERS[name]
-    lay = layout(lib, 2, 24, 72, norm)
+    lay = layout(capi, 2, 24, 72, norm)
     sd, img = case_weights(_SMALL, norm), case_images(_SMALL)
     img[1, 1, 10, 30] = float("nan")
     bad, report, msg = first_rejected(norm, lay, sd, img)

@@ -53,16 +53,6 @@ GUARD = 64                      # fp16 elements of NaN before and after the outp
 MARGIN = 4096                   # NaN bytes after the workspace
 
 
-class _Weights(ctypes.Structure):
-    _fields_ = [("w", ctypes.c_void_p * 14), ("b", ctypes.c_void_p * 14)]
-
-
-class _Args(ctypes.Structure):
-    _fields_ = [("images", ctypes.c_void_p), ("images_dtype", ctypes.c_int), ("n_images", ctypes.c_int), ("H", ctypes.c_int), ("W", ctypes.c_int),
-                ("weights", ctypes.POINTER(_Weights)), ("norm", ctypes.c_int), ("output_dim", ctypes.c_int), ("out", ctypes.c_void_p),
-                ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t), ("stream", ctypes.c_void_p)]
-
-
 class Run:
     """one encoder call set up in guarded NaN-filled buffers: `prefix(k)` runs the first k launches, `forward()` all of them"""
 
@@ -73,7 +63,7 @@ class Run:
         self.lay = layout(L, n, H, W, self.norm)
         self.images = images.to(dev).contiguous()
         self.pk = pack_encoder_weights(sd, "instance" if self.norm else "none", self.od, dev)
-        self.wt = _Weights()
+        self.wt = c_api.EncoderWeights()
         for k in range(14):
             self.wt.w[k], self.wt.b[k] = self.pk[k].data_ptr(), self.pk[14 + k].data_ptr()
         total = self.lay["total"]
@@ -92,8 +82,9 @@ class Run:
 
     def _args(self, out):
         n, _, H, W = self.images.shape
-        return _Args(self.images.data_ptr(), c_api.DBA_F16 if self.images.dtype == torch.float16 else c_api.DBA_F32, n, H, W, ctypes.pointer(self.wt),
-                     self.norm, self.od, self.view(out).data_ptr(), self.ws.data_ptr(), self.lay["total"], stream().value)
+        return c_api.EncoderArgs(self.images.data_ptr(), c_api.DBA_F16 if self.images.dtype == torch.float16 else c_api.DBA_F32, n, H, W,
+                                 ctypes.pointer(self.wt), self.norm, self.od, self.view(out).data_ptr(), self.ws.data_ptr(), self.lay["total"],
+                                 stream().value)
 
     def prefix(self, k):
         c_api.check(self.L.dba_encoder_forward_prefix(ctypes.byref(self._args(self.out)), k), "encoder_forward_prefix")

@@ -71,10 +71,7 @@ def test_cases_exercise_the_reference_behaviours(gold):
 def test_capi_frame_ingest_symbol_and_argument_checks():
     L = c_api.load()
     assert "dba_encoder_forward_frames" in c_api.SYMBOLS and hasattr(L, "dba_encoder_forward_frames")
-
-    class Format(ctypes.Structure):
-        _fields_ = [("channel_order", ctypes.c_int), ("mean", ctypes.c_float * 3), ("std", ctypes.c_float * 3)]
-
-    f = Format(1, (ctypes.c_float * 3)(0.485, 0.456, 0.406), (ctypes.c_float * 3)(0.229, 0.224, 0.225))
+    f = c_api.FrameFormat(1, (ctypes.c_float * 3)(0.485, 0.456, 0.406), (ctypes.c_float * 3)(0.229, 0.224, 0.225))
     assert L.dba_encoder_forward_frames(None, ctypes.byref(f)) == 1                   # null args
-    assert L.dba_encoder_forward_frames(ctypes.c_void_p(8), None) == 1 and b"frame format" in L.dba_last_error()
+    args = ctypes.cast(ctypes.c_void_p(8), ctypes.POINTER(c_api.EncoderArgs))           # a dummy pointer: the null format is refused first
+    assert L.dba_encoder_forward_frames(args, None) == 1 and b"frame format" in L.dba_last_error()

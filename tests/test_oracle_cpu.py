@@ -271,20 +271,105 @@ def test_capi_exports_match_header():
     assert c_api.load().dba_version() >= 100
 
 
+# ---- the Python view of the C ABI (droid_slam_b200/c_api.py) against the header: a struct that grows or is reordered, or a parameter
+# whose type changes, fails here by name instead of handing the kernels misplaced or truncated arguments ----
+HEADER = os.path.join(ROOT, "include", "droid_b200.h")
+MIRRORS = {"dba_ba_args": c_api.BAArgs, "dba_update_weights": c_api.UpdateWeights, "dba_update_args": c_api.UpdateArgs,
+           "dba_encoder_weights": c_api.EncoderWeights, "dba_encoder_args": c_api.EncoderArgs, "dba_frame_format": c_api.FrameFormat}
+
+
+def _header_probe(tmp_path, lines):
+    """compile and run a C program that includes the header and prints `key value` lines -> {key: int}"""
+    src, exe = tmp_path / "probe.c", tmp_path / "probe"
+    src.write_text("\n".join(['#include <stdio.h>', '#include <stddef.h>', '#include "droid_b200.h"', 'int main(void) {'] + lines
+                             + ['  return 0; }']))
+    subprocess.run(["gcc", "-I", os.path.dirname(HEADER), str(src), "-o", str(exe)], check=True)
+    out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split("\n")
+    return {k: int(v) for k, v in (line.split() for line in out if line)}
+
+
+def _header_fields(struct):
+    """the member names of `typedef struct { ... } struct;` in the header, in order"""
+    hdr = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^}]*)\}\s*%s;" % struct, hdr).group(1)
+    return [re.search(r"(\w+)\s*(\[\w+\])?$", d.strip()).group(1) for s in body.split(";") if s.strip() for d in s.split(",")]
+
+
 def test_capi_args_struct_layout_matches_header(tmp_path):
-    """the ctypes mirror of dba_ba_args must have the C header's size and field offsets (the struct grows over time)"""
-    fields = [f[0] for f in c_api.BAArgs._fields_]
-    src = tmp_path / "layout.c"
-    prog = ['#include <stdio.h>', '#include <stddef.h>', '#include "droid_b200.h"', 'int main(void) {',
-            '  printf("%zu\\n", sizeof(dba_ba_args));']
-    prog += ['  printf("%%zu\\n", offsetof(dba_ba_args, %s));' % f for f in fields]
-    prog += ['  return 0; }']
-    src.write_text("\n".join(prog))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    out = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-    assert out[0] == ctypes.sizeof(c_api.BAArgs)
-    assert out[1:] == [getattr(c_api.BAArgs, f).offset for f in fields]
+    """every ctypes mirror has the header's members in the header's order, its size, and each member's offset and size (arrays
+    included)"""
+    for struct, cls in MIRRORS.items():
+        assert [f for f, _ in cls._fields_] == _header_fields(struct), struct
+    lines, want = [], {}
+    for struct, cls in MIRRORS.items():
+        lines.append('  printf("%s %%zu\\n", sizeof(%s));' % (struct, struct))
+        want[struct] = ctypes.sizeof(cls)
+        for f, _ in cls._fields_:
+            key = "%s.%s" % (struct, f)
+            lines.append('  printf("%s@offset %%zu\\n%s@size %%zu\\n", offsetof(%s, %s), sizeof(((%s*)0)->%s));'
+                         % (key, key, struct, f, struct, f))
+            want[key + "@offset"], want[key + "@size"] = getattr(cls, f).offset, getattr(cls, f).size
+    got = _header_probe(tmp_path, lines)
+    bad = ["%s: header %d, c_api %d" % (k, got[k], v) for k, v in want.items() if got[k] != v]
+    assert not bad, bad
+
+
+def _c_kind(t):
+    t = " ".join(t.replace("*", " * ").split())
+    if t == "const char *":
+        return "const char*"
+    m = re.fullmatch(r"(const )?(\w+) \*", t)
+    if m and m.group(2) in MIRRORS:
+        return "pointer to " + m.group(2)
+    if t.endswith("*") or t == "dba_stream_t":
+        return "pointer"
+    return {"int": "int", "float": "float", "double": "double", "size_t": "size_t", "long long int": "int64", "int64_t": "int64"}[t]
+
+
+def _py_kind(t):
+    for struct, cls in MIRRORS.items():
+        if t is ctypes.POINTER(cls):
+            return "pointer to " + struct
+    return {ctypes.c_void_p: "pointer", ctypes.c_char_p: "const char*", ctypes.c_int: "int", ctypes.c_float: "float",
+            ctypes.c_double: "double", ctypes.c_size_t: "size_t", ctypes.c_longlong: "int64"}[t]
+
+
+def test_capi_prototypes_match_header(tmp_path):
+    """every function of the header has a prototype in c_api with the header's return kind and per-parameter kinds: pointer
+    (dba_stream_t included; a pointer to a mirrored struct must be typed as a pointer to its mirror), int, float, double, size_t, 64-bit
+    integer, const char*.  gcc's -aux-info prints each prototype of the header on one normalised line."""
+    src, aux = tmp_path / "protos.c", tmp_path / "protos.txt"
+    src.write_text('#include "droid_b200.h"\n')
+    subprocess.run(["gcc", "-fsyntax-only", "-I", os.path.dirname(HEADER), "-aux-info", str(aux), str(src)], check=True)
+    header = {}
+    for line in aux.read_text().splitlines():
+        m = re.search(r"droid_b200\.h:\d+:\w+ \*/ extern (.*?)\s*\b(dba_\w+) \((.*)\);$", line)
+        if m:
+            header[m.group(2)] = (m.group(1), [] if m.group(3) == "void" else m.group(3).split(", "))
+    assert len(header) == 57 and set(header) == set(c_api.PROTOTYPES), set(header) ^ set(c_api.PROTOTYPES)
+    bad = []
+    for name, (ret, params) in header.items():
+        restype, argtypes = c_api.PROTOTYPES[name]
+        if _c_kind(ret) != _py_kind(restype):
+            bad.append("%s returns %s (%s), c_api %s" % (name, _c_kind(ret), ret, _py_kind(restype)))
+        if len(params) != len(argtypes):
+            bad.append("%s takes %d parameters, c_api %d" % (name, len(params), len(argtypes)))
+        for i, (p, a) in enumerate(zip(params, argtypes)):
+            if _c_kind(p) != _py_kind(a):
+                bad.append("%s parameter %d: header %s (%s), c_api %s" % (name, i, _c_kind(p), p, _py_kind(a)))
+    assert not bad, bad
+
+
+def test_capi_constants_match_header(tmp_path):
+    names = ("DBA_F32", "DBA_F16", "DBA_F64", "DBA_BF16", "DBA_ENCODER_CONVS")
+    got = _header_probe(tmp_path, ['  printf("%s %%d\\n", %s);' % (n, n) for n in names])
+    assert got == {n: getattr(c_api, n) for n in names}
+
+
+def test_update_weights_mirror_follows_packed_order():
+    """the binding stores the k-th packed weight in the k-th pointer of dba_update_weights, so PACKED_ORDER must be its member order"""
+    from droid_slam_b200.update import PACKED_ORDER
+    assert tuple(f for f, _ in c_api.UpdateWeights._fields_) == PACKED_ORDER
 
 
 def test_capi_argument_validation_without_gpu():

@@ -23,7 +23,6 @@ is 1; the number of cases in brackets).  The forward ratio is bounded below 0.5 
   dense                    0.00065 / 0.36 / 0.49 (3)
 The whole file takes about a minute there.
 """
-import ctypes
 import json
 import os
 
@@ -34,14 +33,11 @@ import torch
 from droid_slam_b200 import c_api
 from test_solve_cpu import (CASES, EPS32, OLD_RANDOM_N, T, cdiv, f32, factor_error, forward_ratio, lapack_solve, make_case,
                             old_random, residual_ratio, route, spectrum)
+from util import ptr, stream
 
 pytestmark = pytest.mark.gpu
 dev = "cuda"
 SENTINEL = np.int64(np.uint64(0xFFF7DEADBEEF5A5A).astype(np.int64))   # the resident kernel's "not written yet" bit pattern
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr())
 
 
 class Solve:
@@ -56,8 +52,8 @@ class Solve:
 
     def launch(self, H, b, lm, ep):
         n = b.shape[0]
-        c_api.check(self.L.dba_solve_spd(_ptr(H), _ptr(b), n, lm, ep, _ptr(self.x), _ptr(self.fail), _ptr(self.ws), self.bytes,
-                                         ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "dba_solve_spd")
+        c_api.check(self.L.dba_solve_spd(ptr(H), ptr(b), n, lm, ep, ptr(self.x), ptr(self.fail), ptr(self.ws), self.bytes, stream()),
+                    "dba_solve_spd")
 
     def __call__(self, H, b, lm, ep):
         """(x [n] fp32 on the host, fail)"""

@@ -1,8 +1,6 @@
 """dba_update_workspace_bytes (host only): unchanged where wd % 8 == 0, where the convolutions keep their rectangular tiles, and large
 enough for the row-flattened tiles' partial-sum slots elsewhere.  The expected values are those of the build before row-flattened
 tiles existed."""
-import ctypes
-
 import pytest
 
 from droid_slam_b200 import c_api
@@ -10,10 +8,7 @@ from droid_slam_b200 import c_api
 
 @pytest.fixture(scope="module")
 def ws_bytes():
-    f = c_api.load().dba_update_workspace_bytes
-    f.restype = ctypes.c_size_t
-    f.argtypes = [ctypes.c_int] * 4
-    return f
+    return c_api.load().dba_update_workspace_bytes
 
 
 @pytest.mark.parametrize("shape,expected", [

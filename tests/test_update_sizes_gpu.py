@@ -124,29 +124,13 @@ def test_channels_last_state_round_trip_at_41x73():
     assert float((o2[0].float().cpu() - r2[0]).abs().max()) < 2e-2
 
 
-class _UpdWeights(ctypes.Structure):
-    _fields_ = [(k, ctypes.c_void_p) for k in PACKED_ORDER]
-
-
-class _UpdArgs(ctypes.Structure):
-    _fields_ = [("n_edges", ctypes.c_int), ("ht", ctypes.c_int), ("wd", ctypes.c_int),
-                ("net", ctypes.c_void_p), ("net_dtype", ctypes.c_int), ("net_layout", ctypes.c_int),
-                ("inp", ctypes.c_void_p), ("inp_dtype", ctypes.c_int), ("corr", ctypes.c_void_p), ("corr_dtype", ctypes.c_int),
-                ("flow", ctypes.c_void_p), ("seg", ctypes.c_void_p), ("n_src", ctypes.c_int), ("weights", ctypes.POINTER(_UpdWeights)),
-                ("net_out", ctypes.c_void_p), ("delta", ctypes.c_void_p), ("weight", ctypes.c_void_p), ("eta", ctypes.c_void_p),
-                ("upmask", ctypes.c_void_p), ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t), ("stream", ctypes.c_void_p)]
-
-
 def test_update_forward_reads_nothing_it_did_not_write_at_43x70():
     """dba_update_forward on a NaN-filled workspace and NaN-filled outputs: every output finite and equal to a call on a zeroed workspace
     (a partial-sum slot or tile that no kernel writes would carry the NaN through)"""
     E, ht, wd, n_src = 6, 43, 70, 3
     L = c_api.load()
-    L.dba_update_workspace_bytes.restype = ctypes.c_size_t
-    L.dba_update_workspace_bytes.argtypes = [ctypes.c_int] * 4
-    L.dba_update_forward.argtypes = [ctypes.POINTER(_UpdArgs)]
     pk = pack_update_weights(synth.make_update_weights(0), DEV)
-    W = _UpdWeights(*[pk[k].data_ptr() for k in PACKED_ORDER])
+    W = c_api.UpdateWeights(*[pk[k].data_ptr() for k in PACKED_ORDER])
     net, inp, corr, flow, ii = synth.make_update_inputs(E=E, ht=ht, wd=wd, seed=5, n_src=n_src)
     net, inp, corr = (t[0].half().contiguous().to(DEV) for t in (net, inp, corr))
     flow = flow[0].contiguous().to(DEV)
@@ -159,8 +143,9 @@ def test_update_forward_reads_nothing_it_did_not_write_at_43x70():
         outs = [torch.full(s, float("nan"), dtype=dt, device=DEV) for s, dt in (((E, ht, wd, 128), torch.float16), ((E, ht, wd, 2), torch.float32),
                                                                                  ((E, ht, wd, 2), torch.float32), ((n_src, ht, wd), torch.float32),
                                                                                  ((n_src, 576, ht, wd), torch.float16))]
-        a = _UpdArgs(E, ht, wd, net.data_ptr(), c_api.DBA_F16, 0, inp.data_ptr(), c_api.DBA_F16, corr.data_ptr(), c_api.DBA_F16, flow.data_ptr(),
-                     seg.data_ptr(), n_src, ctypes.pointer(W), *[o.data_ptr() for o in outs], wsp, nbytes, torch.cuda.current_stream().cuda_stream)
+        a = c_api.UpdateArgs(E, ht, wd, net.data_ptr(), c_api.DBA_F16, 0, inp.data_ptr(), c_api.DBA_F16, corr.data_ptr(), c_api.DBA_F16,
+                             flow.data_ptr(), seg.data_ptr(), n_src, ctypes.pointer(W), *[o.data_ptr() for o in outs], wsp, nbytes,
+                             torch.cuda.current_stream().cuda_stream)
         c_api.check(L.dba_update_forward(ctypes.byref(a)), "update_forward")
         torch.cuda.synchronize()
         return outs

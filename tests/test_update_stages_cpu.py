@@ -498,17 +498,12 @@ SELF_CASES = [
 ]
 
 
-@pytest.fixture(scope="module")
-def lib():
-    return c_api.load()
-
-
 @pytest.mark.parametrize("tanh_sign", [-1, 0, 1])
 @pytest.mark.parametrize("case", SELF_CASES, ids=[c[0] for c in SELF_CASES])
-def test_bounds_accept_the_fp32_restatement(lib, case, tanh_sign):
+def test_bounds_accept_the_fp32_restatement(capi, case, tanh_sign):
     sd, pk = case_weights(case)
     ins = cpu_inputs(case)
-    smap = slot_of_pixel(lib, case[2], case[3])
+    smap = slot_of_pixel(capi, case[2], case[3])
     st, out = restate(pk, ins, smap, tanh_sign)
     res = check_stages(pk, ins, st, out, smap)
     want = {"layout.inp", "corr_encoder.0", "corr_encoder.2", "flow_encoder.0", "flow_encoder.2", "gate_partial", "global_context", "z", "rh",
@@ -521,20 +516,20 @@ def test_bounds_accept_the_fp32_restatement(lib, case, tanh_sign):
 
 
 @pytest.mark.parametrize("fault", sorted(FAULTS))
-def test_bounds_reject_planted_fault(lib, fault):
+def test_bounds_reject_planted_fault(capi, fault):
     case = SELF_CASES[1] if fault == "flow_halo_shift_at_x64" else SELF_CASES[0]
     sd, pk = case_weights(case)
     ins = cpu_inputs(case)
-    smap = slot_of_pixel(lib, case[2], case[3])
+    smap = slot_of_pixel(capi, case[2], case[3])
     st, out = restate(pk, ins, smap, 0, fault)
     with pytest.raises(AssertionError, match="^%s:" % FAULTS[fault].replace(".", r"\.")):
         check_stages(pk, ins, st, out, smap)
 
 
-def test_workspace_layout_matches_the_operator(lib):
+def test_workspace_layout_matches_the_operator(capi):
     for E, n_src, ht, wd in ((6, 3, 48, 64), (5, 0, 41, 73), (512, 72, 48, 64), (1, 1, 1, 1)):
-        offs, slots = workspace_layout(lib, E, n_src, ht, wd)
-        total = lib.dba_update_workspace_bytes(E, n_src, ht, wd)
+        offs, slots = workspace_layout(capi, E, n_src, ht, wd)
+        total = capi.dba_update_workspace_bytes(E, n_src, ht, wd)
         HW = ht * wd
         sizes = dict(hin=E * HW * 256, x320=E * HW * 640, cc=E * HW * 400, f0=E * HW * 400, c1=E * HW * 256, f1=E * HW * 256, z=E * HW * 256,
                      rh=E * HW * 256, s=E * HW * 768, partial=E * slots * 512, glo=E * 384 * 4, am=max(n_src, 1) * HW * 256, b2=max(n_src, 1) * HW * 256)
@@ -544,20 +539,20 @@ def test_workspace_layout_matches_the_operator(lib):
         assert spans[-1][1] <= total and all(v % 256 == 0 for v in offs.values())
         assert offs["yh"] == offs["cc"] and E * HW * 144 <= sizes["cc"]          # the head partials reuse the corr staging buffer
         assert offs["ye"] == offs["f0"] and max(n_src, 1) * HW * 48 <= sizes["f0"]
-        smap, n = slot_of_pixel(lib, ht, wd)
+        smap, n = slot_of_pixel(capi, ht, wd)
         assert n == slots and int(smap.max()) < slots
         assert torch.bincount(smap, minlength=slots).max() <= 16                  # 16 pixels per slot at most
     bad = (ctypes.c_size_t * len(UPWS))()
-    assert lib.dba_update_workspace_layout(0, 1, 8, 8, ctypes.cast(bad, ctypes.c_void_p), ctypes.byref(ctypes.c_int())) == 1
+    assert capi.dba_update_workspace_layout(0, 1, 8, 8, ctypes.cast(bad, ctypes.c_void_p), ctypes.byref(ctypes.c_int())) == 1
 
 
-def test_case_table_covers_every_route(lib):
+def test_case_table_covers_every_route(capi):
     routes, mts, flags = set(), set(), set()
     for name, E, ht, wd, segs, n_src, opt in CASES:
         for cname, c0, c1, ks, n in OPERATOR_CONVS:
             if cname in AGG_CONVS and n_src == 0:
                 continue
-            p = conv_plan(lib, ht, wd, c0, c1, ks, n)
+            p = conv_plan(capi, ht, wd, c0, c1, ks, n)
             routes.add("flat" if p["flat"] else "tw%d" % p["TW"])
             mts.add((p["flat"], p["MT"]))
             if p["n_ntiles"] * (n_src if cname in AGG_CONVS else E) * p["tiles"] > H100_SMS:

@@ -36,7 +36,6 @@ from droid_slam_b200 import c_api
 from droid_slam_b200.update import PACKED_ORDER, UpdateModule
 from test_tensor_core_fp64_cpu import conv_plan
 from test_tensor_core_fp64_gpu import Guarded
-from test_update_sizes_gpu import _UpdArgs, _UpdWeights
 from test_update_stages_cpu import CASE_IDS, CASES, UPWS, case_inputs, case_segments, case_weights, check_stages, slot_of_pixel, workspace_layout
 from util import assert_bit_identical
 
@@ -64,7 +63,7 @@ def run_forward(L, pk, net, inp, corr, flow, seg, n_src, layout):
     E = inp.shape[0]
     ht, wd = inp.shape[2:]
     HW = ht * wd
-    W = _UpdWeights(*[pk[k].data_ptr() for k in PACKED_ORDER])
+    W = c_api.UpdateWeights(*[pk[k].data_ptr() for k in PACKED_ORDER])
     nbytes = L.dba_update_workspace_bytes(E, n_src, ht, wd)
     ws = torch.full((nbytes,), 255, dtype=torch.uint8, device=DEV)             # every f16 and f32 in it NaN
     assert ws.data_ptr() % 256 == 0
@@ -72,9 +71,9 @@ def run_forward(L, pk, net, inp, corr, flow, seg, n_src, layout):
     if n_src:
         g.update(eta=Guarded(n_src, ht, wd, dtype=torch.float32), upmask=Guarded(n_src, 576, ht, wd))
     p = lambda k: g[k].t.data_ptr() if k in g else None
-    a = _UpdArgs(E, ht, wd, net.data_ptr(), DT[net.dtype], layout, inp.data_ptr(), DT[inp.dtype], corr.data_ptr(), DT[corr.dtype],
-                 flow.data_ptr() if flow is not None else None, seg.data_ptr() if seg is not None else None, n_src, ctypes.pointer(W),
-                 p("net_out"), p("delta"), p("weight"), p("eta"), p("upmask"), ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream)
+    a = c_api.UpdateArgs(E, ht, wd, net.data_ptr(), DT[net.dtype], layout, inp.data_ptr(), DT[inp.dtype], corr.data_ptr(), DT[corr.dtype],
+                         flow.data_ptr() if flow is not None else None, seg.data_ptr() if seg is not None else None, n_src, ctypes.pointer(W),
+                         p("net_out"), p("delta"), p("weight"), p("eta"), p("upmask"), ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream)
     c_api.check(L.dba_update_forward(ctypes.byref(a)), "update_forward")
     torch.cuda.synchronize()
     offs, slots = workspace_layout(L, E, n_src, ht, wd)
@@ -115,13 +114,8 @@ def sample_edges(L, E, ht, wd, k):
     return sorted(pick[:max(k, 2)])
 
 
-@pytest.fixture(scope="module")
-def lib():
-    return c_api.load()
-
-
 @pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
-def test_update_stages_match_fp64(lib, case):
+def test_update_stages_match_fp64(capi, case):
     name, E, ht, wd, segs, n_src, opt = case
     sd, pk = case_weights(case)
     pk = {k: v.to(DEV) for k, v in pk.items()}
@@ -131,7 +125,7 @@ def test_update_stages_match_fp64(lib, case):
     layout = opt.get("layout", 0)
     if layout == 1:
         net = net.half().permute(0, 2, 3, 1).contiguous()
-    st, out, guards = run_forward(lib, pk, net, inp, corr, flow, seg, n_src, layout)
+    st, out, guards = run_forward(capi, pk, net, inp, corr, flow, seg, n_src, layout)
     for k, gd in guards.items():
         gd.check_guards("update_forward %s %s" % (name, k))
         assert not bool(torch.isnan(gd.t).any()), "%s: %s keeps a NaN" % (name, k)
@@ -139,9 +133,9 @@ def test_update_stages_match_fp64(lib, case):
         # MotionFilter's call: stems 256 wide, nothing aggregated
         assert bool((st["s"][..., 256:].contiguous().view(torch.int16) == -1).all()), "%s: stems wider than 256 without aggregation" % name
         assert bool((st["am"].contiguous().view(torch.int16) == -1).all()), "%s: segment mean written without aggregation" % name
-    edges = sample_edges(lib, E, ht, wd, opt["sample"]) if opt.get("sample") else None
+    edges = sample_edges(capi, E, ht, wd, opt["sample"]) if opt.get("sample") else None
     ins = dict(net=net, inp=inp, corr=corr, flow=flow, layout=layout, seg=seg, n_src=n_src)
-    res = check_stages(pk, ins, st, out, slot_of_pixel(lib, ht, wd), edges)
+    res = check_stages(pk, ins, st, out, slot_of_pixel(capi, ht, wd), edges)
     _report(name, res)
 
 
@@ -154,7 +148,7 @@ def _dilate(mask, r):
 
 
 @pytest.mark.parametrize("where", ["corr", "net"])
-def test_nan_input_propagates_like_the_reference(lib, where):
+def test_nan_input_propagates_like_the_reference(capi, where):
     """A NaN in corr reaches exactly the pixels whose receptive field holds it (the reference's torch.relu keeps NaN; the encoders'
     ReLU must not turn it into 0); a NaN in net makes its edge's global context NaN, so that edge's outputs and its segment's
     aggregation outputs are NaN everywhere.  Every other output is bit-identical to the call without the NaN."""
@@ -165,13 +159,13 @@ def test_nan_input_propagates_like_the_reference(lib, where):
     seg = seg.to(DEV)
     net, inp, corr, flow = case_inputs(case, device=DEV)
     e, y, x = 2, 7, 33
-    clean = run_forward(lib, pk, net, inp, corr, flow, seg, n_src, 0)[1]
+    clean = run_forward(capi, pk, net, inp, corr, flow, seg, n_src, 0)[1]
     bad_net, bad_corr = net.clone(), corr.clone()
     if where == "corr":
         bad_corr[e, 5, y, x] = float("nan")
     else:
         bad_net[e, 7, y, x] = float("nan")
-    got = run_forward(lib, pk, bad_net, inp, bad_corr, flow, seg, n_src, 0)[1]
+    got = run_forward(capi, pk, bad_net, inp, bad_corr, flow, seg, n_src, 0)[1]
     E, ht, wd = 6, 20, 40
     px = torch.zeros(E, ht, wd, dtype=torch.bool, device=DEV)
     px[e, y, x] = True

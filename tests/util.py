@@ -45,18 +45,8 @@ def c_ba(L, poses, disps, intr, disps_sens, targets, weights, eta, ii, jj, t0, t
         ws.fill_(ws_fill)
     dx = torch.full((t1 - t0, 6), float("nan"), device=poses.device)
     dz = torch.full((M, ht * wd), float("nan"), device=poses.device)
-    a = c_api.BAArgs()
-    a.poses, a.disps, a.intrinsics, a.disps_sens = poses.data_ptr(), disps.data_ptr(), intr.data_ptr(), disps_sens.data_ptr()
-    a.targets, a.weights = targets.data_ptr(), weights.data_ptr()
-    a.eta = eta.data_ptr() if eta is not None else None
-    a.eta_rows = eta.shape[0] if eta is not None else 1
-    a.ii, a.jj = ii.data_ptr(), jj.data_ptr()
-    a.n_frames, a.n_edges, a.ht, a.wd, a.t0, a.t1 = N, E, ht, wd, t0, t1
-    a.lm, a.ep, a.motion_only = lm, ep, int(motion_only)
-    a.dx_out, a.dz_out = dx.data_ptr(), dz.data_ptr()
-    a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
-    a.stream = torch.cuda.current_stream().cuda_stream
-    a.own_lo, a.own_hi, a.eta_by_frame = 0, N, 0
+    a = c_api.ba_args(poses, disps, intr, disps_sens, targets, weights, eta, ii, jj, t0, t1, lm, ep, dx, dz, ws,
+                      torch.cuda.current_stream().cuda_stream, motion_only=motion_only)
     c_api.check(L.dba_ba(ctypes.byref(a), itrs) if itrs > 0 else L.dba_ba_prepare(ctypes.byref(a)), "ba")
     m = ctypes.c_int(0); st = ctypes.c_int(0)
     c_api.check(L.dba_ba_read_info(ctypes.byref(a), ctypes.byref(m), ctypes.byref(st)), "ba_read_info")

@@ -41,17 +41,8 @@ class Call:
         self.ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         self.dx = torch.zeros(max(t1 - t0, 1), 6, device=dev)
         self.dz = torch.zeros(M, ht * wd, device=dev)
-        a = c_api.BAArgs()
-        a.poses, a.disps, a.intrinsics, a.disps_sens = self.poses.data_ptr(), self.disps.data_ptr(), intr.data_ptr(), ds.data_ptr()
-        a.targets, a.weights, a.eta, a.eta_rows = tg.data_ptr(), wt.data_ptr(), eta.data_ptr(), eta.shape[0]
-        a.ii, a.jj = ii.data_ptr(), jj.data_ptr()
-        a.n_frames, a.n_edges, a.ht, a.wd, a.t0, a.t1 = N, E, ht, wd, t0, t1
-        a.lm, a.ep, a.motion_only = s["lm"], s["ep"], 0
-        a.dx_out, a.dz_out = self.dx.data_ptr(), self.dz.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), ws_bytes
-        a.stream = torch.cuda.current_stream().cuda_stream
-        a.own_lo, a.own_hi, a.eta_by_frame = 0, N, 0
-        self.a = a
+        self.a = c_api.ba_args(self.poses, self.disps, intr, ds, tg, wt, eta, ii, jj, t0, t1, s["lm"], s["ep"], self.dx, self.dz, self.ws,
+                               torch.cuda.current_stream().cuda_stream)
         self.shape = "E=%d N=%d %dx%d, %d depth frames, window [%d, %d), %d Gauss-Newton iterations" % (E, N, ht, wd, M, t0, t1, self.itrs)
 
     def stage(self, fn):
