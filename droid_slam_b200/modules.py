@@ -41,8 +41,9 @@ kernel for is offered as a hook:
     and backward on csrc/ba_layer.cu (`droid_backends.ba_layer_forward` / `ba_layer_backward`), so `train.py` trains through it.
 
 The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
-it.  If not, strict=True (the default) raises RuntimeError naming the replaced method and the reason; strict=False runs the reference's
-own method.  `update`, `update_lowmem`, `fill_trajectory` and `track` called directly raise in the same words.
+it.  If not, strict=True (the default) raises RuntimeError naming the replaced method or global and the reason; strict=False runs the
+reference's own function -- the one the first install found, however often the hook is installed again.  `update`, `update_lowmem`,
+`fill_trajectory`, `track`, `ba_layer` and `CorrBlock` called directly raise in the same words.
 """
 import copy
 import importlib
@@ -67,19 +68,30 @@ def _require(entry, why):
         raise RuntimeError("%s has no kernel for this call: %s" % (entry, why))
 
 
-def _replace(cls, name, native, unsupported, strict):
-    """replace the method `name` of the reference's class `cls` by native(self, ...) under the strict policy; unsupported(self, ...)
-    takes the same arguments and gives why the native path cannot run the call (None: it can)"""
-    ref = getattr(cls, name)
+def _original(owner, name):
+    """owner.<name> as the reference defines it: taken on the first call and kept on the owner as _b200_reference_<name>, so that a hook
+    installed again reaches the reference's own function, not the previous install's replacement"""
+    key = "_b200_reference_" + name
+    ref = vars(owner).get(key, getattr(owner, name))
+    setattr(owner, key, ref)
+    return ref
 
-    def method(self, *args, **kwargs):
-        why = unsupported(self, *args, **kwargs)
+
+def _replace(owner, name, native, unsupported, strict):
+    """replace `name` of `owner` -- a method of a reference class, or a global of a reference module -- by native under the strict
+    policy.  unsupported, native and the reference's own function (_original) all take the replacement's arguments, self first for a
+    method; unsupported gives why the native path cannot run the call (None: it can)"""
+    ref = _original(owner, name)
+    entry = "%s.%s" % (owner.__name__, name) if isinstance(owner, type) else name
+
+    def replacement(*args, **kwargs):
+        why = unsupported(*args, **kwargs)
         if why is not None and not strict:
-            return ref(self, *args, **kwargs)
-        _require("%s.%s" % (cls.__name__, name), why)
-        return native(self, *args, **kwargs)
+            return ref(*args, **kwargs)
+        _require(entry, why)
+        return native(*args, **kwargs)
 
-    setattr(cls, name, method)
+    setattr(owner, name, replacement)
 
 
 def _graph_unsupported(who, obj, update, encoders=(), own=(), video=()):
@@ -143,21 +155,31 @@ def _no_grad_inputs(who, *ts):
         raise RuntimeError("the native %s is forward only: an input requires grad" % who)
 
 
-def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
-    """why corr_volume_pyramid has no kernel for these CorrBlock arguments (None: it has one)"""
+def _corr_fmaps_unsupported(fmap1, fmap2, num_levels):
+    """why no CorrBlock kernel, of either dtype, takes these arguments (None: one may): both hooks need [B,N,128,ht,wd] CUDA feature maps
+    of one shape with ht, wd >= 8, and 4 levels"""
     if fmap1.dim() != 5 or fmap2.shape != fmap1.shape:
         return "fmap1 and fmap2 must be [B,N,C,H,W] of one shape"
     if not (fmap1.is_cuda and fmap2.is_cuda):
         return "fmaps are not on a CUDA device"
-    if fmap1.dtype != torch.float16 or fmap2.dtype != torch.float16:
-        return "dtype %s / %s (float16 has a kernel)" % (fmap1.dtype, fmap2.dtype)
     if num_levels != 4:
         return "%d levels (4 has a kernel)" % num_levels
-    batch, num, dim, ht, wd = fmap1.shape
+    dim, ht, wd = fmap1.shape[2:]
     if dim != 128:
         return "%d channels (128 has a kernel)" % dim
     if ht < 8 or wd < 8:
         return "%dx%d feature maps (ht and wd must be at least 8)" % (ht, wd)
+    return None
+
+
+def _corr_volume_unsupported(be, fmap1, fmap2, num_levels):
+    """why corr_volume_pyramid has no kernel for these CorrBlock arguments (None: it has one)"""
+    why = _corr_fmaps_unsupported(fmap1, fmap2, num_levels)
+    if why is not None:
+        return why
+    if fmap1.dtype != torch.float16 or fmap2.dtype != torch.float16:
+        return "dtype %s / %s (float16 has a kernel)" % (fmap1.dtype, fmap2.dtype)
+    dim, ht, wd = fmap1.shape[2:]
     if not be.corr_volume_supported(dim, ht, wd):
         return "no kernel for %dx%d" % (ht, wd)
     return None
@@ -173,7 +195,7 @@ def install_corr_volume_hook(corr_module, strict=True, fused_lookup=False):
     under grad mode raise, whichever constructor would run (install_corr_training_hook is the differentiable block)."""
     be = install()
     cls = corr_module.CorrBlock
-    ref_call = cls.__call__
+    ref_call = _original(cls, "__call__")
 
     def __init__(self, fmap1, fmap2, num_levels=4, radius=3):
         batch, num, dim, ht, wd = fmap1.shape
@@ -230,7 +252,7 @@ def install_alt_corr_hook(corr_module, strict=True):
     would otherwise drop their gradients)."""
     be = install()
     cls = corr_module.AltCorrBlock
-    ref_call = cls.__call__
+    ref_call = _original(cls, "__call__")
 
     def __init__(self, fmaps, num_levels=4, radius=3):
         self.num_levels, self.radius = num_levels, radius
@@ -289,8 +311,7 @@ def install_encoder_hook(extractor_module, strict=True):
     be = install()
 
     def forward(self, x):
-        if torch.is_grad_enabled() and x.requires_grad:
-            raise RuntimeError("the native BasicEncoder is forward only: the input requires grad")
+        _no_grad_inputs("BasicEncoder", x)
         b, n, c, h, w = x.shape
         out = be.encoder_forward(x.reshape(b * n, c, h, w).contiguous(), _packed_encoder(self, x.device), 1 if self.norm_fn == "instance" else 0,
                                  self.conv2.out_channels)
@@ -1100,17 +1121,7 @@ def install_ba_layer_hook(droid_net_module, strict=True):
     iteration in DroidNet.forward) to the native layer (`ba_layer`), forward and backward.  A call the layer cannot run (poses not SE3,
     tensors not CUDA float32, rig != 1, fixedp outside [0, N), intrinsics requiring grad, more than BA_LAYER_MAX_POSES pose unknowns)
     raises under strict=True and runs the reference's BA under strict=False."""
-    ref = getattr(droid_net_module, "_b200_reference_BA", None) or droid_net_module.BA
-
-    def BA(*args, **kwargs):
-        why = _ba_layer_unsupported(*args, **kwargs)
-        if why is not None and not strict:
-            return ref(*args, **kwargs)
-        _require("BA", why)
-        return ba_layer(*args, **kwargs)
-
-    droid_net_module._b200_reference_BA = ref
-    droid_net_module.BA = BA
+    _replace(droid_net_module, "BA", ba_layer, _ba_layer_unsupported, strict)
     _record("install_ba_layer_hook", droid_net_module, strict=strict)
     return droid_net_module
 
@@ -1171,21 +1182,14 @@ class _CorrLookup(torch.autograd.Function):
 
 def _corr_training_unsupported(fmap1, fmap2, num_levels=4, radius=3):
     """why the native training CorrBlock cannot run these arguments (None: it can)"""
-    if fmap1.dim() != 5 or fmap2.shape != fmap1.shape:
-        return "fmap1 and fmap2 must be [B,N,C,H,W] of one shape"
-    if not (fmap1.is_cuda and fmap2.is_cuda):
-        return "fmaps are not on a CUDA device"
+    why = _corr_fmaps_unsupported(fmap1, fmap2, num_levels)
+    if why is not None:
+        return why
     if fmap1.dtype != torch.float32 or fmap2.dtype != torch.float32:
         return "dtype %s / %s (float32 has a kernel)" % (fmap1.dtype, fmap2.dtype)
-    if num_levels != 4:
-        return "%d levels (4 has a kernel)" % num_levels
     if radius != 3:
         return "radius %d (3 has a kernel)" % radius
-    batch, num, dim, ht, wd = fmap1.shape
-    if dim != 128:
-        return "%d channels (128 has a kernel)" % dim
-    if ht < 8 or wd < 8:
-        return "%dx%d feature maps (ht and wd must be at least 8)" % (ht, wd)
+    batch, num = fmap1.shape[:2]
     if batch * num > 65535:
         return "%d edges (at most 65535)" % (batch * num)
     return None
@@ -1227,16 +1231,6 @@ def install_corr_training_hook(droid_net_module, strict=True):
     A block it cannot build (not fp32 CUDA [B,N,128,ht,wd] maps with ht, wd >= 8, num_levels != 4, radius != 3; f16 / autocast training
     among them) raises under strict=True and builds the reference's CorrBlock under strict=False.  modules.corr.CorrBlock, which the
     frontend, the factor graph and the motion filter use, is not touched."""
-    ref = getattr(droid_net_module, "_b200_reference_CorrBlock", None) or droid_net_module.CorrBlock
-
-    def make(fmap1, fmap2, num_levels=4, radius=3):
-        why = _corr_training_unsupported(fmap1, fmap2, num_levels, radius)
-        if why is not None and not strict:
-            return ref(fmap1, fmap2, num_levels=num_levels, radius=radius)
-        _require("CorrBlock", why)
-        return CorrBlock(fmap1, fmap2, num_levels, radius)
-
-    droid_net_module._b200_reference_CorrBlock = ref
-    droid_net_module.CorrBlock = make
+    _replace(droid_net_module, "CorrBlock", CorrBlock, _corr_training_unsupported, strict)
     _record("install_corr_training_hook", droid_net_module, strict=strict)
     return droid_net_module
