@@ -9,13 +9,9 @@
   * reanchor: the re-anchoring of droid_async.py:87, :94-96 (dG composed with the frontend's poses whose translations were scaled by s
     in fp32), composed in fp64 and rounded once (what dba_fragment_handover computes).
 """
-import os
-import sys
-
 import torch
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims"))
-from lietorch import SE3  # noqa: E402
+from .shims.lietorch import SE3
 
 BUFFERS = ("poses", "disps", "disps_sens", "images", "tstamp", "intrinsics", "fmaps", "nets", "inps")
 

@@ -12,15 +12,9 @@ dL = g . d for Y -> Exp(d) Y.  Tangent and point inputs get Euclidean gradients.
   * broadcasting is the stand-in's expand, so autograd sums a broadcast operand's gradient.
 `closed_grad` restates the closed forms of lietorch's backward kernels (tests/test_lietorch_cpu.py holds the two equal to 1e-12).
 `right` / `transposed`: planted wrong conventions the test must reject."""
-import importlib.util
-import os
-
 import torch
 
-_SHIM = os.path.join(os.path.dirname(os.path.abspath(__file__)), "shims", "lietorch", "__init__.py")
-_spec = importlib.util.spec_from_file_location("oracle_lietorch_shim", _SHIM)
-shim = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(shim)
+from .shims import lietorch as shim
 
 OPS = ("exp", "log", "inv", "mul", "adj", "adjT", "act", "act4", "vec", "fromvec")
 GROUP_OUT = ("exp", "inv", "mul", "fromvec")

@@ -1,9 +1,9 @@
 """Pure-PyTorch stand-in for the `lietorch` package (SE3 group) -- TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
 The reference's Python call sites on the path (`droid_slam/depth_video.py`, `geom/projective_ops.py`, `geom/ba.py`, `droid_net.py`)
-import `lietorch`, a CUDA extension that cannot be built here (it needs the absent Eigen submodule).  With this directory on
-`sys.path` those files import UNMODIFIED, which is how `oracle.reproject` (row A5) is pinned against
-`pops.projective_transform` itself and how the reference's `geom/ba.py` cross-checks the BA oracle.
+import `lietorch`, a CUDA extension that cannot be built here (it needs the absent Eigen submodule).  With this package in
+sys.modules as `lietorch` (tests/golden/reference.py) those files import UNMODIFIED, which is how `oracle.reproject` (row A5) is
+pinned against `pops.projective_transform` itself and how the reference's `geom/ba.py` cross-checks the BA oracle.
 
 Restates the arithmetic of thirdparty/lietorch/lietorch/include/so3.h and se3.h (file:line cited per function) and the Python
 wrapper thirdparty/lietorch/lietorch/groups.py:51-231,265-285 (broadcasting per broadcasting.py:9-31).  Data layout

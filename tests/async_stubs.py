@@ -9,7 +9,6 @@ buffers are) with counter / ready as multiprocessing Values.  DroidAsyncBackend 
 iteration count and whether the network's update operator is the native one; it runs no BA (BA is not bit-reproducible on large graphs,
 DESIGN §5, so the tests compare the hand-over).  Built from seeds with synth and the lietorch stand-in; the reference tree is not read."""
 import multiprocessing
-import os
 import sys
 from collections import OrderedDict
 
@@ -17,9 +16,7 @@ import torch
 
 import droid_slam_b200
 from droid_slam_b200 import modules, synth
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "shims"))
-from lietorch import SE3  # noqa: E402
+from oracle.shims.lietorch import SE3
 
 
 class CorrBlock:

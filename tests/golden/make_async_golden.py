@@ -16,8 +16,6 @@ fragment is the backend's one seen through a random Sim(3) with noise, as when t
 inputs, the alignment in fp32 and fp64, the back buffers after the pass and the stubs' records.
 tests/test_async_cpu.py holds oracle/async_backend.py to them.
 """
-import contextlib
-import importlib
 import os
 import sys
 import threading
@@ -29,7 +27,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-from make_proximity_golden import REF  # noqa: E402
+from oracle.shims.lietorch import SE3  # noqa: E402
+from reference import reference_modules  # noqa: E402
 
 BUFFER, HT, WD, T1 = 40, 4, 6, 36
 BUFFERS = ("poses", "disps", "disps_sens", "images", "tstamp", "intrinsics", "fmaps", "nets", "inps")
@@ -40,16 +39,9 @@ def cases():
     return [("mono", 28, False, False, 0), ("rgbd", 28, False, True, 1), ("stereo", 28, True, False, 2), ("t0_zero", 0, False, False, 3)]
 
 
-def _se3():
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
-    from lietorch import SE3
-    return SE3
-
-
 def videos(case):
     """(front, back) dicts of the BUFFERS on the CPU for one case"""
     name, t0, stereo, rgbd, seed = case
-    SE3 = _se3()
     g = torch.Generator().manual_seed(seed)
     cams = 2 if stereo else 1
 
@@ -101,26 +93,15 @@ class Video(types.SimpleNamespace):
         return self.counter.get_lock()
 
 
-@contextlib.contextmanager
-def reference_modules():
-    """droid_async and align imported unmodified on the lietorch stand-in; the other modules droid_async.py imports are empty stand-ins"""
-    before = set(sys.modules)
-    path_before = list(sys.path)
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
-    sys.path.insert(0, os.path.join(REF, "droid_slam"))
-    stand_ins = {"droid_net": "DroidNet", "depth_video": "DepthVideo", "motion_filter": "MotionFilter", "droid_frontend": "DroidFrontend",
-                 "droid_backend": "DroidAsyncBackend", "trajectory_filler": "PoseTrajectoryFiller"}
-    for name, cls in stand_ins.items():
-        m = types.ModuleType(name)
-        setattr(m, cls, type(cls, (), {}))
-        sys.modules[name] = m
-    try:
-        yield importlib.import_module("droid_async"), importlib.import_module("align")
-    finally:
-        for name in set(sys.modules) - before:
-            if name in stand_ins or name in ("droid_async", "align"):
-                sys.modules.pop(name, None)
-        sys.path[:] = path_before
+def import_reference():
+    """(droid_async, align) imported unmodified; the modules droid_async.py imports but backend_process does not use are empty stand-ins"""
+    stubs = {}
+    for name, cls in (("droid_net", "DroidNet"), ("depth_video", "DepthVideo"), ("motion_filter", "MotionFilter"),
+                      ("droid_frontend", "DroidFrontend"), ("droid_backend", "DroidAsyncBackend"), ("trajectory_filler", "PoseTrajectoryFiller")):
+        stubs[name] = types.ModuleType(name)
+        setattr(stubs[name], cls, type(cls, (), {}))
+    with reference_modules("droid_async", "align", stubs=stubs) as modules:
+        return modules
 
 
 def run_backend_process(droid_async, case, front, back):
@@ -153,18 +134,18 @@ def run_backend_process(droid_async, case, front, back):
 
 def main():
     out = {}
-    with reference_modules() as (droid_async, align):
-        for case in cases():
-            name, t0, stereo, rgbd, seed = case
-            front, back = videos(case)
-            entry = {"case": case, "front": front, "back": back, "t1": T1}
-            if t0 > 0:
-                for dt, tag in ((torch.float32, "fp32"), (torch.float64, "fp64")):
-                    dG, s = align.align_pose_fragements(front["poses"][t0 - 10:t0 - 1].to(dt), back["poses"][t0 - 10:t0 - 1].to(dt))
-                    entry["align_" + tag] = (dG.data.clone(), s.clone())
-            entry["after"], entry["record"] = run_backend_process(droid_async, case, front, back)
-            out[name] = entry
-            print(name, "s(fp64) =", float(entry["align_fp64"][1]) if t0 > 0 else 1.0, entry["record"])
+    droid_async, align = import_reference()
+    for case in cases():
+        name, t0, stereo, rgbd, seed = case
+        front, back = videos(case)
+        entry = {"case": case, "front": front, "back": back, "t1": T1}
+        if t0 > 0:
+            for dt, tag in ((torch.float32, "fp32"), (torch.float64, "fp64")):
+                dG, s = align.align_pose_fragements(front["poses"][t0 - 10:t0 - 1].to(dt), back["poses"][t0 - 10:t0 - 1].to(dt))
+                entry["align_" + tag] = (dG.data.clone(), s.clone())
+        entry["after"], entry["record"] = run_backend_process(droid_async, case, front, back)
+        out[name] = entry
+        print(name, "s(fp64) =", float(entry["align_fp64"][1]) if t0 > 0 else 1.0, entry["record"])
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "async_backend.pt")
     torch.save(out, path)
     print("wrote", path)

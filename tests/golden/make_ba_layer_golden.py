@@ -3,13 +3,12 @@
     python tests/golden/make_ba_layer_golden.py        -> tests/golden/ba_layer.pt
 
 droid_slam/geom/ba.py BA, with geom/chol.py and geom/projective_ops.py, on the lietorch / torch_scatter stand-ins (oracle/shims), with
-projective_ops.py's `torch.as_tensor(..., device="cuda")` served on the CPU (make_reference_python_golden.import_reference).  The default
+projective_ops.py's `torch.as_tensor(..., device="cuda")` served on the CPU (reference.cuda_on_cpu).  The default
 dtype is fp64 while it runs, so that constant lands in the inputs' dtype.  Per case (tests/ba_layer_cases.py: inputs regenerated from
 seeds, only outputs stored): the outputs of every chained call and the gradients of target, weight, eta, poses (lietorch's left-tangent
 gradient, through poses = Exp(eps) X to first order: oracle.ba_layer.left_perturbed) and disps of loss = sum(a * log(poses')) + sum(b * disps') over the calls.
 """
 import contextlib
-import importlib
 import io
 import os
 import sys
@@ -24,17 +23,16 @@ sys.path.insert(0, HERE)
 
 from ba_layer_cases import cases, loss_weights  # noqa: E402
 from oracle.ba_layer import left_perturbed  # noqa: E402
+from oracle.shims.lietorch import SE3  # noqa: E402
+from reference import cuda_on_cpu, reference_modules  # noqa: E402
 
 NAMES = ("target", "weight", "eta", "poses", "disps")
 
 
 def import_reference_ba():
     """the reference's geom/ba.py BA function, on the stand-ins"""
-    import make_reference_python_golden as mg
-    pops, _ = mg.import_reference()
-    ba = importlib.import_module("geom.ba")
-    ba.pops = pops
-    return ba.BA
+    with reference_modules("geom.ba") as (ba,):
+        return ba.BA
 
 
 def run(BA, SE3, c):
@@ -56,11 +54,11 @@ def run(BA, SE3, c):
 
 def generate():
     BA = import_reference_ba()
-    import lietorch as shim_lietorch                             # oracle/shims, on sys.path after import_reference
     dt = torch.get_default_dtype()
     torch.set_default_dtype(torch.float64)
     try:
-        return {name: run(BA, shim_lietorch.SE3, c) for name, c in cases().items()}
+        with cuda_on_cpu():
+            return {name: run(BA, SE3, c) for name, c in cases().items()}
     finally:
         torch.set_default_dtype(dt)
 

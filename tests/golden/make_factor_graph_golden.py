@@ -21,7 +21,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import oracle  # noqa: E402
 from droid_slam_b200 import synth  # noqa: E402
-from make_proximity_golden import REF, import_reference_factor_graph  # noqa: E402,F401
+from make_proximity_golden import import_reference_factor_graph  # noqa: E402,F401
 
 HT, WD, CH = 16, 18, 128        # the smallest maps the reference's 4-level pyramids take (its last avg_pool2d needs 2 rows)
 DIGESTED = ("net", "disps_up")

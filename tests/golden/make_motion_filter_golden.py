@@ -15,8 +15,6 @@ the first counter slots of tstamp, images, poses, disps, disps_sens, intrinsics,
 their bytes, which is equal exactly when the tensors are bit-identical.
 tests/test_motion_filter_cpu.py holds oracle/motion_filter.py to them.
 """
-import contextlib
-import importlib
 import math
 import os
 import sys
@@ -30,8 +28,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import oracle.encoder as oenc  # noqa: E402
 from droid_slam_b200 import synth  # noqa: E402
-from make_proximity_golden import REF  # noqa: E402
 import make_factor_graph_golden as mk  # noqa: E402
+from reference import cuda_on_cpu, reference_modules  # noqa: E402
 
 HT, WD = mk.HT, mk.WD          # feature maps; frames 8x that
 BUFFER = 16
@@ -127,41 +125,12 @@ class CorrBlock(mk.CorrBlock):
         super().__init__(fmap1.float(), fmap2.float())
 
 
-@contextlib.contextmanager
-def _cuda_is_cpu():
-    """`.cuda()` in track and in the video's setter -> the CPU, for the duration of the reference call only"""
-    cuda = torch.Tensor.cuda
-    torch.Tensor.cuda = lambda self, *a, **k: self
-    try:
-        yield
-    finally:
-        torch.Tensor.cuda = cuda
-
-
 def import_reference():
     """the reference's motion_filter and depth_video modules, imported unmodified on stubs; the filter's CorrBlock is the stand-in"""
-    path_before = list(sys.path)
-    before = set(sys.modules)
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
-    sys.path.insert(0, os.path.join(REF, "droid_slam"))
     stubs = {"droid_net": types.SimpleNamespace(DroidNet=None, cvx_upsample=None), "droid_backends": types.ModuleType("droid_backends")}
-    saved = {k: sys.modules.get(k) for k in stubs}
-    sys.modules.update(stubs)
-    try:
-        mf = importlib.import_module("motion_filter")
-        dv = importlib.import_module("depth_video")
-    finally:
-        for name in set(sys.modules) - before:
-            if name.split(".")[0] in ("motion_filter", "depth_video", "geom", "modules"):
-                sys.modules.pop(name, None)
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
-        sys.path[:] = path_before
-    mf.CorrBlock = CorrBlock
-    return mf, dv
+    with reference_modules("motion_filter", "depth_video", stubs=stubs) as (mf, dv):
+        mf.CorrBlock = CorrBlock
+        return mf, dv
 
 
 def run_reference(mf, dv, case, thresh):
@@ -181,7 +150,7 @@ def run_reference(mf, dv, case, thresh):
 
     f.update = recording
     rows = []
-    with _cuda_is_cpu(), torch.no_grad():
+    with cuda_on_cpu(), torch.no_grad():
         for tstamp, image, depth, intr in stream(case):
             n_before, n_stats = f.video.counter.value, len(stats)
             f.track(tstamp, image, depth, intr)

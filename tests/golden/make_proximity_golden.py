@@ -8,7 +8,7 @@ and records what it passes to `add_factors`.  Substituted for the import only: l
 factor_graph.py imports pyplot and never uses it on this path), droid_backends (not called by this method).  Inputs are regenerated
 from seeds by `cases()`; only the emitted edge lists are stored.
 """
-import importlib
+import importlib.util
 import os
 import sys
 import types
@@ -17,7 +17,9 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("DROID_REFERENCE_ROOT", "/root/reference")
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+
+from reference import reference_modules  # noqa: E402
 
 
 def distance_matrix(t0, t1, t, seed, spread=6.0, far=0.05, nan=0):
@@ -68,31 +70,13 @@ def cases():
 
 
 def import_reference_factor_graph():
-    before = set(sys.modules)
-    path_before = list(sys.path)
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
-    sys.path.insert(0, os.path.join(REF, "droid_slam"))
-    added = []
-    for name in ("matplotlib", "matplotlib.pyplot", "droid_backends"):
-        if name not in sys.modules:
-            try:
-                importlib.import_module(name)
-            except Exception:
-                sys.modules[name] = types.ModuleType(name)
-                added.append(name)
-    if "matplotlib" in added:
-        sys.modules["matplotlib"].pyplot = sys.modules["matplotlib.pyplot"]
-    try:
-        fg = importlib.import_module("factor_graph")
-    finally:
-        # leave no trace: the reference modules imported here were bound to the empty stubs and must not be found by later importers
-        for name in set(sys.modules) - before:
-            if name.split(".")[0] in ("factor_graph", "geom", "modules", "cuda_timer", "matplotlib", "droid_backends"):
-                sys.modules.pop(name, None)
-        for name in added:
-            sys.modules.pop(name, None)
-        sys.path[:] = path_before
-    return fg
+    """the reference's factor_graph module, imported unmodified"""
+    stubs = {"droid_backends": types.ModuleType("droid_backends")}
+    if importlib.util.find_spec("matplotlib") is None:
+        stubs["matplotlib"] = types.ModuleType("matplotlib")
+        stubs["matplotlib.pyplot"] = stubs["matplotlib"].pyplot = types.ModuleType("matplotlib.pyplot")
+    with reference_modules("factor_graph", stubs=stubs) as (fg,):
+        return fg
 
 
 class _Counter:

@@ -13,7 +13,6 @@ modules/corr.py runs on CPU tensors, and `torch.as_tensor(..., device="cuda")` i
 is served on the CPU.  Every line of the reference files themselves executes as written.  Inputs are regenerated from seeds
 (tests/golden/cases.py, droid_slam_b200/synth.py); only outputs are stored.
 """
-import importlib
 import hashlib
 import os
 import sys
@@ -23,43 +22,21 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("DROID_REFERENCE_ROOT", "/root/reference")
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-
-class _TorchOnCpu:
-    """`torch` as seen by projective_ops.py: as_tensor(..., device="cuda") lands on the CPU, everything else is torch"""
-
-    def __getattr__(self, name):
-        return getattr(torch, name)
-
-    @staticmethod
-    def as_tensor(data, **kw):
-        kw.pop("device", None)
-        return torch.as_tensor(data, **kw)
+from reference import cuda_on_cpu, reference_modules  # noqa: E402
 
 
 def import_reference():
     """returns (pops, corr_module) = the reference's geom/projective_ops.py and modules/corr.py, imported unmodified"""
     import oracle
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
     stub = types.ModuleType("droid_backends")
     stub.corr_index_forward = lambda v, c, r: oracle.corr_index_forward(v, c.contiguous(), r)
     stub.corr_index_backward = lambda v, c, g, r: oracle.corr_index_backward(v, c.contiguous(), g, r)
     stub.altcorr_forward = lambda f1, f2, c, ii, jj, r: oracle.altcorr_forward(f1, f2, c, ii, jj, r)
     stub.altcorr_backward = lambda f1, f2, c, g, ii, jj, r: oracle.altcorr_backward(f1, f2, c, g, ii, jj, r)
-    saved = sys.modules.get("droid_backends")
-    sys.modules["droid_backends"] = stub
-    sys.path.insert(0, os.path.join(REF, "droid_slam"))
-    try:
-        pops = importlib.import_module("geom.projective_ops")
-        corr = importlib.import_module("modules.corr")
-    finally:
-        if saved is not None:
-            sys.modules["droid_backends"] = saved
-        else:
-            del sys.modules["droid_backends"]
-    pops.torch = _TorchOnCpu()
-    return pops, corr
+    with reference_modules("geom.projective_ops", "modules.corr", stubs={"droid_backends": stub}) as (pops, corr):
+        return pops, corr
 
 
 def reproject_cases():
@@ -100,9 +77,9 @@ def digest(t):
 
 def main(out_path):
     pops, corr = import_reference()
-    from lietorch import SE3
+    from oracle.shims.lietorch import SE3
     G = {}
-    with torch.no_grad():
+    with torch.no_grad(), cuda_on_cpu():
         for name, poses, disps, intr, ii, jj in reproject_cases():
             coords, valid = pops.projective_transform(SE3(poses[None]), disps[None], intr[None], ii, jj)
             G["reproject_%s_coords" % name] = coords.clone()

@@ -11,8 +11,6 @@ written on CPU stand-ins of CorrBlock (oracle.corr, with `cat`), DepthVideo.repr
 to the CPU.  Only the results are stored: per case the returned poses, every batch's graph edges (ii, jj) as `update` sees them, and
 the video's poses / tstamps / counter afterwards.  tests/test_trajectory_filler_cpu.py holds oracle/trajectory_filler.py to them.
 """
-import contextlib
-import importlib
 import os
 import sys
 import types
@@ -26,8 +24,9 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import oracle  # noqa: E402
 import oracle.encoder as oenc  # noqa: E402
 from droid_slam_b200 import synth  # noqa: E402
-from make_proximity_golden import REF, import_reference_factor_graph  # noqa: E402
+from make_proximity_golden import import_reference_factor_graph  # noqa: E402
 import make_factor_graph_golden as mk  # noqa: E402
+from reference import cuda_on_cpu, reference_modules  # noqa: E402
 
 HT, WD = mk.HT, mk.WD
 BUFFER = 48
@@ -116,45 +115,12 @@ def stream(seed, video, stamps):
     return [(t, torch.randint(0, 255, (1, 3, 8 * HT, 8 * WD), generator=g, dtype=torch.uint8), intr.clone()) for t in stamps]
 
 
-@contextlib.contextmanager
-def _cuda_is_cpu():
-    """`__fill`'s hard-coded "cuda" -> the CPU, for the duration of the reference call only"""
-    cuda, as_tensor = torch.Tensor.cuda, torch.as_tensor
-
-    def _as_tensor(data, dtype=None, device=None):
-        return as_tensor(data, dtype=dtype, device="cpu" if device is not None and str(device).startswith("cuda") else device)
-
-    torch.Tensor.cuda = lambda self, *a, **k: self
-    torch.as_tensor = _as_tensor
-    try:
-        yield
-    finally:
-        torch.Tensor.cuda, torch.as_tensor = cuda, as_tensor
-
-
 def import_reference_trajectory_filler():
     """the reference's trajectory_filler module; its FactorGraph is the unmodified class of factor_graph.py (CorrBlock -> the stand-in)"""
     fg = import_reference_factor_graph()
     fg.CorrBlock = CorrBlock
-    path_before = list(sys.path)
-    before = set(sys.modules)
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
-    sys.path.insert(0, os.path.join(REF, "droid_slam"))
-    stubs = {"factor_graph": fg, "droid_net": types.SimpleNamespace(DroidNet=None)}
-    saved = {k: sys.modules.get(k) for k in stubs}
-    sys.modules.update(stubs)
-    try:
-        tf = importlib.import_module("trajectory_filler")
-    finally:
-        for name in set(sys.modules) - before:
-            if name.split(".")[0] in ("trajectory_filler", "geom", "modules", "cuda_timer"):
-                sys.modules.pop(name, None)
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
-        sys.path[:] = path_before
+    with reference_modules("trajectory_filler", stubs={"factor_graph": fg, "droid_net": types.SimpleNamespace(DroidNet=None)}) as (tf,):
+        pass
 
     class FactorGraph(fg.FactorGraph):
         def __init__(self, video, update_op):
@@ -175,7 +141,7 @@ def run_reference(tf, edges_log, case, seed=0):
     f = object.__new__(tf.PoseTrajectoryFiller)
     f.cnet, f.fnet, f.update, f.count, f.video, f.device, f.MEAN, f.STDV = None, fnet, update, 0, video, "cpu", mean, stdv
     edges_log.clear()
-    with _cuda_is_cpu():
+    with cuda_on_cpu():
         out = tf.PoseTrajectoryFiller.__call__(f, stream(seed, video, stamps))
     edges = []
     for k in range(0, len(edges_log), 6):           # six updates per batch see the same edges

@@ -2,11 +2,11 @@
 
     python tests/golden/make_update_golden.py            -> tests/golden/update_module.pt
 
-`droid_slam/droid_net.py` is imported unmodified from /root/reference.  Two of its imports are absent here and are stubbed before the
-import: `lietorch` (unused by UpdateModule) and `torch_scatter` (its `scatter_mean(src, index, dim=1)` is replaced by an index_add
-mean with the documented semantics: out[:, k] = mean of src[:, e] over e with index[e] == k).  Everything UpdateModule.forward
-executes besides that one call -- the 19 convolutions, the GRU gating, GradientClip, Softplus, views and permutes -- is the
-reference's own code.  Weights and inputs are regenerated from seeds (droid_slam_b200/synth.py); only outputs are stored.
+`droid_slam/droid_net.py` is imported unmodified from /root/reference on the stand-ins of oracle/shims (tests/golden/reference.py):
+`lietorch` (unused by UpdateModule) and `torch_scatter` (its `scatter_mean` with the documented semantics: out[:, k] = mean of
+src[:, e] over e with index[e] == k); `droid_backends`, which modules/corr.py imports, is an empty module.  Everything
+UpdateModule.forward executes besides that one call -- the 19 convolutions, the GRU gating, GradientClip, Softplus, views and
+permutes -- is the reference's own code.  Weights and inputs are regenerated from seeds (droid_slam_b200/synth.py); only outputs are stored.
 """
 import os
 import sys
@@ -16,26 +16,15 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("DROID_REFERENCE_ROOT", "/root/reference")
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+
+from reference import reference_modules  # noqa: E402
 
 
-def _stub_missing_packages():
-    lt = types.ModuleType("lietorch")
-    lt.SE3 = lt.SO3 = lt.Sim3 = type("SE3", (), {})
-    sys.modules.setdefault("lietorch", lt)
-    ts = types.ModuleType("torch_scatter")
-
-    def scatter_mean(src, index, dim=1):
-        assert dim == 1
-        n = int(index.max()) + 1
-        out = torch.zeros((src.shape[0], n) + tuple(src.shape[2:]), dtype=src.dtype)
-        out.index_add_(1, index, src)
-        cnt = torch.bincount(index, minlength=n).to(src.dtype)
-        return out / cnt.view(1, -1, *([1] * (src.dim() - 2)))
-
-    ts.scatter_mean = scatter_mean
-    ts.scatter_sum = lambda *a, **k: (_ for _ in ()).throw(NotImplementedError("not on the UpdateModule path"))   # imported by geom/ba.py only
-    sys.modules.setdefault("torch_scatter", ts)
+def import_reference():
+    """the reference's droid_net module, imported unmodified; `import droid_backends` in modules/corr.py finds an empty stub"""
+    with reference_modules("droid_net", stubs={"droid_backends": types.ModuleType("droid_backends")}) as (droid_net,):
+        return droid_net
 
 
 def upmask_sample_index(n):
@@ -44,11 +33,7 @@ def upmask_sample_index(n):
 
 def main(out_path):
     from droid_slam_b200 import synth
-    _stub_missing_packages()
-    import droid_slam_b200
-    droid_slam_b200.install()                                          # `import droid_backends` in modules/corr.py resolves to the drop-in
-    sys.path.insert(0, os.path.join(REF, "droid_slam"))
-    import droid_net                                                   # the reference file, unmodified
+    droid_net = import_reference()
     torch.manual_seed(0)
     mod = droid_net.UpdateModule().eval()
     w = synth.make_update_weights(0)

@@ -15,9 +15,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 from ba_layer_cases import cases, domain_cases  # noqa: E402
 from oracle import ba_layer as oba  # noqa: E402
+import reference  # noqa: E402
 
 GOLDEN = os.path.join(ROOT, "tests", "golden", "ba_layer.pt")
-REF = os.environ.get("DROID_REFERENCE_ROOT", "/root/reference")
 
 
 def _golden():
@@ -45,7 +45,7 @@ def test_indefinite_case_fails_and_keeps_only_the_dz_path():
     assert all(float(g.abs().max()) > 0 for g in (gold[2], gold[3], gold[4], gold[6]))
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "droid_slam", "geom")), reason="the reference's sources are not present")
+@pytest.mark.skipif(not reference.present("droid_slam", "geom"), reason="the reference's sources are not present")
 def test_fixture_reproduces_from_the_reference():
     import make_ba_layer_golden as mk
     now, gold = mk.generate(), _golden()

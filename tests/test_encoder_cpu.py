@@ -1,8 +1,8 @@
 """CPU checks of the native feature / context encoders: the fp32 oracle against the reference's own outputs (tests/golden/encoder.pt),
 the packed weight layout of pack_encoder_weights (gather K order included) against F.conv2d, the hook's strict / fallback selection and
 grad guard, and the C-ABI symbols."""
-import importlib.util
 import os
+import sys
 import types
 
 import pytest
@@ -14,7 +14,8 @@ from droid_slam_b200 import c_api, synth
 from droid_slam_b200.encoder import ENCODER_CONVS, pack_encoder_weights
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_EXTRACTOR = os.path.join(os.environ.get("DROID_REFERENCE_ROOT", "/root/reference"), "droid_slam", "modules", "extractor.py")
+sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+import reference  # noqa: E402
 
 
 def test_oracle_matches_reference_golden():
@@ -104,11 +105,9 @@ def test_pack_rejects_encoders_without_kernel():
 def _extractor_module():
     """the reference's modules.extractor where the reference tree exists, else a namespace around a subclass of the oracle's stand-in;
     either way a fresh class, so patching it leaves other tests alone"""
-    if os.path.exists(REF_EXTRACTOR):
-        spec = importlib.util.spec_from_file_location("ref_extractor_hooktest", REF_EXTRACTOR)
-        m = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(m)
-        return m
+    if reference.present("droid_slam", "modules", "extractor.py"):
+        with reference.reference_modules("modules.extractor") as (m,):
+            return m
     return types.SimpleNamespace(BasicEncoder=type("BasicEncoder", (oenc.BasicEncoder,), {}))
 
 

@@ -13,8 +13,9 @@ from droid_slam_b200.modules import plan_lowmem_chunks
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import make_factor_graph_golden as mk  # noqa: E402
+import reference  # noqa: E402
 
-REF_PRESENT = os.path.isdir(os.path.join(mk.REF, "droid_slam"))
+REF_PRESENT = reference.present("droid_slam")
 CASES = {c[0]: c for c in mk.cases()}
 
 

@@ -96,11 +96,9 @@ def test_package_on_the_cpu():
 
 @contextlib.contextmanager
 def registered_state():
-    """sys.modules' lietorch / torch_scatter and the hook registry restored after the block (other test modules import the stand-ins)"""
+    """sys.modules' lietorch / torch_scatter and the hook registry restored after the block (install_dependencies registers both)"""
     saved = {k: sys.modules.get(k) for k in ("lietorch", "torch_scatter")}
     hooks = list(modules._HOOKS)
-    for k in saved:
-        sys.modules.pop(k, None)
     try:
         yield
     finally:
@@ -153,10 +151,7 @@ def test_a_spawned_child_registers_the_packages_before_unpickling_its_arguments(
     """DroidAsync starts backend_process(args, video1, video2) with spawn; unpickling the DepthVideo arguments imports depth_video, which
     imports lietorch at import time.  Here the argument is an object of lietorch_user (a module doing `import lietorch` at import time) and
     the child has no other lietorch on its path: it resolves to this package because the BackendProcess, pickled first, registers it"""
-    shims = os.path.join(ROOT, "oracle", "shims")
-    path = list(sys.path)
     with registered_state():
-        sys.path[:] = [p for p in sys.path if os.path.abspath(p) != shims]     # the child inherits sys.path: no stand-in lietorch in it
         try:
             droid_slam_b200.install_dependencies()
             import lietorch_user
@@ -164,16 +159,12 @@ def test_a_spawned_child_registers_the_packages_before_unpickling_its_arguments(
             code, out = _spawn(lietorch_user.backend_process, lietorch_user.Holder())
             assert code == 0 and out == ("droid_slam_b200.lietorch", "droid_slam_b200.lietorch", "droid_slam_b200.torch_scatter"), (code, out)
         finally:
-            sys.path[:] = path
             sys.modules.pop("lietorch_user", None)
 
 
 def test_torch_scatter_against_the_stand_in():
     """the known answers of tests/test_shims_cpu.py (thirdparty/pytorch_scatter/test/test_scatter.py:12-37), on both"""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("oracle_torch_scatter_shim", os.path.join(ROOT, "oracle", "shims", "torch_scatter", "__init__.py"))
-    shim = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(shim)
+    from oracle.shims import torch_scatter as shim
     src = torch.tensor([1., 3, 2, 4, 5, 6]); index = torch.tensor([0, 1, 0, 1, 1, 3])
     cases = [(src, index, -1, None, [3, 12, 0, 6], [1.5, 4, 0, 6])]
     src2 = torch.tensor([[1., 2], [5, 6], [3, 4], [7, 8], [9, 10], [11, 12]])

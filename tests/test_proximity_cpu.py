@@ -13,8 +13,9 @@ import oracle.proximity as prox
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import make_proximity_golden as mk  # noqa: E402
+import reference  # noqa: E402
 
-REF_PRESENT = os.path.isdir(os.path.join(mk.REF, "droid_slam"))
+REF_PRESENT = reference.present("droid_slam")
 
 
 @pytest.fixture(scope="module")

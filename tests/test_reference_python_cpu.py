@@ -15,8 +15,9 @@ import oracle
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 import make_reference_python_golden as mk  # noqa: E402
+import reference  # noqa: E402
 
-REF_PRESENT = os.path.isdir(os.path.join(mk.REF, "droid_slam"))
+REF_PRESENT = reference.present("droid_slam")
 
 
 @pytest.fixture(scope="module")
@@ -59,13 +60,9 @@ def test_reference_python_imports_unmodified_and_reproduces_the_fixture(gold, tm
 def test_reference_corr_module_imports_against_the_native_extension():
     """modules/corr.py needs only torch + droid_backends: with the native extension installed it imports unmodified and finds the
     four correlation ops it calls (the calls themselves need a GPU: tests/test_reference_python_gpu.py)"""
-    import importlib
     import droid_slam_b200
     be = droid_slam_b200.install()
-    sys.path.insert(0, os.path.join(mk.REF, "droid_slam"))
-    sys.modules.pop("modules.corr", None)
-    corr = importlib.import_module("modules.corr")
-    assert corr.droid_backends is be
-    for fn in ("corr_index_forward", "corr_index_backward", "altcorr_forward", "altcorr_backward"):
-        assert callable(getattr(corr.droid_backends, fn))
-    sys.modules.pop("modules.corr", None)
+    with reference.reference_modules("modules.corr", stubs={"droid_backends": be}) as (corr,):
+        assert corr.droid_backends is be
+        for fn in ("corr_index_forward", "corr_index_backward", "altcorr_forward", "altcorr_backward"):
+            assert callable(getattr(corr.droid_backends, fn))

@@ -1,17 +1,10 @@
 """The pure-PyTorch stand-ins for lietorch / torch_scatter (oracle/shims, test infrastructure) against the identities and known
 answers of the packages' own tests: thirdparty/lietorch/lietorch/run_tests.py:16-52, thirdparty/pytorch_scatter/test/test_scatter.py:12-60."""
-import os
-import sys
-
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
-import lietorch  # noqa: E402
-import torch_scatter  # noqa: E402
-from lietorch import SE3, SO3  # noqa: E402
-
-import oracle  # noqa: E402
+import oracle
+from oracle.shims import lietorch, torch_scatter
+from oracle.shims.lietorch import SE3, SO3
 
 
 def _g(seed=0):

@@ -9,9 +9,8 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
 
-import lietorch  # noqa: E402  (the stand-in under oracle/shims)
+from oracle.shims import lietorch  # noqa: E402
 from oracle import trajectory_filler as otf  # noqa: E402
 from droid_slam_b200 import c_api  # noqa: E402
 

@@ -10,10 +10,9 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import lietorch  # noqa: E402  (the stand-in: pure torch, runs the reference's SE3 arithmetic on CUDA tensors in fp32)
+from oracle.shims import lietorch  # noqa: E402  (pure torch: runs the reference's SE3 arithmetic on CUDA tensors in fp32)
 import droid_slam_b200  # noqa: E402
 import oracle  # noqa: E402
 import oracle.encoder as oenc  # noqa: E402

@@ -20,10 +20,9 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle", "shims"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-import lietorch  # noqa: E402  (the stand-in)
+from oracle.shims import lietorch  # noqa: E402
 import droid_slam_b200  # noqa: E402
 import oracle.encoder as oenc  # noqa: E402
 from oracle import trajectory_filler as otf  # noqa: E402
