@@ -46,7 +46,7 @@ def build_library(verbose=False):
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(OBJDIR, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    headers.append(os.path.join(INCLUDE, "droid_b200.h"))
+    headers += [os.path.join(INCLUDE, "droid_b200.h"), os.path.join(INCLUDE, "droid_b200_training.h")]
     jobs = []
     objs = []
     for src in CUDA_SOURCES:
@@ -69,7 +69,7 @@ def build_binding(verbose=False):
     import torch
     os.makedirs(EXTDIR, exist_ok=True)
     src = os.path.join(CSRC, "binding", "droid_backends.cpp")
-    if not _newer(EXT_PATH, [src, os.path.join(INCLUDE, "droid_b200.h"), LIB_PATH]):
+    if not _newer(EXT_PATH, [src, os.path.join(INCLUDE, "droid_b200.h"), os.path.join(INCLUDE, "droid_b200_training.h"), LIB_PATH]):
         return EXT_PATH
     tdir = os.path.dirname(torch.__file__)
     tinc = os.path.join(tdir, "include")

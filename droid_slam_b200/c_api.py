@@ -1,7 +1,9 @@
-"""ctypes view of the C ABI declared in include/droid_b200.h (used by the parity tests, the tools and bench.py's e2e leg).
+"""ctypes view of the C ABI declared in include/droid_b200.h and include/droid_b200_training.h (used by the parity tests, the tools and
+bench.py's e2e leg).
 
-Every function of the header has one prototype in PROTOTYPES, and every header struct that Python fills has one mirror here;
-tests/test_oracle_cpu.py checks both against the header.  Pointers are passed as c_void_p, except pointers to a mirrored struct."""
+Every function of droid_b200.h has one prototype in PROTOTYPES, and every header struct that Python fills has one mirror here;
+tests/test_oracle_cpu.py checks both against the header.  droid_b200_training.h's functions are in TRAINING_PROTOTYPES, checked by
+tests/test_flow_loss_cpu.py.  Pointers are passed as c_void_p, except pointers to a mirrored struct."""
 import ctypes
 import os
 
@@ -130,6 +132,14 @@ PROTOTYPES = {
 
 SYMBOLS = list(PROTOTYPES)
 
+# include/droid_b200_training.h (training's flow loss and upsample_disp's backward), in that header's order
+TRAINING_PROTOTYPES = {
+    "dba_flow_loss_workspace_bytes": (sz, [ci] * 5),
+    "dba_flow_loss_forward": (ci, [vp] * 5 + [ci, vp, vp] + [ci] * 4 + [ctypes.c_double, vp, sz, vp]),
+    "dba_flow_loss_backward": (ci, [vp] * 6 + [ci, vp, vp] + [ci] * 4 + [ctypes.c_double, vp, sz, vp]),
+    "dba_cvx_upsample_backward": (ci, [vp] * 6 + [ci] * 3 + [vp]),
+}
+
 
 def ba_args(poses, disps, intrinsics, disps_sens, targets, weights, eta, ii, jj, t0, t1, lm, ep, dx_out, dz_out, workspace, stream,
             motion_only=False, own=None, eta_by_frame=False):
@@ -164,7 +174,7 @@ def load():
     if not os.path.exists(p):
         raise ImportError("libdroid_b200.so not built; run `python -m droid_slam_b200.build`")
     L = ctypes.CDLL(p)
-    for name, (restype, argtypes) in PROTOTYPES.items():
+    for name, (restype, argtypes) in {**PROTOTYPES, **TRAINING_PROTOTYPES}.items():
         fn = getattr(L, name)
         fn.restype, fn.argtypes = restype, argtypes
     _LIB = L

@@ -18,6 +18,7 @@
 #include <cuda_runtime_api.h>
 #include <cstring>
 #include "../../../include/droid_b200.h"
+#include "../../../include/droid_b200_training.h"
 
 static inline void check_status(int rc, const char* op) {
   TORCH_CHECK(rc == DBA_OK, "droid_backends.", op, " failed (status ", rc, "): ", dba_last_error());
@@ -1026,6 +1027,97 @@ std::vector<torch::Tensor> ba_layer_backward(torch::Tensor grad_poses, torch::Te
   return {g_target, g_weight, g_eta, g_poses, g_disps};
 }
 
+// ---- training's tail: the flow loss and upsample_disp's backward (droid_slam_b200.modules.flow_loss / upsample_disp) ----------------
+
+// a device array of the tensors' data pointers, staged in pinned memory and copied on the current stream (no host synchronisation;
+// the caching host allocator keeps the staging buffer until the copy has run)
+static torch::Tensor device_pointers(const std::vector<torch::Tensor>& ts, const torch::Device& dev) {
+  auto host = torch::empty({(int64_t)ts.size()}, torch::TensorOptions().dtype(I64).pinned_memory(true));
+  int64_t* p = host.data_ptr<int64_t>();
+  for (size_t k = 0; k < ts.size(); k++) p[k] = (int64_t)(uintptr_t)ts[k].data_ptr();
+  return host.to(dev, /*non_blocking=*/true);
+}
+
+// The checks of one flow_loss_forward / flow_loss_backward call: every tensor fp32, contiguous, on one device; Ps [B,N,7], disps
+// [B,N,ht,wd], intrinsics [B,N,4], and every element of poses_est / disps_est (as many of each, at least one) [B,N,7] / [B,N,ht,wd];
+// N >= 2 (the chain graph has an edge), a non-empty batch and image.
+struct FlowArgs {
+  int B, N, ht, wd, n;
+};
+static FlowArgs flow_loss_args(const char* fn, const Expect& expect, const torch::Tensor& Ps, const torch::Tensor& disps,
+                               const std::vector<torch::Tensor>& poses_est, const std::vector<torch::Tensor>& disps_est,
+                               const torch::Tensor& intrinsics) {
+  expect(disps, "disps", {F32}, dims({kAny, kAny, kAny, kAny}));
+  const int64_t B = disps.size(0), N = disps.size(1), ht = disps.size(2), wd = disps.size(3);
+  expect(Ps, "Ps", {F32}, dims({B, N, 7}));
+  expect(intrinsics, "intrinsics", {F32}, dims({B, N, 4}));
+  TORCH_CHECK(!poses_est.empty() && poses_est.size() == disps_est.size(), "droid_backends.", fn, ": poses_est and disps_est must hold "
+              "the same number (at least one) of iterates, got ", poses_est.size(), " and ", disps_est.size());
+  for (size_t k = 0; k < poses_est.size(); k++) {
+    expect(poses_est[k], item("poses_est", k).c_str(), {F32}, dims({B, N, 7}));
+    expect(disps_est[k], item("disps_est", k).c_str(), {F32}, dims({B, N, ht, wd}));
+  }
+  TORCH_CHECK(B >= 1 && ht >= 1 && wd >= 1, "droid_backends.", fn, ": empty batch or image");
+  TORCH_CHECK(N >= 2, "droid_backends.", fn, ": N must be at least 2 (the chain graph of one frame has no edge), got ", N);
+  TORCH_CHECK(B <= 65535 && N <= 32768, "droid_backends.", fn, ": at most 65535 batch elements and 32768 frames, got ", B, " and ", N);
+  return {(int)B, (int)N, (int)ht, (int)wd, (int)poses_est.size()};
+}
+
+// -> [loss (0-dim f32), metrics (f64 [3]: sum of epe where v > 0.5, that count, the count with epe < 1, for the last iterate)]
+std::vector<torch::Tensor> flow_loss_forward(torch::Tensor Ps, torch::Tensor disps, std::vector<torch::Tensor> poses_est,
+                                             std::vector<torch::Tensor> disps_est, torch::Tensor intrinsics, double gamma) {
+  const Expect expect("flow_loss_forward", disps, "disps");
+  const FlowArgs a = flow_loss_args("flow_loss_forward", expect, Ps, disps, poses_est, disps_est, intrinsics);
+  c10::cuda::CUDAGuard guard(expect.dev);
+  torch::Tensor keep;
+  const size_t bytes = dba_flow_loss_workspace_bytes(a.B, a.N, a.ht, a.wd, a.n);
+  void* ws = workspace(bytes, expect.dev, keep);
+  auto pp = device_pointers(poses_est, expect.dev), dp = device_pointers(disps_est, expect.dev);
+  auto loss = torch::empty({}, disps.options()), metrics = torch::empty({3}, disps.options().dtype(torch::kFloat64));
+  check_status(dba_flow_loss_forward(Ps.data_ptr<float>(), disps.data_ptr<float>(), intrinsics.data_ptr<float>(),
+                                     (const float* const*)pp.data_ptr(), (const float* const*)dp.data_ptr(), a.n, loss.data_ptr<float>(),
+                                     metrics.data_ptr<double>(), a.B, a.N, a.ht, a.wd, gamma, ws, bytes, cur_stream()), "flow_loss_forward");
+  return {loss, metrics};
+}
+
+// -> [grad_poses_est[0..n), grad_disps_est[0..n)]; grad: the loss's upstream gradient (0-dim f32 on the device)
+std::vector<torch::Tensor> flow_loss_backward(torch::Tensor grad, torch::Tensor Ps, torch::Tensor disps, std::vector<torch::Tensor> poses_est,
+                                              std::vector<torch::Tensor> disps_est, torch::Tensor intrinsics, double gamma) {
+  const Expect expect("flow_loss_backward", disps, "disps");
+  const FlowArgs a = flow_loss_args("flow_loss_backward", expect, Ps, disps, poses_est, disps_est, intrinsics);
+  expect(grad, "grad", {F32}, Shape{Shape::kDims, c10::IntArrayRef()});
+  c10::cuda::CUDAGuard guard(expect.dev);
+  torch::Tensor keep;
+  const size_t bytes = dba_flow_loss_workspace_bytes(a.B, a.N, a.ht, a.wd, a.n);
+  void* ws = workspace(bytes, expect.dev, keep);
+  std::vector<torch::Tensor> gp, gd;
+  for (int k = 0; k < a.n; k++) { gp.push_back(torch::empty_like(poses_est[k])); gd.push_back(torch::empty_like(disps_est[k])); }
+  auto pp = device_pointers(poses_est, expect.dev), dp = device_pointers(disps_est, expect.dev);
+  auto gpp = device_pointers(gp, expect.dev), gdp = device_pointers(gd, expect.dev);
+  check_status(dba_flow_loss_backward(grad.data_ptr<float>(), Ps.data_ptr<float>(), disps.data_ptr<float>(), intrinsics.data_ptr<float>(),
+                                      (const float* const*)pp.data_ptr(), (const float* const*)dp.data_ptr(), a.n, (float* const*)gpp.data_ptr(),
+                                      (float* const*)gdp.data_ptr(), a.B, a.N, a.ht, a.wd, gamma, ws, bytes, cur_stream()), "flow_loss_backward");
+  gp.insert(gp.end(), gd.begin(), gd.end());
+  return gp;
+}
+
+// the backward of cvx_upsample for fp32 masks: disps [n,ht,wd], mask [n,576,ht,wd], grad_out [n,8ht,8wd] -> [grad_disps, grad_mask]
+std::vector<torch::Tensor> cvx_upsample_backward(torch::Tensor disps, torch::Tensor mask, torch::Tensor grad_out) {
+  const Expect expect("cvx_upsample_backward", disps, "disps");
+  expect(disps, "disps", {F32}, dims({kAny, kAny, kAny}));
+  const int64_t n = disps.size(0), ht = disps.size(1), wd = disps.size(2);
+  expect(mask, "mask", {F32}, dims({n, 576, ht, wd}));
+  expect(grad_out, "grad_out", {F32}, dims({n, 8 * ht, 8 * wd}));
+  c10::cuda::CUDAGuard guard(expect.dev);
+  auto g = ((uintptr_t)grad_out.data_ptr() & 15) ? grad_out.clone() : grad_out;     // the kernel reads 16-byte vectors
+  auto grad_disps = torch::empty_like(disps), grad_mask = torch::empty_like(mask);
+  auto taps = torch::empty({n, 9, 8, ht, wd}, disps.options());
+  check_status(dba_cvx_upsample_backward(disps.data_ptr<float>(), mask.data_ptr<float>(), g.data_ptr<float>(), grad_disps.data_ptr<float>(),
+                                         grad_mask.data_ptr<float>(), taps.data_ptr<float>(), (int)n, (int)ht, (int)wd, cur_stream()),
+               "cvx_upsample_backward");
+  return {grad_disps, grad_mask};
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
   // bundle adjustment kernels
@@ -1103,5 +1195,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("eta"), pybind11::arg("poses"), pybind11::arg("disps"), pybind11::arg("intrinsics"), pybind11::arg("ii"),
         pybind11::arg("jj"), pybind11::arg("fixedp"), pybind11::arg("ep"), pybind11::arg("lm"), pybind11::arg("factor"), pybind11::arg("dx"),
         pybind11::arg("dz"), pybind11::arg("flags"));
+  m.def("flow_loss_forward", &flow_loss_forward, "training's flow loss (reference geom/losses.py flow_loss) on the chain graph, every "
+        "iterate in one pass -> [loss, metrics (sum of epe where v > 0.5, that count, the count with epe < 1)], native extension",
+        pybind11::arg("Ps"), pybind11::arg("disps"), pybind11::arg("poses_est"), pybind11::arg("disps_est"), pybind11::arg("intrinsics"),
+        pybind11::arg("gamma") = 0.9);
+  m.def("flow_loss_backward", &flow_loss_backward, "gradients of flow_loss_forward -> [grad_poses_est..., grad_disps_est...], native extension",
+        pybind11::arg("grad"), pybind11::arg("Ps"), pybind11::arg("disps"), pybind11::arg("poses_est"), pybind11::arg("disps_est"),
+        pybind11::arg("intrinsics"), pybind11::arg("gamma") = 0.9);
+  m.def("cvx_upsample_backward", &cvx_upsample_backward, "gradients of cvx_upsample for fp32 masks -> [grad_disps, grad_mask], native extension",
+        pybind11::arg("disps"), pybind11::arg("mask"), pybind11::arg("grad_out"));
   m.def("_b200_native", []() { return true; });
 }

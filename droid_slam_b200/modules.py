@@ -39,11 +39,15 @@ kernel for is offered as a hook:
     forward and backward, on csrc/corr_train.cu, so `train.py`'s loss reaches fnet through native kernels.
   * `ba_layer(...)` / `install_ba_layer_hook(droid_net)`: DroidNet's differentiable dense BA (geom/ba.py:31-106, `droid_net.BA`) forward
     and backward on csrc/ba_layer.cu (`droid_backends.ba_layer_forward` / `ba_layer_backward`), so `train.py` trains through it.
+  * `flow_loss(...)` / `install_flow_loss_hook(losses)`: train.py's flow loss (geom/losses.py:89-118, `losses.flow_loss`) with every
+    iterate in one pass over the full-resolution pixels and its backward (`droid_backends.flow_loss_forward` / `flow_loss_backward`).
+  * `upsample_disp(...)` / `install_upsample_disp_hook(droid_net)`: DroidNet's disparity upsampling (droid_net.py:37-42,
+    `droid_net.upsample_disp`) on `droid_backends.cvx_upsample` with its backward (`cvx_upsample_backward`).
 
 The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
 it.  If not, strict=True (the default) raises RuntimeError naming the replaced method or global and the reason; strict=False runs the
 reference's own function -- the one the first install found, however often the hook is installed again.  `update`, `update_lowmem`,
-`fill_trajectory`, `track`, `ba_layer` and `CorrBlock` called directly raise in the same words.
+`fill_trajectory`, `track`, `ba_layer`, `CorrBlock`, `flow_loss` and `upsample_disp` called directly raise in the same words.
 """
 import copy
 import importlib
@@ -59,7 +63,7 @@ __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
            "install_trajectory_filler_hook", "track", "install_motion_filter_hook", "hook_registry", "reinstall_hooks",
            "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook", "ba_layer", "install_ba_layer_hook",
-           "install_corr_training_hook"]
+           "install_corr_training_hook", "flow_loss", "install_flow_loss_hook", "upsample_disp", "install_upsample_disp_hook"]
 
 
 def _require(entry, why):
@@ -1233,4 +1237,145 @@ def install_corr_training_hook(droid_net_module, strict=True):
     frontend, the factor graph and the motion filter use, is not touched."""
     _replace(droid_net_module, "CorrBlock", CorrBlock, _corr_training_unsupported, strict)
     _record("install_corr_training_hook", droid_net_module, strict=strict)
+    return droid_net_module
+
+
+# ---- training's tail under the reference's losses / droid_net: the flow loss and upsample_disp ----------------------------------------
+
+def _se3_data(P):
+    """P's [..., 7] data when P is an SE3, else None"""
+    data = getattr(P, "data", None) if type(P).__name__ == "SE3" else None
+    return data if torch.is_tensor(data) and data.shape[-1:] == (7,) else None
+
+
+def _f32_cuda(t):
+    return torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32
+
+
+def _flow_loss_unsupported(Ps, disps, poses_est, disps_est, intrinsics, graph=None, gamma=0.9):
+    """why the native flow loss cannot run this call, or None"""
+    if _se3_data(Ps) is None:
+        return "Ps must be an SE3 [B,N,7] (got %s)" % type(Ps).__name__
+    if len(poses_est) == 0 or len(poses_est) != len(disps_est):
+        return "%d pose and %d disparity iterates (the same number, at least one, has a kernel)" % (len(poses_est), len(disps_est))
+    for k, P in enumerate(poses_est):
+        if _se3_data(P) is None:
+            return "poses_est[%d] must be an SE3 [B,N,7] (got %s)" % (k, type(P).__name__)
+    named = [("Ps", Ps.data), ("disps", disps), ("intrinsics", intrinsics)]
+    named += [("poses_est[%d]" % k, P.data) for k, P in enumerate(poses_est)] + [("disps_est[%d]" % k, d) for k, d in enumerate(disps_est)]
+    for name, t in named:
+        if not _f32_cuda(t):
+            return "%s must be a CUDA float32 tensor" % name
+    if disps.dim() != 4:
+        return "disps must be [B,N,ht,wd] (got shape %s)" % (tuple(disps.shape),)
+    B, N, ht, wd = disps.shape
+    for name, t in named:
+        want = (B, N, 7) if name.startswith(("Ps", "poses_est")) else (B, N, 4) if name == "intrinsics" else (B, N, ht, wd)
+        if tuple(t.shape) != want:
+            return "%s has shape %s, not %s" % (name, tuple(t.shape), want)
+    if N < 2:
+        return "N = %d (the chain graph needs 2 frames)" % N
+    if B * ht * wd == 0:
+        return "an empty batch or image"
+    for name, t in (("Ps", Ps.data), ("disps", disps), ("intrinsics", intrinsics)):
+        if t.requires_grad:
+            return "%s requires grad (the native loss gives it none)" % name
+    return None
+
+
+class _FlowLoss(torch.autograd.Function):
+    """geom/losses.py flow_loss on droid_backends.flow_loss_forward / flow_loss_backward over the 2n iterate tensors (poses' data,
+    then disparities).  Nothing but the inputs is kept: the backward recomputes every per-pixel term."""
+
+    @staticmethod
+    def forward(ctx, Ps, disps, intrinsics, gamma, *est):
+        n = len(est) // 2
+        loss, metrics = install().flow_loss_forward(Ps, disps, list(est[:n]), list(est[n:]), intrinsics, gamma)
+        ctx.gamma = gamma
+        ctx.save_for_backward(Ps, disps, intrinsics, *est)
+        ctx.mark_non_differentiable(metrics)
+        return loss, metrics
+
+    @staticmethod
+    def backward(ctx, grad_loss, _):
+        Ps, disps, intrinsics, *est = ctx.saved_tensors
+        n = len(est) // 2
+        g = install().flow_loss_backward(grad_loss.reshape(()).float().contiguous(), Ps, disps, est[:n], est[n:], intrinsics, ctx.gamma)
+        return (None, None, None, None, *g)
+
+
+def flow_loss(Ps, disps, poses_est, disps_est, intrinsics, graph=None, gamma=0.9):
+    """flow_loss(Ps, disps, poses_est, disps_est, intrinsics, graph, gamma=0.9) of geom/losses.py:89-118 -> (loss, metrics): every
+    iterate in one pass over the full-resolution pixels of the chain graph (graph is ignored, as the reference ignores it), nothing
+    materialised per pixel; differentiable in every poses_est[i] (lietorch's convention) and disps_est[i].  metrics is the reference's
+    dict of Python floats ('f_error', '1px': NaN when no pixel is valid, as the mean of an empty tensor) from one host read."""
+    _require("flow_loss", _flow_loss_unsupported(Ps, disps, poses_est, disps_est, intrinsics, graph, gamma))
+    args = (Ps.data.contiguous(), disps.contiguous(), intrinsics.contiguous())
+    est = [P.data.contiguous() for P in poses_est] + [d.contiguous() for d in disps_est]
+    if torch.is_grad_enabled() and any(t.requires_grad for t in est):
+        loss, metrics = _FlowLoss.apply(*args, float(gamma), *est)
+    else:
+        n = len(poses_est)
+        loss, metrics = install().flow_loss_forward(*args[:2], est[:n], est[n:], args[2], float(gamma))
+    s, count, below = metrics.tolist()
+    nan = float("nan")
+    return loss, {"f_error": s / count if count else nan, "1px": below / count if count else nan}
+
+
+def install_flow_loss_hook(losses_module, strict=True):
+    """losses_module = the imported reference module `geom.losses`.  Sets its global `flow_loss` (losses.py:89, which train.py calls
+    through the module) to the native loss (`flow_loss`), forward and backward.  A call it cannot run (Ps or a poses_est[i] not an SE3
+    [B,N,7], a tensor not CUDA float32, shapes that disagree, N < 2, no iterates, Ps / disps / intrinsics requiring grad) raises under
+    strict=True and runs the reference's flow_loss under strict=False.  projective_transform itself is not touched."""
+    _replace(losses_module, "flow_loss", flow_loss, _flow_loss_unsupported, strict)
+    _record("install_flow_loss_hook", losses_module, strict=strict)
+    return losses_module
+
+
+def _upsample_disp_unsupported(disp, mask):
+    """why the native upsample_disp cannot run this call, or None"""
+    if not (_f32_cuda(disp) and disp.dim() == 4):
+        return "disp must be a CUDA float32 [B,N,ht,wd] tensor"
+    B, N, ht, wd = disp.shape
+    if not (_f32_cuda(mask) and tuple(mask.shape) == (B, N, 576, ht, wd)):
+        return "mask must be a CUDA float32 [B,N,576,ht,wd] = %s tensor (got %s %s)" % (
+            (B, N, 576, ht, wd), getattr(mask, "dtype", type(mask).__name__), tuple(getattr(mask, "shape", ())))
+    return None
+
+
+class _UpsampleDisp(torch.autograd.Function):
+    """droid_net.py upsample_disp on droid_backends.cvx_upsample and cvx_upsample_backward; disp [n,ht,wd], mask [n,576,ht,wd]"""
+
+    @staticmethod
+    def forward(ctx, disp, mask):
+        ctx.save_for_backward(disp, mask)
+        return install().cvx_upsample(disp, mask)
+
+    @staticmethod
+    def backward(ctx, grad):
+        disp, mask = ctx.saved_tensors
+        return tuple(install().cvx_upsample_backward(disp, mask, grad.contiguous()))
+
+
+def upsample_disp(disp, mask):
+    """upsample_disp(disp, mask) of droid_net.py:37-42 for fp32 CUDA inputs: disp [B,N,ht,wd], mask [B,N,576,ht,wd] -> [B,N,8ht,8wd],
+    the forward droid_backends.cvx_upsample's, differentiable in both (the softmax recomputed from the mask, nothing else kept)"""
+    _require("upsample_disp", _upsample_disp_unsupported(disp, mask))
+    B, N, ht, wd = disp.shape
+    d = disp.reshape(B * N, ht, wd).contiguous()
+    m = mask.reshape(B * N, 576, ht, wd).contiguous()
+    if torch.is_grad_enabled() and (d.requires_grad or m.requires_grad):
+        out = _UpsampleDisp.apply(d, m)
+    else:
+        out = install().cvx_upsample(d, m)
+    return out.view(B, N, 8 * ht, 8 * wd)
+
+
+def install_upsample_disp_hook(droid_net_module, strict=True):
+    """droid_net_module = the imported reference module `droid_net`.  Sets its global `upsample_disp` (droid_net.py:37, called once per
+    update iteration by DroidNet.forward) to the native one (`upsample_disp`), forward and backward.  A call with a disp that is not a
+    CUDA float32 [B,N,ht,wd] or a mask that is not a CUDA float32 [B,N,576,ht,wd] raises under strict=True and runs the reference's
+    upsample_disp under strict=False."""
+    _replace(droid_net_module, "upsample_disp", upsample_disp, _upsample_disp_unsupported, strict)
+    _record("install_upsample_disp_hook", droid_net_module, strict=strict)
     return droid_net_module
