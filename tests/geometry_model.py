@@ -1,7 +1,7 @@
 """First-order running error bounds for the geometry kernels (csrc/geom.cu) and cvx_upsample, in each kernel's own operation order.
 
 A value the kernel computes in fp32 is carried as R(v, b): v its fp64 restatement, b a bound on |fp32 result - v|.  Every fp32 rounding
-is charged u |result| (u = 2^-24), except where the operands are exact (b = 0) and the fp64 result is an fp32 number: then the fp32
+is charged u |result| (u = 2^-24), plus 2^-150 below the normal range where the spacing stops shrinking, except where the operands are exact (b = 0) and the fp64 result is an fp32 number: then the fp32
 operation returns it exactly, contracted into an FMA or not.  An FMA rounds once and is covered by the two charges of its product and
 sum.  Sums, products and quotients propagate the operands' bounds in the usual way (second-order terms of products included; a
 quotient whose divisor's bound reaches the divisor has no bound).  The fp64 value v itself is the kernel's expression evaluated in fp64,
@@ -9,6 +9,7 @@ in the same order as oracle/geom.py, which the CPU test checks.
 
 Decisions (a comparison of a bounded value with a constant) are `sure` where the fp64 margin exceeds the bound: the kernel must then
 decide as fp64 does.  Inside the window either answer is allowed."""
+import contextlib
 import math
 
 import torch
@@ -28,9 +29,19 @@ def _exact(z):
     return torch.isfinite(z) & (z.float().double() == z)
 
 
+def _charge(z, b):
+    """one fp32 rounding of z (bound b before it): u |z|, and half the smallest subnormal (2^-150) below the normal range, where the
+    spacing is fixed; nothing for an exact 0 (a product with an exact 0 operand)"""
+    tiny = (z.abs() < 2.0 ** -126) & ((z != 0) | (b > 0))
+    return U * z.abs() + torch.where(tiny, torch.full_like(z, 2.0 ** -150), torch.zeros_like(z))
+
+
 class R:
-    """fp64 value and first-order bound of an fp32 kernel value"""
+    """fp64 value and first-order bound of an fp32 kernel value.  Inside `with R.double():` each operation is the kernel's fp64
+    arithmetic instead: it propagates the operands' bounds and charges 2^-53 |result| for its own rounding, exact operands or not
+    (an fp64 FMA may round where the host does not)."""
     __slots__ = ("v", "b")
+    u = U
 
     def __init__(self, v, b=None):
         self.v = torch.as_tensor(v, dtype=torch.float64)
@@ -40,9 +51,24 @@ class R:
     def lift(x):
         return x if isinstance(x, R) else R(x)
 
+    @staticmethod
+    @contextlib.contextmanager
+    def double():
+        R.u = 2.0 ** -53
+        try:
+            yield
+        finally:
+            R.u = U
+
+    def f32(self):
+        """the kernel's (float) of an fp64 value"""
+        return R(self.v, self.b + torch.where(_exact(self.v), torch.zeros_like(self.v), _charge(self.v, self.b)))
+
     def _rounded(self, z, b, x, y):
+        if R.u != U:
+            return R(z, b + R.u * z.abs())
         exact = (x.b == 0) & (y.b == 0) & _exact(z)
-        return R(z, b + torch.where(exact, torch.zeros_like(z), U * z.abs()))
+        return R(z, b + torch.where(exact, torch.zeros_like(z), _charge(z, b)))
 
     def __add__(self, y):
         y = R.lift(y)
