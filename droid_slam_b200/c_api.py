@@ -132,12 +132,15 @@ PROTOTYPES = {
 
 SYMBOLS = list(PROTOTYPES)
 
-# include/droid_b200_training.h (training's flow loss and upsample_disp's backward), in that header's order
+# include/droid_b200_training.h (training's flow loss, upsample_disp's backward and the ConvGRU), in that header's order
 TRAINING_PROTOTYPES = {
     "dba_flow_loss_workspace_bytes": (sz, [ci] * 5),
     "dba_flow_loss_forward": (ci, [vp] * 5 + [ci, vp, vp] + [ci] * 4 + [ctypes.c_double, vp, sz, vp]),
     "dba_flow_loss_backward": (ci, [vp] * 6 + [ci, vp, vp] + [ci] * 4 + [ctypes.c_double, vp, sz, vp]),
     "dba_cvx_upsample_backward": (ci, [vp] * 6 + [ci] * 3 + [vp]),
+    "dba_conv_gru_workspace_bytes": (sz, [ci] * 4),
+    "dba_conv_gru_forward": (ci, [vp] * 9 + [ci] * 3 + [vp, sz, vp]),
+    "dba_conv_gru_backward": (ci, [vp] * 14 + [ci] * 3 + [vp, sz, vp]),
 }
 
 

@@ -1118,6 +1118,85 @@ std::vector<torch::Tensor> cvx_upsample_backward(torch::Tensor disps, torch::Ten
   return {grad_disps, grad_mask};
 }
 
+// ---- the update operator's ConvGRU for training (droid_slam_b200.modules.conv_gru) ---------------------------------------------------
+
+// the shapes of ConvGRU(128, 320)'s 14 parameters in the module's order (include/droid_b200_training.h)
+static const std::vector<int64_t> kConvGruParamShapes[14] = {
+    {128, 448, 3, 3}, {128}, {128, 448, 3, 3}, {128}, {128, 448, 3, 3}, {128}, {128, 128, 1, 1}, {128},
+    {128, 128, 1, 1}, {128}, {128, 128, 1, 1}, {128}, {128, 128, 1, 1}, {128}};
+static const char* const kConvGruParamNames[14] = {
+    "convz.weight", "convz.bias", "convr.weight", "convr.bias", "convq.weight", "convq.bias", "w.weight", "w.bias",
+    "convz_glo.weight", "convz_glo.bias", "convr_glo.weight", "convr_glo.bias", "convq_glo.weight", "convq_glo.bias"};
+
+// The checks of one conv_gru_forward / conv_gru_backward call: every tensor fp32, contiguous, on net's device; net, inp, corr
+// [b,128,ht,wd], flow [b,64,ht,wd], b, ht, wd >= 1; the 14 parameters in their shapes.  -> (b, ht, wd) and the parameter pointers
+struct GruArgs {
+  int b, ht, wd;
+  std::vector<const float*> params;
+};
+static GruArgs conv_gru_args(const char* fn, const Expect& expect, const torch::Tensor& net, const torch::Tensor& inp,
+                             const torch::Tensor& corr, const torch::Tensor& flow, const std::vector<torch::Tensor>& params) {
+  expect(net, "net", {F32}, dims({kAny, 128, kAny, kAny}));
+  const int64_t b = net.size(0), ht = net.size(2), wd = net.size(3);
+  expect(inp, "inp", {F32}, dims({b, 128, ht, wd}));
+  expect(corr, "corr", {F32}, dims({b, 128, ht, wd}));
+  expect(flow, "flow", {F32}, dims({b, 64, ht, wd}));
+  TORCH_CHECK(b >= 1 && ht >= 1 && wd >= 1, "droid_backends.", fn, ": empty batch or image");
+  TORCH_CHECK(b <= 65535 && b * 448 * ht * wd <= INT32_MAX, "droid_backends.", fn, ": at most 65535 edges and b * 448 * ht * wd < 2^31, got ",
+              b, " edges of ", ht, "x", wd);
+  TORCH_CHECK(params.size() == 14, "droid_backends.", fn, ": params must hold ConvGRU's 14 parameters, got ", params.size());
+  GruArgs a{(int)b, (int)ht, (int)wd, {}};
+  for (size_t k = 0; k < 14; k++) {
+    expect(params[k], (item("params", k) + " (" + kConvGruParamNames[k] + ")").c_str(), {F32}, dims(kConvGruParamShapes[k]));
+    a.params.push_back(params[k].data_ptr<float>());
+  }
+  return a;
+}
+
+// -> [out [b,128,ht,wd], zr [b,256,ht,wd], q [b,128,ht,wd], glo [b,128]]: the output and what conv_gru_backward reads
+std::vector<torch::Tensor> conv_gru_forward(torch::Tensor net, torch::Tensor inp, torch::Tensor corr, torch::Tensor flow,
+                                            std::vector<torch::Tensor> params) {
+  const Expect expect("conv_gru_forward", net, "net");
+  const GruArgs a = conv_gru_args("conv_gru_forward", expect, net, inp, corr, flow, params);
+  c10::cuda::CUDAGuard guard(expect.dev);
+  auto out = torch::empty_like(net), zr = torch::empty({a.b, 256, a.ht, a.wd}, net.options()), q = torch::empty_like(net);
+  auto glo = torch::empty({a.b, 128}, net.options());
+  torch::Tensor keep;
+  const size_t bytes = dba_conv_gru_workspace_bytes(a.b, a.ht, a.wd, 0);
+  void* ws = workspace(bytes, expect.dev, keep);
+  check_status(dba_conv_gru_forward(net.data_ptr<float>(), inp.data_ptr<float>(), corr.data_ptr<float>(), flow.data_ptr<float>(),
+                                    a.params.data(), out.data_ptr<float>(), zr.data_ptr<float>(), q.data_ptr<float>(), glo.data_ptr<float>(),
+                                    a.b, a.ht, a.wd, ws, bytes, cur_stream()), "conv_gru_forward");
+  return {out, zr, q, glo};
+}
+
+// -> [grad_net, grad_inp, grad_corr, grad_flow, grad_params[0..14)] from the upstream gradient grad [b,128,ht,wd] and the forward's
+// zr, q, glo
+std::vector<torch::Tensor> conv_gru_backward(torch::Tensor grad, torch::Tensor net, torch::Tensor inp, torch::Tensor corr, torch::Tensor flow,
+                                             std::vector<torch::Tensor> params, torch::Tensor zr, torch::Tensor q, torch::Tensor glo) {
+  const Expect expect("conv_gru_backward", net, "net");
+  const GruArgs a = conv_gru_args("conv_gru_backward", expect, net, inp, corr, flow, params);
+  expect(grad, "grad", {F32}, dims({a.b, 128, a.ht, a.wd}));
+  expect(zr, "zr", {F32}, dims({a.b, 256, a.ht, a.wd}));
+  expect(q, "q", {F32}, dims({a.b, 128, a.ht, a.wd}));
+  expect(glo, "glo", {F32}, dims({a.b, 128}));
+  c10::cuda::CUDAGuard guard(expect.dev);
+  std::vector<torch::Tensor> g = {torch::empty_like(net), torch::empty_like(inp), torch::empty_like(corr), torch::empty_like(flow)};
+  std::vector<float*> gp;
+  for (size_t k = 0; k < 14; k++) {
+    g.push_back(torch::empty_like(params[k]));
+    gp.push_back(g.back().data_ptr<float>());
+  }
+  torch::Tensor keep;
+  const size_t bytes = dba_conv_gru_workspace_bytes(a.b, a.ht, a.wd, 1);
+  void* ws = workspace(bytes, expect.dev, keep);
+  check_status(dba_conv_gru_backward(grad.data_ptr<float>(), net.data_ptr<float>(), inp.data_ptr<float>(), corr.data_ptr<float>(),
+                                     flow.data_ptr<float>(), a.params.data(), zr.data_ptr<float>(), q.data_ptr<float>(), glo.data_ptr<float>(),
+                                     g[0].data_ptr<float>(), g[1].data_ptr<float>(), g[2].data_ptr<float>(), g[3].data_ptr<float>(), gp.data(),
+                                     a.b, a.ht, a.wd, ws, bytes, cur_stream()), "conv_gru_backward");
+  return g;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100-native droid_backends (drop-in for princeton-vl/DROID-SLAM src/droid.cpp)";
   // bundle adjustment kernels
@@ -1204,5 +1283,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("intrinsics"), pybind11::arg("gamma") = 0.9);
   m.def("cvx_upsample_backward", &cvx_upsample_backward, "gradients of cvx_upsample for fp32 masks -> [grad_disps, grad_mask], native extension",
         pybind11::arg("disps"), pybind11::arg("mask"), pybind11::arg("grad_out"));
+  m.def("conv_gru_forward", &conv_gru_forward, "the update operator's ConvGRU(128, 320) (reference modules/gru.py), fp32 forward -> [out, "
+        "zr, q, glo], native extension", pybind11::arg("net"), pybind11::arg("inp"), pybind11::arg("corr"), pybind11::arg("flow"),
+        pybind11::arg("params"));
+  m.def("conv_gru_backward", &conv_gru_backward, "gradients of conv_gru_forward -> [grad_net, grad_inp, grad_corr, grad_flow, grad_params...], "
+        "native extension", pybind11::arg("grad"), pybind11::arg("net"), pybind11::arg("inp"), pybind11::arg("corr"), pybind11::arg("flow"),
+        pybind11::arg("params"), pybind11::arg("zr"), pybind11::arg("q"), pybind11::arg("glo"));
   m.def("_b200_native", []() { return true; });
 }

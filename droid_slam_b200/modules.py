@@ -43,11 +43,14 @@ kernel for is offered as a hook:
     iterate in one pass over the full-resolution pixels and its backward (`droid_backends.flow_loss_forward` / `flow_loss_backward`).
   * `upsample_disp(...)` / `install_upsample_disp_hook(droid_net)`: DroidNet's disparity upsampling (droid_net.py:37-42,
     `droid_net.upsample_disp`) on `droid_backends.cvx_upsample` with its backward (`cvx_upsample_backward`).
+  * `conv_gru(module, net, *inputs)` / `install_conv_gru_hook(gru)`: the update operator's ConvGRU (modules/gru.py:19-32,
+    `ConvGRU.forward`) forward and backward on csrc/gru_train.cu (`droid_backends.conv_gru_forward` / `conv_gru_backward`).
 
 The strict policy, one for every hook with a `strict` flag (`_replace`): each call first asks, once, whether the native path can run
 it.  If not, strict=True (the default) raises RuntimeError naming the replaced method or global and the reason; strict=False runs the
 reference's own function -- the one the first install found, however often the hook is installed again.  `update`, `update_lowmem`,
-`fill_trajectory`, `track`, `ba_layer`, `CorrBlock`, `flow_loss` and `upsample_disp` called directly raise in the same words.
+`fill_trajectory`, `track`, `ba_layer`, `CorrBlock`, `flow_loss`, `upsample_disp` and `conv_gru` called directly raise in the same
+words.
 """
 import copy
 import importlib
@@ -63,7 +66,8 @@ __all__ = ["install_corr_volume_hook", "install_alt_corr_hook", "install_encoder
            "install_depth_video_hook", "update", "update_lowmem", "install_factor_graph_hook", "plan_lowmem_chunks", "fill_trajectory",
            "install_trajectory_filler_hook", "track", "install_motion_filter_hook", "hook_registry", "reinstall_hooks",
            "install_update_module_hook", "handover_round", "BackendProcess", "install_async_hook", "ba_layer", "install_ba_layer_hook",
-           "install_corr_training_hook", "flow_loss", "install_flow_loss_hook", "upsample_disp", "install_upsample_disp_hook"]
+           "install_corr_training_hook", "flow_loss", "install_flow_loss_hook", "upsample_disp", "install_upsample_disp_hook", "conv_gru",
+           "install_conv_gru_hook"]
 
 
 def _require(entry, why):
@@ -1379,3 +1383,88 @@ def install_upsample_disp_hook(droid_net_module, strict=True):
     _replace(droid_net_module, "upsample_disp", upsample_disp, _upsample_disp_unsupported, strict)
     _record("install_upsample_disp_hook", droid_net_module, strict=strict)
     return droid_net_module
+
+
+# ---- the update operator's ConvGRU under modules.gru -------------------------------------------------------------------------------
+
+# ConvGRU(128, 128+128+64) as UpdateModule builds it: the parameters' names, in the order droid_backends.conv_gru_* take them
+CONV_GRU_PARAMS = ("convz.weight", "convz.bias", "convr.weight", "convr.bias", "convq.weight", "convq.bias", "w.weight", "w.bias",
+                   "convz_glo.weight", "convz_glo.bias", "convr_glo.weight", "convr_glo.bias", "convq_glo.weight", "convq_glo.bias")
+
+
+def _conv_gru_params(module):
+    return [module.get_parameter(name) for name in CONV_GRU_PARAMS]
+
+
+def _conv_gru_unsupported(module, net, *inputs):
+    """why the native ConvGRU cannot run this call (None: it can)"""
+    convs = [getattr(module, name.split(".")[0], None) for name in CONV_GRU_PARAMS[::2]]
+    want = [(128, 448, 3)] * 3 + [(128, 128, 1)] * 4
+    got = [(c.out_channels, c.in_channels, c.kernel_size[0]) if isinstance(c, torch.nn.Conv2d) else None for c in convs]
+    if got != want or any(c.bias is None for c in convs):
+        return "the module is not ConvGRU(128, 320): (out, in, kernel) of its convolutions are %s, not %s" % (got, want)
+    tensors = [("net", net)] + [("inputs[%d]" % k, t) for k, t in enumerate(inputs)]
+    if not all(torch.is_tensor(t) for _, t in tensors):
+        return "net and the inputs must be tensors"
+    channels = tuple(t.shape[1] if t.dim() == 4 else None for _, t in tensors)
+    if channels != (128, 128, 128, 64):
+        return "net and inputs must be 4-d with 128 / (128, 128, 64) channels, got %s" % (channels,)
+    shapes = {(t.shape[0],) + tuple(t.shape[2:]) for _, t in tensors}
+    if len(shapes) > 1:
+        return "net and the inputs disagree in (b, h, w): %s" % sorted(shapes)
+    b, h, w = shapes.pop()
+    if b * h * w == 0:
+        return "an empty batch or image"
+    if b > 65535 or b * 448 * h * w >= 2 ** 31:
+        return "%d edges of %dx%d (at most 65535 edges and b * 448 * h * w < 2^31)" % (b, h, w)
+    named = tensors + list(zip(CONV_GRU_PARAMS, _conv_gru_params(module)))
+    for name, t in named:
+        if not _f32_cuda(t):
+            return "%s must be a CUDA float32 tensor (got %s on %s)" % (name, t.dtype, t.device)
+    devs = {t.device for _, t in named}
+    if len(devs) > 1:
+        return "the tensors and parameters are on %d devices (%s), not one" % (len(devs), ", ".join(sorted(map(str, devs))))
+    if torch.is_autocast_enabled("cuda"):
+        return "CUDA autocast is enabled (the reference would run float16 convolutions)"
+    return None
+
+
+class _ConvGRU(torch.autograd.Function):
+    """modules/gru.py ConvGRU.forward on droid_backends.conv_gru_forward / conv_gru_backward.  The parameters are inputs, so autograd
+    accumulates their .grad.  The forward keeps z, r, q (384 channels) and glo beyond the inputs and parameters."""
+
+    @staticmethod
+    def forward(ctx, net, inp, corr, flow, *params):
+        out, zr, q, glo = install().conv_gru_forward(net, inp, corr, flow, list(params))
+        ctx.save_for_backward(net, inp, corr, flow, zr, q, glo, *params)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        net, inp, corr, flow, zr, q, glo, *params = ctx.saved_tensors
+        return tuple(install().conv_gru_backward(grad.contiguous(), net, inp, corr, flow, params, zr, q, glo))
+
+
+def conv_gru(module, net, *inputs):
+    """ConvGRU.forward(net, *inputs) of modules/gru.py:19-32 for `module` = ConvGRU(128, 128+128+64) and fp32 CUDA tensors net
+    [b,128,h,w], inputs (inp, corr, flow) [b,128|128|64,h,w] -> the new net [b,128,h,w], differentiable in net, the inputs and the
+    module's 14 parameters (3xTF32 on the tensor cores, fixed-order sums: two runs give the same bits).  Non-contiguous tensors are
+    copied.  Under no_grad, or with nothing requiring grad, nothing is kept.  No host synchronisation."""
+    _require("ConvGRU.forward", _conv_gru_unsupported(module, net, *inputs))
+    args = [t.contiguous() for t in (net,) + tuple(inputs)]
+    params = _conv_gru_params(module)
+    if torch.is_grad_enabled() and any(t.requires_grad for t in args + params):
+        return _ConvGRU.apply(*args, *params)
+    return install().conv_gru_forward(*args, [p.detach() for p in params])[0]
+
+
+def install_conv_gru_hook(gru_module, strict=True):
+    """gru_module = the imported reference module `modules.gru`.  Replaces `ConvGRU.forward` in place on the class (UpdateModule runs it
+    once per update iteration, droid_net.py:127) by `conv_gru`, forward and backward.  A call it cannot run (not ConvGRU(128, 320), a
+    tensor or parameter not CUDA float32 on one device, CUDA autocast enabled, other channel counts, mismatched b / h / w) raises under
+    strict=True and runs the reference's forward under strict=False.  The inference operator's install_update_module_hook replaces the
+    whole UpdateModule, so a network built under it never calls ConvGRU.forward."""
+    _replace(gru_module.ConvGRU, "forward", conv_gru, _conv_gru_unsupported, strict)
+    _record("install_conv_gru_hook", gru_module, strict=strict)
+    return gru_module

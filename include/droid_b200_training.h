@@ -1,6 +1,7 @@
-/* droid_b200_training.h -- the C ABI of training's tail: DroidNet's flow loss and the backward of its disparity upsampling.
- * Declared apart from droid_b200.h, whose function set (57 entry points) the project's ABI checks pin; c_api.TRAINING_PROTOTYPES
- * mirrors this file and tests/test_flow_loss_cpu.py checks the two against each other. */
+/* droid_b200_training.h -- the C ABI of DroidNet's training passes beyond droid_b200.h: the flow loss, the backward of the disparity
+ * upsampling, and the update operator's ConvGRU forward and backward.  Declared apart from droid_b200.h, whose function set (57 entry
+ * points) the project's ABI checks pin; c_api.TRAINING_PROTOTYPES mirrors this file and tests/test_flow_loss_cpu.py checks the two
+ * against each other. */
 #ifndef DROID_B200_TRAINING_H
 #define DROID_B200_TRAINING_H
 #include "droid_b200.h"
@@ -30,6 +31,24 @@ int dba_flow_loss_backward(const float* grad_loss, const float* Ps, const float*
  * (per-tap sums, gathered in a fixed order: no atomics). */
 int dba_cvx_upsample_backward(const float* disps, const float* mask, const float* grad_out, float* grad_disps, float* grad_mask,
                               float* tap_partials, int n, int ht, int wd, dba_stream_t stream);
+
+/* ---- ConvGRU(128, 128+128+64) of the update operator (reference modules/gru.py:19-32), forward and backward ---------------------------
+ * fp32, contiguous NCHW: net [b,128,ht,wd], inp [b,128,ht,wd], corr [b,128,ht,wd], flow [b,64,ht,wd]; b, ht, wd >= 1, b <= 65535 and
+ * b * 448 * ht * wd < 2^31.  params: a host array of 14 device pointers to the module's parameters in their own layout and order --
+ * convz, convr, convq ([128,448,3,3], [128]), w, convz_glo, convr_glo, convq_glo ([128,128,1,1], [128]), weight then bias each.
+ * dba_conv_gru_forward writes out [b,128,ht,wd] and what the backward reads: zr [b,256,ht,wd] (z, then r), q [b,128,ht,wd] and
+ * glo [b,128].  dba_conv_gru_backward reads the upstream gradient grad_out [b,128,ht,wd] and writes the gradients of net and of the
+ * three inputs (their shapes) and, through grad_params (a host array of 14 device pointers, the params' order and shapes), of every
+ * parameter.  Every product is 3xTF32 on the tensor cores with fp32 accumulation; sums over pixels are partials added in a fixed
+ * order (no atomics: two runs give the same bits).  workspace: dba_conv_gru_workspace_bytes(b, ht, wd, 0) bytes for the forward,
+ * (.., 1) for the backward, 256-byte aligned.  Neither synchronises the host. */
+size_t dba_conv_gru_workspace_bytes(int b, int ht, int wd, int backward);
+int dba_conv_gru_forward(const float* net, const float* inp, const float* corr, const float* flow, const float* const* params, float* out,
+                         float* zr, float* q, float* glo, int b, int ht, int wd, void* workspace, size_t workspace_bytes, dba_stream_t stream);
+int dba_conv_gru_backward(const float* grad_out, const float* net, const float* inp, const float* corr, const float* flow,
+                          const float* const* params, const float* zr, const float* q, const float* glo, float* grad_net, float* grad_inp,
+                          float* grad_corr, float* grad_flow, float* const* grad_params, int b, int ht, int wd, void* workspace,
+                          size_t workspace_bytes, dba_stream_t stream);
 
 #ifdef __cplusplus
 }
